@@ -4,6 +4,7 @@
     python bench.py --gpus N --steps K --warmup W                 # config 2 (default): the BASELINE metric, our arm
     python bench.py --config {2,3,4,5} ...                         # 3: YOLO-NAS-M train, 4: ResNet-50 train, 5: POSE-L predict()
     python bench.py --impl reference [--config C] --gpus N ...     # the reference's CPU path (oracle port) on the host cores
+    python bench.py ... --dump-outputs DIR                         # also write what the last timed step computed, DIR/<name>.npy
 
   config 2  YOLO-NAS-S  640x640 train step, 32 images / GPU (fwd + PPYoloELoss/TAL + bwd + AdamW + EMA)      [BASELINE metric]
   config 3  YOLO-NAS-M  640x640 train step, 16 images / GPU (same step; the weak-scaling sweep config)
@@ -38,9 +39,8 @@ CONFIGS = {
 # kept for tools/ that import them
 METRIC, WORKLOAD, IMG, BATCH = CONFIGS[2]["metric"], CONFIGS[2]["workload"], 640, 32
 TRAIN_GFLOP_PER_IMG = CONFIGS[2]["gflop"]
-# dram__bytes_read.sum + dram__bytes_write.sum of the conv family over ONE step from a committed ncu launch list of this command
-# (None: not captured for that configuration); the JSON line names the file
-NCU_CONV_DRAM = {(2, 32): (17.99e9, "profiles/r2_launches_graph_step.txt")}
+# Upper bound on what --dump-outputs writes in all; larger outputs are written as a fixed, seeded sample
+DUMP_MAX_BYTES = 64 << 20
 
 
 def synth_batch(batch, seed, img=640):
@@ -81,7 +81,7 @@ def synth_images_u8(batch, seed, img=640):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md).
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.
 
     ONE nvidia-smi process per job (rank 0 samples every GPU of the node), started BEFORE the warm-up steps: spawning it costs
     ~100 ms of NVML initialisation during which driver calls of the benchmark can stall -- round 1 started one process per rank at
@@ -154,8 +154,27 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3; 700 W card)"
+
+
+def dump_outputs(outdir, arrays):
+    """Writes {name: tensor} as outdir/<name>.npy in float32 (float64 stays float64).  Every array keeps at most its share of
+    DUMP_MAX_BYTES: a larger one is written as the 1-D sample at sorted flat indices drawn from a generator seeded with 0, so
+    two runs of the same shapes sample the same elements."""
+    import numpy as np
+    import torch
+
+    os.makedirs(outdir, exist_ok=True)
+    share = DUMP_MAX_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        t = t.detach()
+        t = t.double() if t.dtype == torch.float64 else t.float()
+        limit = share // t.element_size()
+        if t.numel() > limit:
+            idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(0))[:limit].sort().values
+            t = t.reshape(-1)[idx.to(t.device)]
+        np.save(os.path.join(outdir, f"{name}.npy"), t.cpu().numpy())
 
 
 # =============================================================================================== reference arm (CPU)
@@ -418,10 +437,10 @@ def run_train(args, cfg):
         if prof_range:
             torch.cuda.profiler.start()
         e0.record()
-        loss = None
+        loss = items = None
         for i in range(args.steps):
             step.set_hyper_params(lr_at(i), ema_decay)
-            loss, _ = step.run(dev_x[i % nbuf], dev_t[i % nbuf])
+            loss, items = step.run(dev_x[i % nbuf], dev_t[i % nbuf])
         e1.record()
         barrier()
         if prof_range:
@@ -432,9 +451,11 @@ def run_train(args, cfg):
             t = torch.tensor([ms], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t)
-        return ms, clocks, loss
+        return ms, clocks, loss, items
 
-    ms, clocks, loss = timed_region()
+    ms, clocks, loss, items = timed_region()
+    if args.dump_outputs:  # before anything else advances the model: the state the K timed steps left
+        dump_outputs(args.dump_outputs, {"loss": loss.reshape(1), "loss_items": items, "params": step.flat.params})
     # a thermally / hardware-throttled region, or clocks pinned far below max without a reason, is measured once more (every
     # rank follows rank 0's verdict: the region contains collectives)
     bad = {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"} & set(clocks.get("reasons", []))
@@ -444,7 +465,7 @@ def run_train(args, cfg):
         dist.broadcast(redo, src=0)
     if int(redo) == 1 and not prof_range:
         first = clocks
-        ms, clocks, loss = timed_region()
+        ms, clocks, loss, _ = timed_region()
         clocks["remeasured_after"] = {"reasons": first.get("reasons"), "sm_mhz": first.get("sm_mhz")}
     sampler.stop()
     final_loss = float(loss)
@@ -522,7 +543,7 @@ def run_train(args, cfg):
         "config": {
             "workload": cfg["workload"], "config": args.config, "per_gpu_batch": batch,
             "global_batch": batch * world, "parallelism": f"dp{world}", "cuda_graph": use_graph,
-            "l2": f"4 distinct {host_x[0].numel() * 4 / 1e6:.0f} MB input batches rotate (each > 126 MB L2); activations of a step (> 10 GB) never fit L2",
+            "l2": f"4 distinct {host_x[0].numel() * 4 / 1e6:.0f} MB input batches rotate (each > 50 MB L2); activations of a step (> 10 GB) never fit L2",
         },
         "e2e": {"value": e2e, "unit": "images/sec", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": ms2 / e2e_steps},
         "gpu_launches": launches_per_step * args.steps, "gpu_launches_per_step": launches_per_step,
@@ -545,13 +566,12 @@ def conv_roofline(profile, n_prof, cfg, batch, step_ms, config_id):
     conv_bytes /= n_prof
     flops = cfg["gflop"] * 1e9 * batch
     achieved = flops / (conv_ms / 1e3) / 1e12
-    traffic, traffic_src = NCU_CONV_DRAM.get((config_id, batch), (None, None))
     return {
         "bound": "tensor", "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved / tf_peak,
-        "traffic": traffic, "traffic_source": traffic_src or "not captured for this configuration",
-        "kernel": "conv family of one step = one 'launch': conv3x3_halo_kernel / conv1x1_tile_kernel + wgrad3x3_halo_kernel (stride 1), conv_umma_kernel + wgrad_umma_kernel (stride 2, wide 1x1)",
+        "traffic": None, "traffic_source": "not measured",
+        "kernel": "conv family of one step = one 'launch': conv_wgmma_kernel (fprop / dgrad) + wgrad_wgmma_kernel, mma.sync kernels for the stems",
         "peak_source": which, "conv_ms_per_step": conv_ms, "conv_share_of_step": conv_ms / step_ms,
-        "timing": "CUDA events around every launch of an eager pass on its launching stream (the in-graph kernels run ~25 % faster: tools/timeline.py)",
+        "timing": "CUDA events around every launch of an eager pass on its launching stream (in-graph kernels run without the per-launch host gaps)",
         "algorithmic_flops_per_step": flops, "algorithmic_activation_bytes_per_step": conv_bytes,
         "hbm_view": {"achieved_GBps": conv_bytes / (conv_ms / 1e3) / 1e9, "peak_GBps": hbm_peak, "frac": conv_bytes / (conv_ms / 1e3) / 1e9 / hbm_peak,
                      "note": "narrow layers (32..192 channels) are HBM / shared-memory-operand bound, not tensor bound (DESIGN.md section 3)"},
@@ -621,6 +641,8 @@ def run_predict(args, cfg):
         out = gpu_step(dev_x[i % nbuf])
     e1.record()
     barrier()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dict(zip(("rows", "poses", "anchor_index", "count"), out)))
     clocks = sampler.snapshot()
     sampler.stop()
     ms = e0.elapsed_time(e1)
@@ -705,6 +727,7 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="per-GPU batch (default: the configuration's)")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step computed as DIR/<name>.npy (<= 64 MB in all)")
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * sgb200.h -- C ABI of libsgb200.so: the B200 (sm_100a) hot path behind SuperGradients' YOLO-NAS / ResNet
+ * sgb200.h -- C ABI of libsgb200.so: the H100 (sm_90a) hot path behind SuperGradients' YOLO-NAS / ResNet
  * training and inference modules.
  *
  * The reference (Deci-AI/super-gradients) has no FFI: every kernel on this path is reached through
@@ -27,7 +27,7 @@ extern "C" {
 #define SGB_E_INVALID (-1)     /* bad shape / argument */
 #define SGB_E_UNSUPPORTED (-2) /* valid but not implemented for this configuration */
 #define SGB_E_CUDA (-3)        /* a CUDA runtime / driver call failed (see sgb_last_error) */
-#define SGB_E_ARCH (-4)        /* device is not sm_100 */
+#define SGB_E_ARCH (-4)        /* device is not sm_90 */
 
 #define SGB_ACT_NONE 0
 #define SGB_ACT_RELU 1
@@ -60,17 +60,11 @@ typedef struct SgbEpilogue {
 
 const char* sgb_last_error(void);
 int sgb_version(void);
-/* 0 if the current device is sm_100 and the library was built for it. */
+/* 0 if the current device is sm_90 and the library was built for it. */
 int sgb_check_device(void);
-/* Number of tcgen05/TMA convolution launches issued by this process so far (evidence that the Blackwell-native path,
+/* Number of wgmma/TMA convolution launches issued by this process so far (evidence that the Hopper-native path,
  * not the generic mma.sync kernel, served a call). */
 int64_t sgb_sm100_launches(void);
-/* ... of which served by the halo-tile 3x3 kernel (conv_halo_sm100.cu). */
-int64_t sgb_sm100_halo_launches(void);
-
-/* Developer hook: copies the 12 x 512 SM-clock stamps recorded by CTA 0 of the last tcgen05 convolution launched with
- * SGB_DEBUG_SKIP & 16 into host_out (int64[6144]); used by tools/ to study the TMA / MMA pipeline, never by the product. */
-int sgb_debug_read_trace(int64_t* host_out);
 
 /* ---- convolution family (rows C1-C5, C8, C10 of SURVEY.md section 8a) --------------------------------------
  * replaces nn.Conv2d forward in modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,

@@ -92,4 +92,4 @@ def activation_code(act_type) -> str:
         return "relu"
     if act_type is nn.SiLU:
         return "silu"
-    raise NotImplementedError(f"activation {act_type} has no sm_100a epilogue in super_gradients_b200")
+    raise NotImplementedError(f"activation {act_type} has no sm_90a epilogue in super_gradients_b200")

@@ -158,7 +158,7 @@ extern "C" int sgb_atss_assign(const SgbLossDesc* d, const float* reg_distri, co
   SGB_REQUIRE(acc == d->L, "level sizes must add up to the number of anchors");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t BL = (int64_t)d->B * d->L;
-  const int grid = (int)((BL + 255) / 256 > 148 * 8 ? 148 * 8 : (BL + 255) / 256);
+  const int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
   int* count = reinterpret_cast<int*>(workspace);
   int* owner = count + BL;
   atss_init_kernel<<<grid, 256, 0, st>>>(count, owner, BL);

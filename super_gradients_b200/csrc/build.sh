@@ -1,30 +1,28 @@
 #!/usr/bin/env bash
-# Builds libsgb200.so (sm_100a only) in-tree.  Usage: build.sh [extra nvcc flags]
+# Builds libsgb200.so (sm_90a only) in-tree.  Usage: build.sh [extra nvcc flags]
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 ROOT="$(cd "$HERE/../.." && pwd)"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-OUT="${SGB_OUT:-$HERE/../libsgb200.so}"   # SGB_OUT / SGB_OBJ: build a variant (e.g. -DSGB_DETERMINISTIC_STATS) next to the default library
+OUT="${SGB_OUT:-$HERE/../libsgb200.so}"   # SGB_OUT / SGB_OBJ: build a variant (e.g. without -DSGB_DETERMINISTIC_STATS) next to the default library
 OBJ="${SGB_OBJ:-$HERE/obj}"
-# Default feature set (each measured on B200 in round 2, tools/gpu_call.sh; profiles/r2_variants_bench.txt, r2_determinism_repro.txt):
-#   SGB_DETERMINISTIC_STATS  per-warp BatchNorm-statistics slots summed in a fixed order: removes the run-to-run last-bit
-#                            differences of interleaved models (DESIGN.md section 8.1) at < 1 % cost
-#   SGB_UMMA_WIDE_STORE      256-bit stores in the im2col kernels' fast epilogue (+2 %)
-#   SGB_HALO_1X1             1x1 stride-1 convolutions on the halo-tile pipeline (+1 %)
-# -DSGB_PDL (programmatic dependent launch) measured 2 % SLOWER on the graph step and stays off.
-DEFS=(${SGB_DEFS:--DSGB_DETERMINISTIC_STATS -DSGB_UMMA_WIDE_STORE -DSGB_HALO_1X1})
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I"$ROOT/include" -I"$HERE" --expt-relaxed-constexpr "${DEFS[@]}")
+# Default feature set:
+#   SGB_DETERMINISTIC_STATS  per-warp BatchNorm-statistics slots of the mma.sync kernels summed in a fixed order: removes the
+#                            run-to-run last-bit differences of interleaved models (DESIGN.md section 8.1)
+# -DSGB_PDL (programmatic dependent launch) is an experiment and stays off.
+DEFS=(${SGB_DEFS:--DSGB_DETERMINISTIC_STATS})
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I"$ROOT/include" -I"$HERE" --expt-relaxed-constexpr "${DEFS[@]}")
 mkdir -p "$OBJ"
 pids=()
 for f in "$HERE"/*.cu; do
   o="$OBJ/$(basename "${f%.cu}").o"
   stale=0
-  for h in "$HERE"/*.cuh "$HERE"/*.h "$HERE"/*.inc "$ROOT/include/sgb200.h"; do [[ "$h" -nt "$o" ]] && stale=1; done
+  for h in "$HERE"/*.cuh "$HERE"/*.h "$ROOT/include/sgb200.h" "$HERE/build.sh"; do [[ "$h" -nt "$o" ]] && stale=1; done
   if [[ ! -f "$o" || "$f" -nt "$o" || $stale -eq 1 ]]; then
     "$NVCC" "${FLAGS[@]}" "$@" -c "$f" -o "$o" &
     pids+=($!)
   fi
 done
-for p in "${pids[@]:-}"; do [[ -n "$p" ]] && wait "$p"; done
-"$NVCC" -shared -o "$OUT" "$OBJ"/*.o -lcudart
+for p in "${pids[@]:-}"; do [[ -n "$p" ]] && { wait "$p" || exit 1; }; done
+"$NVCC" -gencode arch=compute_90a,code=sm_90a -shared -o "$OUT" "$OBJ"/*.o -lcudart
 echo "built $OUT"

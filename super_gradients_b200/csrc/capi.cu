@@ -28,17 +28,11 @@ extern "C" int sgb_check_device(void) {
   if (int rc = sgb_cuda_check(cudaGetDevice(&dev), "cudaGetDevice")) return rc;
   cudaDeviceProp prop;
   if (int rc = sgb_cuda_check(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties")) return rc;
-  if (prop.major != 10) {
-    sgb_set_error("libsgb200 is built for sm_100a only; device is sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9) {
+    sgb_set_error("libsgb200 is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
     return SGB_E_ARCH;
   }
   return SGB_OK;
 }
 
 extern "C" int64_t sgb_sm100_launches(void) { return (int64_t)sm100::launch_count(); }
-extern "C" int64_t sgb_sm100_halo_launches(void) { return (int64_t)sm100::halo_launch_count(); }
-
-extern "C" int sgb_debug_read_trace(int64_t* host_out) {
-  if (!host_out) return SGB_E_INVALID;
-  return sm100::read_trace(reinterpret_cast<long long*>(host_out));
-}

@@ -1,4 +1,4 @@
-// Shared device helpers for libsgb200 (sm_100a only).
+// Shared device helpers for libsgb200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -78,13 +78,13 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-// CTA cap of the streaming per-channel kernels: 148 SMs x SGB_CHAN_CTAS_PER_SM (default 6; the environment variable is a tuning hook)
+// CTA cap of the streaming per-channel kernels: 132 SMs x SGB_CHAN_CTAS_PER_SM (default 6; the environment variable is a tuning hook)
 static inline int sgb_chan_grid_cap() {
   static int cap = 0;
   if (cap == 0) {
     const char* e = getenv("SGB_CHAN_CTAS_PER_SM");
     const int per_sm = (e && atoi(e) > 0) ? atoi(e) : 6;
-    cap = 148 * per_sm;
+    cap = 132 * per_sm;
   }
   return cap;
 }

@@ -777,7 +777,7 @@ extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb
   if (d->K > 64 && d->K <= 96) bmw = 32;  // 3 x 32 wastes nothing
   int mt = ceil_div(d->K, bmw), nt = ceil_div(p.ncols, 64);
   int total_slices = ceil_div(p.npix, BK);
-  int target = 148 * 4;
+  int target = 132 * 4;
   int splits = target / (mt * nt);
   if (splits < 1) splits = 1;
   if (splits > total_slices) splits = total_slices;

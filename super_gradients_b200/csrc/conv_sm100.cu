@@ -1,17 +1,16 @@
-// Blackwell-native implicit-GEMM convolution, TMA-im2col engine: tcgen05.mma (UMMA, M=128) with the accumulator in TMEM,
-// the A operand streamed by TMA *im2col* descriptors straight from the NHWC activation tensor, the B operand (KRSC / CRSK
-// filters) by tiled TMA, persistent warp-specialised CTAs (1-3 co-resident per SM):
-//     warp 0      TMA producer            (one elected lane)
-//     warp 1      TMEM allocator + MMA issuer (the warp stays converged; the elected lane's tcgen05.mma / commit issue)
-//     warps 2..5  epilogue: tcgen05.ld -> (scale, shift, residual, activation) -> bf16 -> global,
-//                 plus the per-channel sum / sum-of-squares needed by train-mode BatchNorm (butterfly transpose-reduce)
-// Two TMEM accumulators are ping-ponged so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Hopper-native implicit-GEMM convolution: wgmma (M = 64 per warpgroup, fp32 accumulators in registers), the A operand
+// streamed by TMA *im2col* descriptors straight from the NHWC activation tensor, the B operand (KRSC / CRSK filters) by
+// tiled TMA, an mbarrier ring of shared-memory stages, persistent CTAs of three warpgroups:
+//     warpgroup 0     TMA producer (one elected lane)
+//     warpgroups 1-2  wgmma over 64 rows each of the 128-pixel tile, then the epilogue straight from the accumulator
+//                     registers: (scale, shift, residual, activation) -> bf16 -> global, plus the per-channel sum /
+//                     sum-of-squares needed by train-mode BatchNorm, combined across warps in a fixed order
+// The producer runs up to `stages` k-iterations ahead, so the loads of tile i+1 overlap the epilogue of tile i.
 //
-// Serves what the halo-tile engine (conv_halo_sm100.cu: every 3x3 stride-1 convolution with C in {32..128}) does not:
-// 1x1 convolutions, stride-2 3x3 (fprop; dgrad as s^2 output-parity classes through the explicit tap table), C >= 192,
-// fused scale / shift / residual / activation epilogues, and the weight gradients of those shapes (wgrad_umma_kernel,
-// MN-major operands).  launch() / wgrad_launch() try the halo engine first.  3-channel stems that are not padded to
-// 16 channels, 7x7, ragged channel counts and fp32 outputs stay on the mma.sync kernels of conv_mma.cu.
+// Serves every 1x1 and 3x3 convolution with C % 16 == 0 (fprop; stride-1 dgrad over the flipped CRSK filter; stride-2 dgrad as
+// s^2 output-parity classes through the explicit tap table) and their weight gradients (wgrad_wgmma_kernel, MN-major
+// operands).  3-channel stems that are not padded to 16 channels, 7x7, ragged channel counts and fp32 outputs stay on the
+// mma.sync kernels of conv_mma.cu.
 //
 // Reference arithmetic replaced: nn.Conv2d forward / input-gradient / weight-gradient as used by
 // modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,
@@ -29,20 +28,19 @@
 namespace sm100 {
 
 constexpr int BLOCK_M = 128;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;
+constexpr int CONSUMER_THREADS = 256;
 constexpr int MAX_STAGES = 8;
 
 struct Params {
   int M;            // output pixels (GEMM rows)
   int N;            // output channels (GEMM cols)
   int C;            // channels per tap of the gathered tensor
-  int R, S;         // taps
   int KC;           // channels per TMA box (16 / 32 / 64)
-  int BN;           // N tile (multiple of 16, <= 256)
+  int n_tiles;      // N tiles of BN columns
   int stages;
   int P, Q;         // output spatial size (rows -> (n, p, q))
   int stride, pad;  // traversal stride, lower padding of the gather
-  int flip;         // 1: B columns are visited with spatially flipped taps (dgrad)
   int b_cols_per_tap;
   int ntaps;                  // taps visited (R*S for fprop / stride-1 dgrad; a subset for a stride-2 dgrad parity class)
   signed char tap_dh[9], tap_dw[9], tap_b[9];  // im2col offsets of each tap and its column block in the B matrix
@@ -58,12 +56,6 @@ struct Params {
   double* stats;
   int stats_repl;
   int act;
-  int tmem_cols;
-  // b_resident: the whole filter (ntaps x chunks tiles of BN x KC) is loaded ONCE per CTA into its own shared-memory region instead of
-  // being re-streamed from L2 with every k-iteration of every 128-pixel tile (the floor of the stride-2 layers: DESIGN.md section 3).
-  int b_resident;
-  uint32_t b_tile_bytes;
-  int dbg;  // SGB_DEBUG_SKIP bit mask (perf experiments only): 1 no stores, 2 no stats, 4 no A loads
 };
 
 __device__ __forceinline__ long long out_row(const Params& p, long long m) {
@@ -75,73 +67,54 @@ __device__ __forceinline__ long long out_row(const Params& p, long long m) {
   return ((long long)n * p.outH + j * p.o_mul + p.oh_add) * p.outW + i * p.o_mul + p.ow_add;
 }
 
-// SGB_DEBUG_SKIP & 16: CTA 0 records SM clock stamps of its first 512 k-iterations (perf experiments only):
-// [0] producer passed the empty wait, [1] producer issued its TMA, [2] MMA warp passed the full wait, [3] MMA committed
-__device__ long long g_trace[12][512];
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory"); }
+
+// Shared-memory layout after the stages: full / empty barriers, then (statistics only) the per-warp column partials of the
+// current tile [8 warps][2][BN] and the CTA's per-channel totals [2][N].
+constexpr uint32_t CTRL_BAR_BYTES = 16u * MAX_STAGES;
 
 // ------------------------------------------------------------------------------------------------ the kernel
-template <int NCH, bool STATS>
+template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
   SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = p.BN * p.KC * 2;
-  const uint32_t stage_bytes = a_bytes + (p.b_resident ? 0u : ((b_bytes + 1023u) & ~1023u));
-  // resident filter tiles after the stages, then the control block
-  const uint32_t bres_base = smem_base + p.stages * stage_bytes;
-  const uint32_t ctrl = bres_base + (p.b_resident ? (uint32_t)(p.ntaps * ((p.C + p.KC - 1) / p.KC)) * p.b_tile_bytes : 0u);
+  const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = BN * p.KC * 2;
+  const uint32_t stage_bytes = a_bytes + ((b_bytes + 1023u) & ~1023u);
+  const uint32_t ctrl = smem_base + p.stages * stage_bytes;
   auto full_bar = [&](int s) { return ctrl + 8u * s; };
   auto empty_bar = [&](int s) { return ctrl + 8u * (MAX_STAGES + s); };
-  auto tfull_bar = [&](int b) { return ctrl + 8u * (2 * MAX_STAGES + b); };
-  auto tempty_bar = [&](int b) { return ctrl + 8u * (2 * MAX_STAGES + 2 + b); };
-  const uint32_t tmem_slot = ctrl + 8u * (2 * MAX_STAGES + 4);
-  const uint32_t bres_bar = tmem_slot + 8u;  // second half of the 16-byte slot
-  float* s_stats = reinterpret_cast<float*>(smem_raw + (ctrl - smem_u32(smem_raw)) + 8u * (2 * MAX_STAGES + 4) + 16);
+  float* s_part = reinterpret_cast<float*>(smem_raw + (ctrl + CTRL_BAR_BYTES - smem_u32(smem_raw)));
+  float* s_stats = s_part + 8 * 2 * BN;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M, n_tiles = (p.N + p.BN - 1) / p.BN;
-  const int total_tiles = m_tiles * n_tiles;
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int total_tiles = m_tiles * p.n_tiles;
   const int chunks = (p.C + p.KC - 1) / p.KC;  // a last chunk reaching past C is zero-filled by TMA (out-of-bounds channels)
   const int k_iters = p.ntaps * chunks;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), 4);
-    }
-    mbar_init(bres_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   if (p.stats)
-    for (int i = threadIdx.x; i < SGB_STATS_SLOTS * 2 * p.N; i += NUM_THREADS) s_stats[i] = 0.f;
-  if (warp == 1) tcgen05_alloc(tmem_slot, p.tmem_cols);
-  tcgen05_fence_before();
+    for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) s_stats[i] = 0.f;
   __syncthreads();
-  tcgen05_fence_after();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory / TMEM
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (warp == 0) {
     // ===================================================================================== TMA producer
     if (elect_one()) {
-      int it = 0, stg = 0;
+      int stg = 0;
       uint32_t par = 1;  // parity awaited on the empty barriers: the first pass through the ring is free
       const int pq = p.P * p.Q;
-      if (p.b_resident && (int)blockIdx.x < total_tiles) {  // the whole filter, once (n_tiles == 1)
-        mbar_expect_tx(bres_bar, (uint32_t)k_iters * b_bytes);
-        for (int tap = 0; tap < p.ntaps; ++tap)
-          for (int ck = 0; ck < chunks; ++ck)
-            tma_load_2d(bres_base + (uint32_t)(tap * chunks + ck) * p.b_tile_bytes, &map_b, bres_bar, p.tap_b[tap] * p.b_cols_per_tap + ck * p.KC, 0);
-      }
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
+        const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
         const int m0 = mt * BLOCK_M;
         const int n_img = m0 / pq;
         const int rem = m0 - n_img * pq;
@@ -150,17 +123,12 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const int r = p.tap_dh[tap], s = p.tap_dw[tap];
           const int btap = p.tap_b[tap];
-          for (int ck = 0; ck < chunks; ++ck, ++it) {
+          for (int ck = 0; ck < chunks; ++ck) {
             mbar_wait(empty_bar(stg), par);
-            const bool tr = (p.dbg & 16) && blockIdx.x == 0 && it < 512;
-            if (tr) g_trace[0][it] = clock64();
             const uint32_t sa = smem_base + stg * stage_bytes, sb = sa + a_bytes;
-            mbar_expect_tx(full_bar(stg), ((p.dbg & 4) ? 0u : a_bytes) + (p.b_resident ? 0u : b_bytes));
-            if (tr) g_trace[4][it] = clock64();
-            if (!(p.dbg & 4)) tma_load_im2col_4d(sa, &map_a, full_bar(stg), ck * p.KC, w0, h0, n_img, (uint16_t)s, (uint16_t)r);
-            if (tr) g_trace[5][it] = clock64();
-            if (!p.b_resident) tma_load_2d(sb, &map_b, full_bar(stg), btap * p.b_cols_per_tap + ck * p.KC, nt * p.BN);
-            if (tr) g_trace[1][it] = clock64();
+            mbar_expect_tx(full_bar(stg), a_bytes + b_bytes);
+            tma_load_im2col_4d(sa, &map_a, full_bar(stg), ck * p.KC, w0, h0, n_img, (uint16_t)s, (uint16_t)r);
+            tma_load_2d(sb, &map_b, full_bar(stg), btap * p.b_cols_per_tap + ck * p.KC, nt * BN);
             if (++stg == p.stages) {
               stg = 0;
               par ^= 1;
@@ -169,309 +137,182 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================================== MMA issuer
-    // The warp stays converged (descriptors live in uniform registers); only the elected lane's instructions issue.
-    const uint32_t leader = elect_one() ? 1u : 0u;
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-    const uint64_t desc_hi = make_smem_desc(0, p.KC);
-    const uint32_t ksteps = (uint32_t)p.KC / 16;
-    int it = 0, tcount = 0, stg = 0;
+  } else if (warp >= 4) {
+    // ===================================================================================== MMA + epilogue
+    const int wg = (warp >> 2) - 1;  // rows [64 * wg, 64 * wg + 64) of the tile
+    const int wq = warp & 3;         // 16-row slice of the warpgroup's 64 rows
+    const int row_bytes = p.KC * 2;
+    const uint32_t sbo = 8u * (uint32_t)row_bytes;
+    const int ksteps = p.KC / 16;
+    float acc[BN / 2];
+    int stg = 0;
     uint32_t par = 0;
-    if (p.b_resident && (int)blockIdx.x < total_tiles) {
-      mbar_wait(bres_bar, 0);
-      tcgen05_fence_after();
-    }
-    const uint32_t bres16 = bres_base >> 4, btile16 = p.b_tile_bytes >> 4;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-      const int ab = tcount & 1;
-      const uint32_t apar = ((tcount >> 1) & 1) ^ 1;
-      mbar_wait(tempty_bar(ab), apar);
-      tcgen05_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(ab * p.BN);
-      for (int k = 0; k < k_iters; ++k, ++it) {
-        const bool tr0 = (p.dbg & 16) && blockIdx.x == 0 && it < 512 && lane == 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+      int prev = -1;
+      for (int k = 0; k < k_iters; ++k) {
         mbar_wait(full_bar(stg), par);
-        if (tr0) g_trace[2][it] = clock64();
-        tcgen05_fence_after();
-        const uint32_t sa = (smem_base + stg * stage_bytes) >> 4, sb = p.b_resident ? bres16 + (uint32_t)k * btile16 : sa + (a_bytes >> 4);
-#pragma unroll
-        for (uint32_t j = 0; j < 4; ++j) {
-          // advance 16 bf16 (32 bytes) along K inside the swizzle atom: +2 in the (addr >> 4) field
-          const uint64_t da = desc_hi | (uint64_t)((sa + 2 * j) & 0x3fff), db = desc_hi | (uint64_t)((sb + 2 * j) & 0x3fff);
-          if (!(p.dbg & 8)) umma_bf16_if((j < ksteps) ? leader : 0u, d_tmem, da, db, idesc, (k | (int)j) != 0);
+        const uint32_t sa = smem_base + stg * stage_bytes, sb = sa + a_bytes;
+        const uint32_t sa_wg = sa + (uint32_t)wg * 64u * (uint32_t)row_bytes;
+        wgmma_fence();
+        for (int j = 0; j < ksteps; ++j) {
+          // advance 16 bf16 (32 bytes) along K inside the swizzle atom
+          const uint64_t da = smem_desc(sa_wg + 32u * j, row_bytes, 16u, sbo), db = smem_desc(sb + 32u * j, row_bytes, 16u, sbo);
+          mma_kk<BN>(acc, da, db, (k | j) != 0);
         }
-        umma_commit_if(leader, empty_bar(stg));
-        if (k == k_iters - 1) umma_commit_if(leader, tfull_bar(ab));
-        if (tr0) g_trace[3][it] = clock64();
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();  // the previous stage's MMAs are complete: its shared memory may be refilled
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(prev));
+        }
+        prev = stg;
         if (++stg == p.stages) {
           stg = 0;
           par ^= 1;
         }
       }
-    }
-  } else {
-    // ===================================================================================== epilogue
-    const int quarter = warp & 3;  // TMEM lanes [32*quarter, 32*quarter+32) are the ones this warp may read
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const int row = quarter * 32 + lane;
-    int tcount = 0;
-    if constexpr (NCH > 0) {
-      // ---- fast path: one N tile of NCH*16 columns, no scale / shift / residual / activation.  The per-channel
-      // statistics are accumulated per thread (row) in registers across ALL tiles of this CTA and reduced across the
-      // warp once at the end, so a tile costs ~3.5 instructions per element.
-      float a1[STATS ? NCH * 16 : 1], a2[STATS ? NCH * 16 : 1];
-#ifdef SGB_UMMA_WIDE_STORE
-      const bool wide_store = (p.y_pitch % 16 == 0) && (p.y_off % 16 == 0) && ((reinterpret_cast<uintptr_t>(p.y) & 31) == 0);
-#endif
-      if constexpr (STATS) {
+      wgmma_wait<0>();
+      fence_regs(acc);
+      __syncwarp();
+      if (lane == 0 && prev >= 0) mbar_arrive(empty_bar(prev));
+
+      // ---- epilogue: thread holds rows r_lo, r_lo + 8 and column pairs 8 j + 2 (lane % 4)
+      const int r_lo = wg * 64 + wq * 16 + (lane >> 2);
+      const int n0 = nt * BN;
+      const int ncols = min(BN, p.N - n0);
+      const long long m_lo = (long long)mt * BLOCK_M + r_lo;
+      bf16* yrow[2];
+      const bf16* rrow[2];
+      bool row_ok[2];
 #pragma unroll
-        for (int i = 0; i < NCH * 16; ++i) a1[i] = a2[i] = 0.f;
+      for (int h = 0; h < 2; ++h) {
+        const long long m = m_lo + 8 * h;
+        row_ok[h] = m < p.M;
+        const long long orow = out_row(p, row_ok[h] ? m : 0);
+        yrow[h] = p.y + orow * p.y_pitch + p.y_off + n0;
+        rrow[h] = p.residual ? p.residual + orow * p.y_pitch + p.y_off + n0 : nullptr;
       }
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-        const int ab = tcount & 1;
-        mbar_wait(tfull_bar(ab), (tcount >> 1) & 1);
-        tcgen05_fence_after();
-        const long long m = (long long)tile * BLOCK_M + row;
-        const bool row_ok = m < p.M;
-        bf16* yrow = p.y + out_row(p, m) * p.y_pitch + p.y_off;
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          float v[16];
-          tmem_ld16(tmem_base + lane_base + (uint32_t)(ab * (NCH * 16) + c * 16), v);
-          uint32_t pk[8];
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        const bool col_ok = col < ncols;  // N % 8 == 0: both columns of the pair are valid or neither
+        float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-            pk[i] = *reinterpret_cast<uint32_t*>(&h);
+        for (int h = 0; h < 2; ++h) {
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          const bool ok = row_ok[h] && col_ok;
+          if (p.scale && col_ok) {
+            v0 *= p.scale[n0 + col];
+            v1 *= p.scale[n0 + col + 1];
           }
-          if (row_ok) {
-            if (!(p.dbg & 1)) {
-#ifdef SGB_UMMA_WIDE_STORE  // experiment: one 256-bit store per 16 channels (as the halo kernels do) when the row is 32-byte aligned
-              if (wide_store) {
-                asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(yrow + c * 16), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]),
-                             "r"(pk[3]), "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7])
-                             : "memory");
-              } else
-#endif
-              {
-                *reinterpret_cast<uint4*>(yrow + c * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                *reinterpret_cast<uint4*>(yrow + c * 16 + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-              }
-            }
-            if constexpr (STATS) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float lo = __uint_as_float(pk[i] << 16), hi = __uint_as_float(pk[i] & 0xffff0000u);
-                a1[c * 16 + 2 * i] += lo;
-                a2[c * 16 + 2 * i] = fmaf(lo, lo, a2[c * 16 + 2 * i]);
-                a1[c * 16 + 2 * i + 1] += hi;
-                a2[c * 16 + 2 * i + 1] = fmaf(hi, hi, a2[c * 16 + 2 * i + 1]);
-              }
-            }
+          if (p.shift && col_ok) {
+            v0 += p.shift[n0 + col];
+            v1 += p.shift[n0 + col + 1];
           }
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(ab));
-      }
-      if constexpr (STATS) {
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          float t1[16], t2[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            t1[i] = a1[c * 16 + i];
-            t2[i] = a2[c * 16 + i];
-          }
-          const float s1 = butterfly_colsum(t1, lane), s2 = butterfly_colsum(t2, lane);
-          if ((lane & 1) == 0) {
-#if SGB_STATS_SLOTS == 1
-            atomicAdd(&s_stats[c * 16 + col_of_lane(lane)], s1);
-            atomicAdd(&s_stats[p.N + c * 16 + col_of_lane(lane)], s2);
-#else
-            float* mine = s_stats + quarter * 2 * p.N;  // this warp's slot: each (even lane, column) is written by one lane
-            mine[c * 16 + col_of_lane(lane)] += s1;
-            mine[p.N + c * 16 + col_of_lane(lane)] += s2;
-#endif
-          }
-        }
-      }
-    } else {
-      // ---- general path: ragged N, several N tiles, fused scale / shift / residual / activation
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-        const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-        const int ab = tcount & 1;
-        mbar_wait(tfull_bar(ab), (tcount >> 1) & 1);
-        tcgen05_fence_after();
-        const long long m = (long long)mt * BLOCK_M + row;
-        const bool row_ok = m < p.M;
-        const int n0 = nt * p.BN;
-        const long long orow = out_row(p, m);
-        bf16* yrow = p.y + orow * p.y_pitch + p.y_off + n0;
-        const bf16* rrow = p.residual ? p.residual + orow * p.y_pitch + p.y_off + n0 : nullptr;
-        const int ncols = min(p.BN, p.N - n0);
-        for (int c0 = 0; c0 < ncols; c0 += 16) {
-          float v[16];
-          tmem_ld16(tmem_base + lane_base + (uint32_t)(ab * p.BN + c0), v);
-          const bool full = c0 + 16 <= ncols;
-          if (p.scale) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (full || c0 + i < ncols) v[i] *= p.scale[n0 + c0 + i];
-          }
-          if (p.shift) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (full || c0 + i < ncols) v[i] += p.shift[n0 + c0 + i];
-          }
-          if (rrow && row_ok) {
-            if (full) {
-              const uint4 r0 = *reinterpret_cast<const uint4*>(rrow + c0), r1 = *reinterpret_cast<const uint4*>(rrow + c0 + 8);
-              const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                v[2 * i] += __uint_as_float(rr[i] << 16);
-                v[2 * i + 1] += __uint_as_float(rr[i] & 0xffff0000u);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i)
-                if (c0 + i < ncols) v[i] += __bfloat162float(rrow[c0 + i]);
-            }
+          if (rrow[h] && ok) {
+            const uint32_t rr = *reinterpret_cast<const uint32_t*>(rrow[h] + col);
+            v0 += __uint_as_float(rr << 16);
+            v1 += __uint_as_float(rr & 0xffff0000u);
           }
           if (p.act != SGB_ACT_NONE) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = apply_act(v[i], p.act);
+            v0 = apply_act(v0, p.act);
+            v1 = apply_act(v1, p.act);
           }
-          uint32_t pk[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-            pk[i] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          if (row_ok && !(p.dbg & 1)) {
-            if (full) {
-              *reinterpret_cast<uint4*>(yrow + c0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              *reinterpret_cast<uint4*>(yrow + c0 + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                if (c0 + 2 * i < ncols) yrow[c0 + 2 * i] = __ushort_as_bfloat16((unsigned short)(pk[i] & 0xffffu));
-                if (c0 + 2 * i + 1 < ncols) yrow[c0 + 2 * i + 1] = __ushort_as_bfloat16((unsigned short)(pk[i] >> 16));
-              }
-            }
-          }
-          if (p.stats && !(p.dbg & 2)) {
-            float t1[16], t2[16];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const bool ok0 = row_ok && (full || c0 + 2 * i < ncols), ok1 = row_ok && (full || c0 + 2 * i + 1 < ncols);
-              const float lo = ok0 ? __uint_as_float(pk[i] << 16) : 0.f, hi = ok1 ? __uint_as_float(pk[i] & 0xffff0000u) : 0.f;
-              t1[2 * i] = lo;
-              t1[2 * i + 1] = hi;
-              t2[2 * i] = lo * lo;
-              t2[2 * i + 1] = hi * hi;
-            }
-            const float s1 = butterfly_colsum(t1, lane), s2 = butterfly_colsum(t2, lane);
-            const int c = c0 + col_of_lane(lane);
-            if ((lane & 1) == 0 && c < ncols) {
-#if SGB_STATS_SLOTS == 1
-              atomicAdd(&s_stats[n0 + c], s1);
-              atomicAdd(&s_stats[p.N + n0 + c], s2);
-#else
-              float* mine = s_stats + quarter * 2 * p.N;  // tiles are visited in a fixed order by this warp
-              mine[n0 + c] += s1;
-              mine[p.N + n0 + c] += s2;
-#endif
-            }
+          __nv_bfloat162 hh = __floats2bfloat162_rn(v0, v1);
+          const uint32_t pk = *reinterpret_cast<uint32_t*>(&hh);
+          if (ok) {
+            *reinterpret_cast<uint32_t*>(yrow[h] + col) = pk;
+            const float lo = __uint_as_float(pk << 16), hi = __uint_as_float(pk & 0xffff0000u);
+            sum0 += lo;
+            sum1 += hi;
+            sq0 = fmaf(lo, lo, sq0);
+            sq1 = fmaf(hi, hi, sq1);
           }
         }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(ab));
+        if (p.stats) {
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+            sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+            sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
+            sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
+          }
+          if (lane < 4) {
+            float* part = s_part + (wg * 4 + wq) * 2 * BN;
+            part[col] = sum0;
+            part[col + 1] = sum1;
+            part[BN + col] = sq0;
+            part[BN + col + 1] = sq1;
+          }
+        }
+      }
+      if (p.stats) {
+        // the eight warps' partials of this tile, summed in a fixed order (bit-reproducible statistics)
+        consumer_sync();
+        for (int i = threadIdx.x - 128; i < 2 * BN; i += CONSUMER_THREADS) {
+          const int which = i / BN, c = i - which * BN;
+          if (c < ncols) {
+            float v = 0.f;
+#pragma unroll
+            for (int w = 0; w < 8; ++w) v += s_part[w * 2 * BN + i];
+            s_stats[which * p.N + n0 + c] += v;
+          }
+        }
+        consumer_sync();
       }
     }
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  if (warp == 1) tcgen05_dealloc(tmem_base, p.tmem_cols);
   if (p.stats) {
     double* st = p.stats + (long long)(blockIdx.x & (p.stats_repl - 1)) * 2 * p.N;
     for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) {
-      float v = s_stats[i];
-#if SGB_STATS_SLOTS > 1
-#pragma unroll
-      for (int q = 1; q < SGB_STATS_SLOTS; ++q) v += s_stats[q * 2 * p.N + i];  // fixed order
-#endif
+      const float v = s_stats[i];
       if (v != 0.f) atomicAdd(&st[i], (double)v);
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ wgrad kernel
-// dW[ko][(r,s,c)] += sum_pix dy[pix][ko] * x[pix @ (r,s)][c]       (fp32 atomics over pixel splits)
-// GEMM view: M = out-channels (TMEM lanes), N = in-channels of one tap (TMEM columns, one column range per tap),
-// K = pixels.  Both operands are "MN-major": a TMA box of [PIX pixels][channels] IS the canonical MN-major swizzled
-// layout (each K index is one swizzled row), so dy and the im2col'd x stream straight from NHWC memory with no
-// transpose.  One CTA = (64 x 128 out-channels) x (group of taps) x (c tile) x (pixel range).
+// dW[ko][(r,s,c)] += sum_pix dy[pix][ko] * x[pix @ (r,s)][c]       (fp32 reductions over pixel splits)
+// GEMM view: M = out-channels (64 per consumer warpgroup), N = NB in-channels of one tap, K = pixels.  Both operands are
+// "MN-major": a TMA box of [WPIX pixels][channels] IS the canonical MN-major swizzled layout (each K index is one swizzled
+// row), so dy and the im2col'd x stream straight from NHWC memory with no transpose.
+// One CTA = (128 out-channels) x (one tap) x (NB in-channels) x (pixel range).
 struct WParams {
   int K, C;            // out / in channels
   int R, S, stride, pad, P, Q;
   int npix;            // N*P*Q
-  int CB;              // in-channels per im2col box (32 or 64)
-  int c_tile;          // in-channels handled by one CTA
-  int tpg;             // taps per CTA (tap group)
-  int n_groups, n_ctiles, n_ktiles;
+  int CB;              // in-channels per im2col box (16 / 32 / 64)
+  int n_ctiles, n_ktiles;
   int pix_per_cta;     // multiple of WPIX
   int stages;
   int cpad;            // channel count of the KRSC output rows (x channels incl. padding)
   float* dw;
-  int tmem_cols;
-  int wide_n;  // 1: ONE MMA per (tap, 16 pixels) with N = c_tile spanning the tap's boxes (LBO = box size) instead of one per box
-  int dbg;  // SGB_DEBUG_SKIP (perf experiments): 1 no atomics, 4 no x loads, 8 no dy loads
 };
 constexpr int WPIX = 64;  // pixels (GEMM K) per pipeline stage
 
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr, int row_bytes, uint32_t lbo_bytes) {
-  // MN-major canonical layout: rows of row_bytes (= swizzle span: 128 / 64 / 32), 8-row groups along K
-  const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);
-  const uint32_t sbo = (uint32_t)(8 * row_bytes) >> 4;
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)(sbo & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
-}
-
+template <int NB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-wgrad_umma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WParams p) {
+wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WParams p) {
   SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_bytes = 2 * WPIX * 128;                       // two 64-channel blocks of dy
   const uint32_t b_box = WPIX * p.CB * 2;                        // one im2col box
-  const int boxes_per_tap = p.c_tile / p.CB;
-  const uint32_t b_bytes = (uint32_t)(p.tpg * boxes_per_tap) * b_box;
-  const uint32_t stage_bytes = a_bytes + b_bytes;                // multiples of 1024 by construction
+  const int boxes = NB / p.CB;
+  const uint32_t stage_bytes = a_bytes + (uint32_t)boxes * b_box;  // multiples of 1024 by construction
   const uint32_t ctrl = smem_base + p.stages * stage_bytes;
   auto full_bar = [&](int s) { return ctrl + 8u * s; };
   auto empty_bar = [&](int s) { return ctrl + 8u * (MAX_STAGES + s); };
-  const uint32_t done_bar = ctrl + 8u * (2 * MAX_STAGES);
-  const uint32_t tmem_slot = ctrl + 8u * (2 * MAX_STAGES + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // decode the CTA's work item
   int w = blockIdx.x;
   const int ktile = w % p.n_ktiles; w /= p.n_ktiles;
   const int ctile = w % p.n_ctiles; w /= p.n_ctiles;
-  const int group = w % p.n_groups; w /= p.n_groups;
+  const int tap = w % (p.R * p.S); w /= p.R * p.S;
   const int split = w;
-  const int tap0 = group * p.tpg;
-  const int ntaps = min(p.tpg, p.R * p.S - tap0);
   const int pix0 = split * p.pix_per_cta;
   const int pix1 = min(pix0 + p.pix_per_cta, p.npix);
   const int n_iters = (pix1 - pix0 + WPIX - 1) / WPIX;
@@ -479,138 +320,86 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_const
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);
     }
-    mbar_init(done_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tcgen05_alloc(tmem_slot, p.tmem_cols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory / TMEM
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (n_iters > 0) {
     if (warp == 0) {
       if (elect_one()) {
         const int pq = p.P * p.Q;
+        const int r = tap / p.S, s = tap - r * p.S;
         int stg = 0;
         uint32_t par = 1;
         for (int it = 0; it < n_iters; ++it) {
           mbar_wait(empty_bar(stg), par);
           const uint32_t sa = smem_base + stg * stage_bytes, sb = sa + a_bytes;
-          mbar_expect_tx(full_bar(stg), ((p.dbg & 8) ? 0u : a_bytes) + ((p.dbg & 4) ? 0u : (uint32_t)(ntaps * boxes_per_tap) * b_box) +
-                                            ((p.dbg & 12) == 12 ? 16u : 0u));
+          mbar_expect_tx(full_bar(stg), a_bytes + (uint32_t)boxes * b_box);
           const int pix = pix0 + it * WPIX;
-          if (!(p.dbg & 8)) {
-            tma_load_2d(sa, &map_dy, full_bar(stg), ktile * 128, pix);
-            tma_load_2d(sa + WPIX * 128, &map_dy, full_bar(stg), ktile * 128 + 64, pix);
-          }
-          if ((p.dbg & 12) == 12) {  // keep the barrier protocol alive with a 16-byte dummy transfer
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 16, [%2];" ::"r"(sa),
-                         "l"(p.dw), "r"(full_bar(stg))
-                         : "memory");
-          }
+          tma_load_2d(sa, &map_dy, full_bar(stg), ktile * 128, pix);
+          tma_load_2d(sa + WPIX * 128, &map_dy, full_bar(stg), ktile * 128 + 64, pix);
           const int n_img = pix / pq;
           const int rem = pix - n_img * pq;
           const int p0 = rem / p.Q, q0 = rem - p0 * p.Q;
           const int w0 = q0 * p.stride - p.pad, h0 = p0 * p.stride - p.pad;
-          for (int t = 0; t < ntaps; ++t) {
-            const int tap = tap0 + t, r = tap / p.S, s = tap - r * p.S;
-            for (int bx = 0; bx < boxes_per_tap && !(p.dbg & 4); ++bx)
-              tma_load_im2col_4d(sb + (uint32_t)(t * boxes_per_tap + bx) * b_box, &map_x, full_bar(stg),
-                                 ctile * p.c_tile + bx * p.CB, w0, h0, n_img, (uint16_t)s, (uint16_t)r);
-          }
+          for (int bx = 0; bx < boxes; ++bx)
+            tma_load_im2col_4d(sb + (uint32_t)bx * b_box, &map_x, full_bar(stg), ctile * NB + bx * p.CB, w0, h0, n_img, (uint16_t)s,
+                               (uint16_t)r);
           if (++stg == p.stages) {
             stg = 0;
             par ^= 1;
           }
         }
       }
-    } else if (warp == 1) {
-      // A and B are MN-major: a_major (bit 15) and b_major (bit 16) set; M = 128, N = CB
-      const uint32_t leader = elect_one() ? 1u : 0u;
-      // wide_n: the tap's boxes are consecutive N atoms of ONE operand (leading-dimension byte offset = box size), so a tap costs
-      // WPIX / 16 MMAs of N = c_tile instead of boxes_per_tap times as many of N = CB (N = 16 / 32 MMAs are issue-bound)
-      // An M = 128, K = 16 MMA reads 4 KB of A from shared memory whatever its N: with N = 16 .. 48 the tensor pipe waits on the operand
-      // port (measured: 62 clocks per N = 48 MMA).  So one MMA covers as many boxes as 256 columns hold -- across TAPS too: box a of
-      // the stage (a = tap * boxes_per_tap + box) sits at a * b_box in shared memory and owns TMEM columns [a * CB, (a + 1) * CB).
-      const int n_atoms = p.wide_n ? ntaps * boxes_per_tap : 0;
-      const int apm = 256 / p.CB;  // boxes per MMA
-      const uint32_t idesc_base = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t idesc = idesc_base | ((uint32_t)(p.CB >> 3) << 17);
+    } else if (warp >= 4) {
+      const int wg = (warp >> 2) - 1, wq = warp & 3;
       const int b_row_bytes = p.CB * 2;
-      const uint64_t a_hi = make_smem_desc_mn(0, 128, WPIX * 128), b_hi = make_smem_desc_mn(0, b_row_bytes, p.wide_n ? b_box : 0u);
-      int stg = 0;
+      float acc[NB / 2];
+      int stg = 0, prev = -1;
       uint32_t par = 0;
       for (int it = 0; it < n_iters; ++it) {
         mbar_wait(full_bar(stg), par);
-        tcgen05_fence_after();
-        const uint32_t sa = (smem_base + stg * stage_bytes) >> 4, sb = sa + (a_bytes >> 4);
-        if (p.wide_n) {
-          for (int a0 = 0; a0 < n_atoms; a0 += apm) {
-            const int na = min(apm, n_atoms - a0);
-            const uint32_t idesc_w = idesc_base | ((uint32_t)((na * p.CB) >> 3) << 17);
-            const uint32_t sbox = sb + (((uint32_t)a0 * b_box) >> 4);
-            const uint32_t d_tmem = tmem_base + (uint32_t)(a0 * p.CB);
+        const uint32_t sa = smem_base + stg * stage_bytes + (uint32_t)wg * (WPIX * 128), sb = smem_base + stg * stage_bytes + a_bytes;
+        wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < WPIX / 16; ++j) {
-              const uint64_t da = a_hi | (uint64_t)((sa + ((j * 16 * 128) >> 4)) & 0x3fff);
-              const uint64_t db = b_hi | (uint64_t)((sbox + (uint32_t)((j * 16 * b_row_bytes) >> 4)) & 0x3fff);
-              umma_bf16_if(leader, d_tmem, da, db, idesc_w, (it | j) != 0);
-            }
-          }
-        } else {
-          for (int t = 0; t < ntaps; ++t)
-            for (int bx = 0; bx < boxes_per_tap; ++bx) {
-              const uint32_t sbox = sb + (((uint32_t)(t * boxes_per_tap + bx) * b_box) >> 4);
-              const uint32_t d_tmem = tmem_base + (uint32_t)(t * p.c_tile + bx * p.CB);
-#pragma unroll
-              for (int j = 0; j < WPIX / 16; ++j) {
-                const uint64_t da = a_hi | (uint64_t)((sa + ((j * 16 * 128) >> 4)) & 0x3fff);
-                const uint64_t db = b_hi | (uint64_t)((sbox + (uint32_t)((j * 16 * b_row_bytes) >> 4)) & 0x3fff);
-                umma_bf16_if(leader, d_tmem, da, db, idesc, (it | j) != 0);
-              }
-            }
+        for (int j = 0; j < WPIX / 16; ++j) {
+          // A: one 64-channel atom of 128-byte pixel rows; B: the boxes are consecutive MN atoms (LBO = box size)
+          const uint64_t da = smem_desc(sa + (uint32_t)j * 16u * 128u, 128, WPIX * 128, 8 * 128);
+          const uint64_t db = smem_desc(sb + (uint32_t)j * 16u * (uint32_t)b_row_bytes, b_row_bytes, b_box, 8u * (uint32_t)b_row_bytes);
+          mma_mn<NB>(acc, da, db, (it | j) != 0);
         }
-        umma_commit_if(leader, empty_bar(stg));
-        if (it == n_iters - 1) umma_commit_if(leader, done_bar);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(prev));
+        }
+        prev = stg;
         if (++stg == p.stages) {
           stg = 0;
           par ^= 1;
         }
       }
-    } else {
-      const int quarter = warp & 3;
-      mbar_wait(done_bar, 0);
-      tcgen05_fence_after();
-      const int ko = ktile * 128 + quarter * 32 + lane;
+      wgmma_wait<0>();
+      fence_regs(acc);
       const int row_len = p.R * p.S * p.cpad;
-      float* drow = p.dw + (long long)ko * row_len;
-      for (int t = 0; t < ntaps; ++t) {
-        const int tap = tap0 + t;
-        for (int c0 = 0; c0 < p.c_tile; c0 += 16) {
-          float v[16];
-          tmem_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(t * p.c_tile + c0), v);
-          if (ko < p.K && !(p.dbg & 1)) {
-            float* dst = drow + tap * p.cpad + ctile * p.c_tile + c0;  // 64-byte aligned: cpad, c_tile, c0 are multiples of 16
 #pragma unroll
-            for (int i = 0; i < 16; i += 4)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + i), "f"(v[i]), "f"(v[i + 1]), "f"(v[i + 2]),
-                           "f"(v[i + 3])
-                           : "memory");
-          }
+      for (int h = 0; h < 2; ++h) {
+        const int ko = ktile * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        if (ko < p.K) {
+          float* drow = p.dw + (long long)ko * row_len + tap * p.cpad + ctile * NB + 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < NB / 8; ++j)
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(drow + 8 * j), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1])
+                         : "memory");
         }
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  if (warp == 1) tcgen05_dealloc(tmem_base, p.tmem_cols);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -619,9 +408,6 @@ EncodeIm2colFn g_im2col = nullptr;
 int g_num_sms = 0;
 long long g_launches = 0;
 long long launch_count() { return g_launches; }
-int read_trace(long long* host_out) {
-  return sgb_cuda_check(cudaMemcpyFromSymbol(host_out, g_trace, sizeof(long long) * 12 * 512), "cudaMemcpyFromSymbol(g_trace)");
-}
 
 int init_driver() {
   if (g_tiled && g_im2col) return SGB_OK;
@@ -648,17 +434,6 @@ CUtensorMapSwizzle swizzle_for(int kc) {
   return kc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (kc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-long long* trace_buffer() {
-  void* ptr = nullptr;
-  cudaGetSymbolAddress(&ptr, g_trace);
-  return reinterpret_cast<long long*>(ptr);
-}
-
-int debug_skip_mask() {
-  const char* e = getenv("SGB_DEBUG_SKIP");
-  return e ? atoi(e) : 0;
-}
-
 bool enabled() {
   static int v = -1;
   if (v < 0) {
@@ -680,42 +455,65 @@ bool supported(const Problem& q) {
   return true;
 }
 
+namespace {
+
+// kernel variant of one N tile width + its register footprint (decides how many CTAs can share an SM)
+template <class Fn>
+struct Variant {
+  int bn;
+  Fn fn;
+  int regs;
+  bool ready;
+};
+typedef void (*ConvFn)(const CUtensorMap, const CUtensorMap, const Params);
+typedef void (*WgradFn)(const CUtensorMap, const CUtensorMap, const WParams);
+Variant<ConvFn> g_conv[] = {{16, conv_wgmma_kernel<16>, 0, false},   {32, conv_wgmma_kernel<32>, 0, false},
+                            {48, conv_wgmma_kernel<48>, 0, false},   {64, conv_wgmma_kernel<64>, 0, false},
+                            {96, conv_wgmma_kernel<96>, 0, false},   {128, conv_wgmma_kernel<128>, 0, false}};
+Variant<WgradFn> g_wgrad[] = {{16, wgrad_wgmma_kernel<16>, 0, false}, {32, wgrad_wgmma_kernel<32>, 0, false},
+                              {48, wgrad_wgmma_kernel<48>, 0, false}, {64, wgrad_wgmma_kernel<64>, 0, false},
+                              {96, wgrad_wgmma_kernel<96>, 0, false}, {128, wgrad_wgmma_kernel<128>, 0, false}};
+
+template <class Fn>
+int prepare(Variant<Fn>& v, const char* what) {
+  if (v.ready) return SGB_OK;
+  if (int rc = sgb_cuda_check(cudaFuncSetAttribute(v.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), what)) return rc;
+  cudaFuncAttributes fa{};
+  if (int rc = sgb_cuda_check(cudaFuncGetAttributes(&fa, v.fn), what)) return rc;
+  v.regs = fa.numRegs;
+  v.ready = true;
+  return SGB_OK;
+}
+
+// N tile: the narrowest variant that holds N in one tile, else the widest of 128 / 96 / 64 with the least padding
+int pick_bn(int n) {
+  for (int bn : {16, 32, 48, 64, 96, 128})
+    if (n <= bn) return bn;
+  int best = 128, best_waste = (n + 127) / 128 * 128 - n;
+  for (int bn : {96, 64}) {
+    const int waste = (n + bn - 1) / bn * bn - n;
+    if (waste < best_waste) { best_waste = waste; best = bn; }
+  }
+  return best;
+}
+
+}  // namespace
+
 int launch(const Problem& q, cudaStream_t st) {
-  if (halo_supported(q)) return halo_launch(q, st);
   if (int rc = init_driver()) return rc;
   Params p{};
   p.M = q.N * q.P * q.Q;
   p.N = q.b_rows;
   p.C = q.C;
-  p.R = q.R;
-  p.S = q.S;
   p.KC = q.C % 64 == 0 ? 64 : (q.C % 32 == 0 ? 32 : 16);
-  {
-    // Few channels per k-iteration make the pipeline latency-bound (one mbarrier round trip per 4-8 KB of A): with 48 / 96 / 288
-    // channels use 64-channel boxes anyway -- the channels past C are zero-filled by TMA's bounds check (the matching B columns
-    // belong to the next tap or are out of bounds: finite x 0), so C = 48 runs 1 k-iteration per tap instead of 3 and C = 96 runs 2
-    // instead of 3, at the price of some zero MMA work.  SGB_UMMA_KC_PAD=0 restores exact chunks.
-    static int kc_pad = -1;
-    if (kc_pad < 0) {
-      const char* e = getenv("SGB_UMMA_KC_PAD");
-      kc_pad = (e && e[0] == '0') ? 0 : 1;
-    }
-    if (kc_pad && p.KC < 64 && q.C > 32) p.KC = 64;
-  }
-  // N tile: whole N when it fits one accumulator, else the divisor-friendly size with least padding
-  int bn;
-  if (p.N <= 256) {
-    bn = ((p.N + 15) / 16) * 16;
-  } else {
-    bn = 256;
-    int best_waste = ((p.N + 255) / 256) * 256 - p.N;
-    for (int cand = 240; cand >= 128; cand -= 16) {
-      int waste = ((p.N + cand - 1) / cand) * cand - p.N;
-      if (waste < best_waste) { best_waste = waste; bn = cand; }
-    }
-  }
-  p.BN = bn;
-  p.P = q.P; p.Q = q.Q; p.stride = q.stride; p.pad = q.pad; p.flip = q.flip;
+  // Few channels per k-iteration make the pipeline latency-bound (one mbarrier round trip per 4-8 KB of A): with 48 / 96 / 288
+  // channels use 64-channel boxes anyway -- the channels past C are zero-filled by TMA's bounds check (the matching B columns
+  // belong to the next tap or are out of bounds: finite x 0), so C = 48 runs 1 k-iteration per tap instead of 3 and C = 96 runs 2
+  // instead of 3, at the price of some zero MMA work.
+  if (p.KC < 64 && q.C > 32) p.KC = 64;
+  const int bn = pick_bn(p.N);
+  p.n_tiles = (p.N + bn - 1) / bn;
+  p.P = q.P; p.Q = q.Q; p.stride = q.stride; p.pad = q.pad;
   if (q.ntaps > 0) {
     p.ntaps = q.ntaps;
     for (int t = 0; t < q.ntaps; ++t) { p.tap_dh[t] = (signed char)q.tap_dh[t]; p.tap_dw[t] = (signed char)q.tap_dw[t]; p.tap_b[t] = (signed char)q.tap_b[t]; }
@@ -727,79 +525,33 @@ int launch(const Problem& q, cudaStream_t st) {
       p.tap_b[t] = (signed char)(q.flip ? (p.ntaps - 1 - t) : t);
     }
   }
+  if (p.ntaps > 9) return SGB_E_UNSUPPORTED;
   p.out_mode = q.out_mode; p.o_mul = q.o_mul; p.oh_add = q.oh_add; p.ow_add = q.ow_add; p.outH = q.outH; p.outW = q.outW;
   p.b_cols_per_tap = q.b_cols_per_tap;
   p.y = (bf16*)q.y; p.y_pitch = q.y_pitch; p.y_off = q.y_off;
   p.scale = q.scale; p.shift = q.shift; p.residual = (const bf16*)q.residual;
   p.stats = q.stats; p.stats_repl = q.stats_repl > 0 ? q.stats_repl : 1; p.act = q.act;
-  {
-    const char* e = getenv("SGB_DEBUG_SKIP");
-    p.dbg = e ? atoi(e) : 0;
-  }
-  int tc = 32;
-  while (tc < 2 * bn) tc <<= 1;
-  p.tmem_cols = tc;
-  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M, n_tiles = (p.N + bn - 1) / bn;
-  const bool plain = !p.scale && !p.shift && !p.residual && p.act == SGB_ACT_NONE && n_tiles == 1 && p.N == bn && !(p.dbg & 2);
-  if (p.ntaps > 9) return SGB_E_UNSUPPORTED;
-  const int nch = plain ? bn / 16 : 0;
-  const bool stats = p.stats != nullptr;
-  // kernel variant + its register footprint (decides how many CTAs can share an SM)
-  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const Params);
-  struct Variant { KernelFn fn; int regs; bool ready; };
-  static Variant variants[9] = {
-      {conv_umma_kernel<0, false>, 0, false}, {conv_umma_kernel<2, false>, 0, false}, {conv_umma_kernel<2, true>, 0, false},
-      {conv_umma_kernel<3, false>, 0, false}, {conv_umma_kernel<3, true>, 0, false},  {conv_umma_kernel<4, false>, 0, false},
-      {conv_umma_kernel<4, true>, 0, false},  {conv_umma_kernel<6, false>, 0, false}, {conv_umma_kernel<6, true>, 0, false}};
-  int vi = 0;
-  if (nch == 2) vi = stats ? 2 : 1;
-  else if (nch == 3) vi = stats ? 4 : 3;
-  else if (nch == 4) vi = stats ? 6 : 5;
-  else if (nch == 6) vi = stats ? 8 : 7;
-  Variant& var = variants[vi];
-  if (!var.ready) {
-    if (int rc = sgb_cuda_check(cudaFuncSetAttribute(var.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
-                                "cudaFuncSetAttribute(conv_umma_kernel)"))
-      return rc;
-    cudaFuncAttributes fa{};
-    if (int rc = sgb_cuda_check(cudaFuncGetAttributes(&fa, var.fn), "cudaFuncGetAttributes(conv_umma_kernel)")) return rc;
-    var.regs = fa.numRegs;
-    var.ready = true;
-  }
-  // A CTA's pipeline is latency-bound when its k-iterations are small (few channels per tap): co-resident CTAs overlap
-  // each other's TMA / MMA / epilogue chains.  Limits: TMEM columns (512 per SM), registers (64K per SM), shared memory.
-  const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = bn * p.KC * 2;
-  p.b_tile_bytes = (b_bytes + 1023u) & ~1023u;
-  const uint32_t bres_all = (uint32_t)(p.ntaps * ((p.C + p.KC - 1) / p.KC)) * p.b_tile_bytes;
-  {
-    static int bres_on = -1, bres_min = 4;
-    if (bres_on < 0) {
-      const char* e = getenv("SGB_UMMA_B_RESIDENT");
-      bres_on = (e && e[0] == '0') ? 0 : 1;
-      const char* m = getenv("SGB_UMMA_B_RESIDENT_MINTILES");  // tiles per SM from which the one-off filter load pays
-      if (m && atoi(m) > 0) bres_min = atoi(m);
-    }
-    // worth it when every CTA walks many tiles (the filter load is amortised) and the filter leaves room for a deep A ring
-    p.b_resident = (bres_on && n_tiles == 1 && bres_all <= 112u * 1024u && m_tiles >= bres_min * g_num_sms && 2 * b_bytes >= a_bytes) ? 1 : 0;  // BN >= 64: narrow filters gain nothing (measured)
-  }
-  const uint32_t stage_bytes = a_bytes + (p.b_resident ? 0u : p.b_tile_bytes);
-  const uint32_t ctrl_bytes = 8 * (2 * MAX_STAGES + 4) + 16 + SGB_STATS_SLOTS * 2 * p.N * 4 + 64 + (p.b_resident ? bres_all : 0u);
-  int ctas_per_sm = 3;
-  {
-    const char* e = getenv("SGB_CTAS_PER_SM");
-    if (e) ctas_per_sm = atoi(e);
-    if (ctas_per_sm < 1) ctas_per_sm = 1;
-  }
-  const int regs_alloc = ((var.regs + 7) / 8) * 8 * NUM_THREADS;
-  while (ctas_per_sm > 1 && (ctas_per_sm * tc > 512 || ctas_per_sm * regs_alloc > 65536)) --ctas_per_sm;
+  Variant<ConvFn>* var = nullptr;
+  for (auto& v : g_conv)
+    if (v.bn == bn) var = &v;
+  if (int rc = prepare(*var, "conv_wgmma_kernel")) return rc;
+  // Small tiles leave the pipeline latency-bound: co-resident CTAs overlap each other's loads, MMAs and epilogues.
+  // Limits: registers (64K per SM) and shared memory (228 KB per SM, 227 KB per CTA).
+  const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = ((uint32_t)(bn * p.KC * 2) + 1023u) & ~1023u;
+  const uint32_t stage_bytes = a_bytes + b_bytes;
+  const uint32_t ctrl_bytes = CTRL_BAR_BYTES + (p.stats ? (uint32_t)(8 * 2 * bn + 2 * p.N) * 4u : 0u);
+  const int regs_alloc = ((var->regs + 7) / 8) * 8 * NUM_THREADS;
+  int ctas_per_sm = 65536 / regs_alloc;
+  if (ctas_per_sm > 2) ctas_per_sm = 2;
+  if (ctas_per_sm < 1) ctas_per_sm = 1;
   int stages = 0;
   for (;; --ctas_per_sm) {
-    const uint32_t budget = (ctas_per_sm == 1 ? 200u : 224u / ctas_per_sm - 2u) * 1024u;
+    const uint32_t budget = (ctas_per_sm == 1 ? 226u : 227u / ctas_per_sm - 1u) * 1024u;
     stages = budget > ctrl_bytes + 1024 ? (int)((budget - ctrl_bytes - 1024) / stage_bytes) : 0;
-    if (stages > 8) stages = 8;
+    if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages >= 4 || ctas_per_sm == 1) break;
   }
-  if (stages < 2) { sgb_set_error("conv_sm100: tile does not fit shared memory"); return SGB_E_UNSUPPORTED; }
+  if (stages < 2) { sgb_set_error("conv_wgmma: tile does not fit shared memory"); return SGB_E_UNSUPPORTED; }
   p.stages = stages;
   const size_t smem = 1024 + (size_t)stages * stage_bytes + ctrl_bytes;
 
@@ -837,11 +589,12 @@ int launch(const Problem& q, cudaStream_t st) {
       return SGB_E_CUDA;
     }
   }
-  int grid = m_tiles * n_tiles;
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  int grid = m_tiles * p.n_tiles;
   if (grid > g_num_sms * ctas_per_sm) grid = g_num_sms * ctas_per_sm;
-  SGB_LAUNCH(var.fn, grid, NUM_THREADS, smem, st, map_a, map_b, p);
+  SGB_LAUNCH(var->fn, grid, NUM_THREADS, smem, st, map_a, map_b, p);
   ++g_launches;
-  return sgb_cuda_check(cudaGetLastError(), "conv_umma_kernel");
+  return sgb_cuda_check(cudaGetLastError(), "conv_wgmma_kernel");
 }
 
 bool wgrad_supported(const WgradProblem& q) {
@@ -856,50 +609,31 @@ bool wgrad_supported(const WgradProblem& q) {
 }
 
 int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
-  if (wgrad_halo_supported(q)) return wgrad_halo_launch(q, st);
   if (int rc = init_driver()) return rc;
   WParams p{};
   p.K = q.K; p.C = q.C; p.R = q.R; p.S = q.S; p.stride = q.stride; p.pad = q.pad; p.P = q.P; p.Q = q.Q;
   p.npix = q.N * q.P * q.Q;
-  p.CB = q.C % 64 == 0 ? 64 : (q.C % 32 == 0 ? 32 : 16);
-  p.c_tile = q.C <= 512 ? q.C : 256;
-  if (q.C % p.c_tile != 0) p.c_tile = p.CB;
-  const int taps = q.R * q.S;
-  int tpg = 512 / p.c_tile;
-  if (tpg < 1) tpg = 1;
-  if (tpg > taps) tpg = taps;
-  p.n_groups = (taps + tpg - 1) / tpg;
-  p.tpg = (taps + p.n_groups - 1) / p.n_groups;
-  p.n_ctiles = q.C / p.c_tile;
+  // in-channels per CTA: the widest variant that divides C; boxes as wide as the swizzle allows
+  int nb = 16;
+  for (int cand : {128, 96, 64, 48, 32})
+    if (q.C % cand == 0) { nb = cand; break; }
+  p.CB = nb % 64 == 0 ? 64 : (nb % 32 == 0 ? 32 : 16);
+  p.n_ctiles = q.C / nb;
   p.n_ktiles = (q.K + 127) / 128;
   p.cpad = q.C;
   p.dw = q.dw;
-  {
-    const char* e = getenv("SGB_DEBUG_SKIP");
-    p.dbg = e ? atoi(e) : 0;
-  }
-  int tc = 32;
-  while (tc < p.tpg * p.c_tile) tc <<= 1;
-  p.tmem_cols = tc;
-  {
-    static int wide = -1;
-    if (wide < 0) {
-      const char* e = getenv("SGB_WGRAD_WIDE_N");
-      wide = (e && e[0] == '0') ? 0 : 1;
-    }
-    p.wide_n = (wide && p.tpg * (p.c_tile / p.CB) > 1) ? 1 : 0;  // more than one box per stage
-  }
-  const uint32_t a_bytes = 2 * WPIX * 128;
-  const uint32_t b_bytes = (uint32_t)p.tpg * (p.c_tile / p.CB) * WPIX * p.CB * 2;
-  const uint32_t stage_bytes = a_bytes + b_bytes;
-  const uint32_t ctrl_bytes = 8 * (2 * MAX_STAGES + 2) + 64;
-  int stages = (int)((200 * 1024 - ctrl_bytes - 1024) / stage_bytes);
+  Variant<WgradFn>* var = nullptr;
+  for (auto& v : g_wgrad)
+    if (v.bn == nb) var = &v;
+  if (int rc = prepare(*var, "wgrad_wgmma_kernel")) return rc;
+  const uint32_t stage_bytes = 2 * WPIX * 128 + (uint32_t)(nb / p.CB) * WPIX * p.CB * 2;
+  int stages = (int)((200 * 1024 - CTRL_BAR_BYTES - 1024) / stage_bytes);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) return SGB_E_UNSUPPORTED;
   p.stages = stages;
-  const size_t smem = 1024 + (size_t)stages * stage_bytes + ctrl_bytes;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + CTRL_BAR_BYTES;
   // pixel splits: fill ~2 waves of SMs, keep at least 8 pipeline iterations per CTA
-  const int base_ctas = p.n_ktiles * p.n_ctiles * p.n_groups;
+  const int base_ctas = p.n_ktiles * p.n_ctiles * q.R * q.S;
   const int total_iters = (p.npix + WPIX - 1) / WPIX;
   int splits = (2 * g_num_sms + base_ctas - 1) / base_ctas;
   if (splits > total_iters / 8) splits = total_iters / 8;
@@ -931,17 +665,10 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { sgb_set_error("cuTensorMapEncodeIm2col(x, wgrad) failed with %d", (int)r); return SGB_E_CUDA; }
   }
-  static bool attr = false;
-  if (!attr) {
-    if (int rc = sgb_cuda_check(cudaFuncSetAttribute(wgrad_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
-                                "cudaFuncSetAttribute(wgrad_umma_kernel)"))
-      return rc;
-    attr = true;
-  }
   const int grid = base_ctas * splits;
-  SGB_LAUNCH(wgrad_umma_kernel, grid, NUM_THREADS, smem, st, map_dy, map_x, p);
+  SGB_LAUNCH(var->fn, grid, NUM_THREADS, smem, st, map_dy, map_x, p);
   ++g_launches;
-  return sgb_cuda_check(cudaGetLastError(), "wgrad_umma_kernel");
+  return sgb_cuda_check(cudaGetLastError(), "wgrad_wgmma_kernel");
 }
 
 }  // namespace sm100

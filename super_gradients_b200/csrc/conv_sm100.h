@@ -41,6 +41,5 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st);
 bool supported(const Problem& q);
 int launch(const Problem& q, cudaStream_t st);
 long long launch_count();
-int read_trace(long long* host_out);  // 12 x 512 SM-clock stamps of the last SGB_DEBUG_SKIP&16 launch
 
 }  // namespace sm100

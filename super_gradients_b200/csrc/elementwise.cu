@@ -44,7 +44,7 @@ __device__ __forceinline__ void st8(bf16* p, const V8& a) {
   *reinterpret_cast<uint4*>(p) = r;
 }
 
-inline int grid_for(int64_t work, int per_cta = TPB, int max_ctas = 148 * 8) {
+inline int grid_for(int64_t work, int per_cta = TPB, int max_ctas = 132 * 8) {
   int64_t g = (work + per_cta - 1) / per_cta;
   if (g > max_ctas) g = max_ctas;
   if (g < 1) g = 1;
@@ -484,7 +484,7 @@ int launch_chan_reduce(F f, int64_t M, int C, double* out, int out_stride, cudaS
     per_sm = n;
   }
   int64_t want = (M + 255) / 256;  // >= 256 pixels per CTA
-  int64_t cap = (int64_t)148 * per_sm;
+  int64_t cap = (int64_t)132 * per_sm;
   if (cap > sgb_chan_grid_cap()) cap = sgb_chan_grid_cap();
   int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
   (void)cvb;

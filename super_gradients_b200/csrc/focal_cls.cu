@@ -40,7 +40,7 @@ extern "C" int sgb_focal_cls_fwd_bwd(const SgbLossDesc* d, const float* cls_logi
   cudaStream_t st = (cudaStream_t)stream;
   cudaMemsetAsync(sums, 0, sizeof(double), st);  // drop the varifocal sum the fused kernel left in sums[0]
   const int64_t total = (int64_t)d->B * d->L * d->ncls;
-  const int grid = (int)((total + 255) / 256 > 148 * 8 ? 148 * 8 : (total + 255) / 256);
+  const int grid = (int)((total + 255) / 256 > 132 * 8 ? 132 * 8 : (total + 255) / 256);
   focal_cls_kernel<<<grid, 256, 0, st>>>(*d, cls_logits, assigned_label, assigned_score, sums, grad_scale, alpha, grad_cls);
   SGB_LAUNCH_CHECK("focal_cls_kernel");
   return SGB_OK;

@@ -643,7 +643,7 @@ extern "C" int sgb_dfl_decode(const sgb_bf16* reg, int reg_pitch, const sgb_bf16
     }
   }
   int64_t total = (int64_t)N * Hf * Wf * (4 + ncls);
-  int grid = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  int grid = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
   dfl_decode_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const bf16*)reg, reg_pitch, (const bf16*)cls, cls_pitch, N,
                                                             Hf, Wf, L, anchor_base, ncls, reg_max, stride, cell_offset,
                                                             pred_bboxes, pred_scores, cls_logits, reg_distri);
@@ -660,7 +660,7 @@ extern "C" int sgb_pose_keypoint_decode(const sgb_bf16* pose, int pose_pitch, co
   SGB_REQUIRE(pose_pitch >= 2 * J && logit_pitch >= logit_off + J && logit_off >= 0, "channel range exceeds pitch");
   SGB_REQUIRE(anchor_base >= 0 && anchor_base + Hf * Wf <= L, "anchor range");
   int64_t total = (int64_t)N * Hf * Wf * J;
-  int grid = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  int grid = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
   pose_keypoint_decode_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       (const bf16*)pose, pose_pitch, (const bf16*)logit, logit_pitch, logit_off, N, Hf, Wf, L, anchor_base, J, stride, cell_offset,
       offset_multiplier, compensate_grid_cell_offset ? cell_offset : 0.f, pose_coords, pose_scores, pose_logits);
@@ -675,13 +675,13 @@ extern "C" int sgb_head_grad_scatter(const float* grad, int gC, int N, int HW, i
   if (cpad > pitch) cpad = pitch;
   if (pitch % 8 == 0 && cpad % 8 == 0 && (uintptr_t)dy % 16 == 0 && (uintptr_t)grad % 16 == 0 && (int64_t)N * HW * (cpad / 8) < (1ll << 31)) {
     const uint32_t tot = (uint32_t)((int64_t)N * HW * (cpad / 8));
-    const int grid8 = (int)((tot + 255u) / 256u > 148u * 16u ? 148u * 16u : (tot + 255u) / 256u);
+    const int grid8 = (int)((tot + 255u) / 256u > 132u * 16u ? 132u * 16u : (tot + 255u) / 256u);
     head_grad_scatter_v8_kernel<<<grid8 < 1 ? 1 : grid8, 256, 0, (cudaStream_t)stream>>>(grad, gC, HW, L, anchor_base, (bf16*)dy, pitch, cpad / 8, tot);
     SGB_LAUNCH_CHECK("head_grad_scatter_v8_kernel");
     return SGB_OK;
   }
   int64_t total = (int64_t)N * HW * cpad;
-  int grid = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  int grid = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
   head_grad_scatter_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(grad, gC, N, HW, L, anchor_base, (bf16*)dy, pitch,
                                                                    cpad);
   SGB_LAUNCH_CHECK("head_grad_scatter_kernel");
@@ -708,7 +708,7 @@ extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, con
   const int nmax = d->n_max > 0 ? d->n_max : 1;
   TalWs w = tal_ws_carve(workspace, d->B, d->L, nmax, d->topk);
   const int64_t BL = (int64_t)d->B * d->L;
-  int grid = (int)((BL + 255) / 256 > 148 * 8 ? 148 * 8 : (BL + 255) / 256);
+  int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
   tal_decode_kernel<<<grid, 256, 0, st>>>(*d, reg_distri, anchor_points, stride_tensor, w.pbox);
   SGB_LAUNCH_CHECK("tal_decode_kernel");
   if (d->n_max > 0) {
@@ -751,7 +751,7 @@ extern "C" int sgb_dfl_iou_loss_fwd_bwd(const SgbLossDesc* d, const float* cls_l
   const int64_t BL = (int64_t)d->B * d->L;
   int64_t warps_per_cta = 8;
   int64_t want = (BL + warps_per_cta - 1) / warps_per_cta;
-  int grid = (int)(want > 148 * 8 ? 148 * 8 : want);
+  int grid = (int)(want > 132 * 8 ? 132 * 8 : want);
   loss_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(*d, cls_logits, reg_distri, anchor_points, stride_tensor,
                                                       assigned_label, assigned_box, assigned_score, sums, grad_scale,
                                                       grad_cls, grad_reg);

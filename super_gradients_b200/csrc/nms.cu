@@ -331,7 +331,7 @@ __global__ void __launch_bounds__(NT, 2) nms_prefilter_kernel(SgbNmsDesc d, cons
 }
 
 // Split form of the per-image work for large candidate counts.  With ~1000 candidates the IoU bit-matrix is 500 k IoU evaluations
-// (fp32 division each) and dominated the one-CTA-per-image kernel (32 CTAs on 148 SMs); it is the only part with no sequential
+// (fp32 division each) and dominated the one-CTA-per-image kernel (32 CTAs on 132 SMs); it is the only part with no sequential
 // dependence, so it runs as its own launch over (row block, image) CTAs between a "front" launch (selection, sort, gather, offsets,
 // areas -> NmsStage in global memory) and a "back" launch (greedy sweep over the matrix + output rows).  Same arithmetic, same
 // order of operations per IoU.
@@ -654,7 +654,7 @@ extern "C" int sgb_batched_nms(const SgbNmsDesc* d, const float* boxes, const fl
     conf = reinterpret_cast<float*>(workspace);
     lab = reinterpret_cast<int*>(conf + (int64_t)d->B * d->L);
     int64_t rows = (int64_t)d->B * d->L;
-    int grid = (int)((rows + 255) / 256 > 148 * 8 ? 148 * 8 : (rows + 255) / 256);
+    int grid = (int)((rows + 255) / 256 > 132 * 8 ? 132 * 8 : (rows + 255) / 256);
     nms_argmax_kernel<<<grid, 256, 0, st>>>(scores, rows, d->ncls, conf, lab);
     SGB_LAUNCH_CHECK("nms_argmax_kernel");
   }

@@ -245,7 +245,7 @@ extern "C" int sgb_pose_tal_assign(const SgbPoseLossDesc* d, const float* cls_lo
   SGB_REQUIRE(d->n_max > 0 ? (gt_boxes && gt_poses && gt_crowd && gt_valid) : true, "gt pointers");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t BL = (int64_t)d->B * d->L;
-  const int grid = (int)((BL + 255) / 256 > 148 * 8 ? 148 * 8 : (BL + 255) / 256);
+  const int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
   if (d->n_max == 0) {  // no targets in the batch: every anchor is background (:118-131)
     fill_assign_kernel<<<grid, 256, 0, st>>>(assigned_gt, assigned_score, BL);
     SGB_LAUNCH_CHECK("fill_assign_kernel");
@@ -289,7 +289,7 @@ extern "C" int sgb_pose_loss_fwd_bwd(const SgbPoseLossDesc* d, const float* cls_
   if (grad_reg) cudaMemsetAsync(grad_reg, 0, BL * 4 * (d->reg_max + 1) * sizeof(float), st);
   if (grad_pose) cudaMemsetAsync(grad_pose, 0, BL * d->J * 2 * sizeof(float), st);
   if (grad_pose_logits) cudaMemsetAsync(grad_pose_logits, 0, BL * d->J * sizeof(float), st);
-  const int grid = (int)((BL + 255) / 256 > 148 * 8 ? 148 * 8 : (BL + 255) / 256);
+  const int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
   pose_loss_kernel<<<grid, 256, 0, st>>>(*d, cls_logits, reg_distri, pose_coords, pose_logits, anchor_points, stride_tensor,
                                          gt_boxes, gt_poses, sigmas, assigned_gt, assigned_score, sums, grad_scale, grad_cls,
                                          grad_reg, grad_pose, grad_pose_logits);

@@ -29,7 +29,7 @@ extern "C" int sgb_preprocess_u8(const SgbPreprocDesc* d, const uint8_t* src, sg
               "the resized image must fit the padded canvas");
   SGB_REQUIRE(d->out_pitch >= d->src_c, "output channel pitch");
   const int64_t total = (int64_t)d->out_h * d->out_w;
-  const int grid = (int)((total + 255) / 256 > 148 * 8 ? 148 * 8 : (total + 255) / 256);
+  const int grid = (int)((total + 255) / 256 > 132 * 8 ? 132 * 8 : (total + 255) / 256);
   preprocess_u8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(*d, src, (bf16*)out);
   SGB_LAUNCH_CHECK("preprocess_u8_kernel");
   return SGB_OK;

@@ -1,16 +1,6 @@
-// Host-side state shared by the tcgen05 / TMA translation units: the driver's tensor-map encoders (resolved through
+// Host-side state of the wgmma / TMA convolution kernels: the driver's tensor-map encoders (resolved through
 // cudaGetDriverEntryPoint, so the library has no link-time dependency on libcuda), the SM count and the launch counter.
 #pragma once
-
-// Per-CTA BatchNorm-statistics partials in shared memory.  Default (1 slot): the four epilogue warps add their fp32 partials
-// with shared-memory atomics -- their arrival order is not fixed, so the partial (and with it mean / rstd, in the last fp32
-// bit) can differ between two runs of the same problem.  -DSGB_DETERMINISTIC_STATS gives every epilogue warp its own slot
-// and sums the four slots in a fixed order (bit-reproducible per CTA; costs 3x the statistics' shared memory).
-#ifdef SGB_DETERMINISTIC_STATS
-#define SGB_STATS_SLOTS 4
-#else
-#define SGB_STATS_SLOTS 1
-#endif
 
 #include <cuda.h>
 
@@ -29,15 +19,5 @@ extern long long g_launches;
 
 int init_driver();                          // SGB_OK or an error code (message in sgb_last_error)
 CUtensorMapSwizzle swizzle_for(int kc);     // 64 / 32 / 16 bf16 channels per row -> 128B / 64B / 32B swizzle
-long long* trace_buffer();                 // device address of the [12][512] clock-stamp buffer (SGB_DEBUG_SKIP & 16)
-int debug_skip_mask();                      // SGB_DEBUG_SKIP (perf experiments only)
-
-struct Problem;
-bool halo_supported(const Problem& q);      // conv_halo_sm100.cu: 3x3 stride-1 convolutions read from one halo tile
-int halo_launch(const Problem& q, cudaStream_t st);
-long long halo_launch_count();
-struct WgradProblem;
-bool wgrad_halo_supported(const WgradProblem& q);  // 3x3 stride-1 weight gradient from halo tiles
-int wgrad_halo_launch(const WgradProblem& q, cudaStream_t st);
 
 }  // namespace sm100

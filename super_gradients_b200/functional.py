@@ -181,13 +181,13 @@ def flush_wgrads(ctx: StepContext, device) -> int:
 
 # Folded QARepVGG (default; SGB_QAREP_FOLD=0 restores the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
 # of ONE 3x3 convolution with 2K output channels (rows [0, K) = the 3x3 filters, rows [K, 2K) = alpha * K1 + I embedded at the centre),
-# so y3 and u come out of one halo-kernel launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
+# so y3 and u come out of one convolution launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
 # epilogue) and wgrad produces both gradients in one launch (for K <= 64 inside the M = 128 padding the 3x3 weight gradient pays
-# for anyway).  Measured on B200 (YOLO-NAS-S, batch 32): 1679 -> 1722 img/s, 830 -> 718 launches per step, once the folded filters
-# are written in place by the step's batched re-layout launch (FoldedWeightCache) and the weight gradient goes to the side stream.
+# for anyway).  The folded filters are written in place by the step's batched re-layout launch (FoldedWeightCache) and the weight
+# gradient goes to the side stream.
 QAREP_FOLD = [__import__("os").environ.get("SGB_QAREP_FOLD", "1") != "0"]
 QAREP_FOLD_MAXPIX = [int(__import__("os").environ.get("SGB_QAREP_FOLD_MAXPIX", "0"))]  # > 0: fold only maps of at most this many pixels (N*H*W)
-_FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts the halo-tile kernels are instantiated for
+_FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS stride-1 blocks that fold
 
 
 def qarep_fold_supported(cin: int, x_channels: int, kout: int, stride: int) -> bool:
@@ -326,10 +326,8 @@ class ConcatWeightCache:
 # the buffer.  Autograd's sum is unchanged whatever else consumes the tensor (non-participating consumers are added by autograd
 # as before).  It relies on every registered consumer running in the same backward pass; a pass that reaches only some of them
 # (part of the outputs unused) is detected by a callback at the end of the pass and raises instead of returning wrong gradients
-# Measured on B200 (YOLO-NAS-S, batch 32): the 39 ATen adds disappear (-0.78 ms) but the accumulating epilogues of the halo / 1x1
-# tile kernels read the residual row with one dependent 16-byte load per thread and cost more than that (+1.3 ms): 1627 img/s
-# with the mechanism against 1673 without, so it is OFF by default (SGB_SHARE_GRADS=1 turns it on) until those epilogues prefetch
-# the residual through TMA.
+# The ATen adds disappear, but the accumulating convolution epilogues read the residual row with dependent loads; the mechanism is
+# OFF by default (SGB_SHARE_GRADS=1 turns it on) until those epilogues prefetch the residual through TMA.
 SHARE_GRADS = [__import__("os").environ.get("SGB_SHARE_GRADS", "0") == "1"]
 
 
@@ -603,7 +601,7 @@ def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracke
 
 
 # Output channels that are not a multiple of 16 (the 68-channel DFL regression convolution, yolo_nas/dfl_heads.py:66) do not fit the
-# tcgen05 kernels' N granularity and used to fall back to the mma.sync kernels for forward, input gradient and weight gradient.
+# wgmma kernels' N granularity and used to fall back to the mma.sync kernels for forward, input gradient and weight gradient.
 # They now run as a convolution with K rounded up to 16: zero filter rows / bias entries for the padding channels (staged fp32 copy,
 # refreshed when the parameter changes), the output allocated with that pitch and handed on as its first K channels, and in the
 # backward the incoming gradient re-described with the padded channel count when its producer marked the padding as zero
@@ -612,11 +610,11 @@ KPAD = [__import__("os").environ.get("SGB_KPAD", "1") != "0"]
 
 
 # ------------------------------------------------------------------------------------------------------------ conv + BN stem on patches
-# ResNet's first layer (7 x 7, stride 2, 3 input channels; training/models/classification_models/resnet.py:162 of the reference) has no tcgen05
+# ResNet's first layer (7 x 7, stride 2, 3 input channels; training/models/classification_models/resnet.py:162 of the reference) has no wgmma
 # kernel of its own: padded to 16 channels it ran on the mma.sync implicit GEMM at 130-145 TF/s -- 2.2 ms forward + 2.5 ms weight
 # gradient of a 30 ms ResNet-50 step at batch 256.  Like the YOLO-NAS stem it becomes ONE 1 x 1 GEMM over gathered patches
 # (3 * 7 * 7 = 147 patch channels padded to 160): the gather reads the image once, forward and weight gradient are im2col-free
-# tcgen05 GEMMs, and there is no dgrad (the image needs no gradient).  Same products of the same bf16 operands, fp32 accumulation.
+# wgmma GEMMs, and there is no dgrad (the image needs no gradient).  Same products of the same bf16 operands, fp32 accumulation.
 STEM_PATCH_MAX_CHANNELS = 256
 
 

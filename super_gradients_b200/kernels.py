@@ -336,7 +336,7 @@ def convt2x2_fprop(x_small, w_up, bias, C_up):
 # ------------------------------------------------------------------------------------------------ layout
 def nchw_f32_to_nhwc_bf16(x: torch.Tensor, c_align: int = 8) -> torch.Tensor:
     """c_align: channel count of the result is C rounded up to a multiple of it (16 lets a 3-channel image use the
-    tcgen05 path, whose K-chunk is 16 channels)."""
+    wgmma path, whose K-chunk is 16 channels)."""
     require_cuda(x, "x")
     n, c, h, w = x.shape
     x = x.contiguous().float()

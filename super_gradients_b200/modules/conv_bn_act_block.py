@@ -1,5 +1,5 @@
 """`Conv`, `ConvBNAct` with the reference's constructor signature and state-dict keys
-(modules/conv_bn_act_block.py:9-104); forward is the fused sm_100a path (functional.conv_bn_act)."""
+(modules/conv_bn_act_block.py:9-104); forward is the fused sm_90a path (functional.conv_bn_act)."""
 from typing import Tuple, Type, Union
 
 from torch import nn
@@ -19,9 +19,9 @@ def _single(v):
 
 def check_conv_supported(conv: nn.Conv2d):
     if conv.groups != 1:
-        raise NotImplementedError("grouped convolutions have no sm_100a kernel in super_gradients_b200")
+        raise NotImplementedError("grouped convolutions have no sm_90a kernel in super_gradients_b200")
     if _single(conv.dilation) != 1:
-        raise NotImplementedError("dilated convolutions have no sm_100a kernel in super_gradients_b200")
+        raise NotImplementedError("dilated convolutions have no sm_90a kernel in super_gradients_b200")
     if conv.padding_mode != "zeros":
         raise NotImplementedError("only zero padding is implemented")
 

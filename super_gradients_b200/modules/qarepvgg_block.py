@@ -33,7 +33,7 @@ class QARepVGGBlock(nn.Module):
     ):
         super().__init__()
         if groups != 1 or dilation != 1:
-            raise NotImplementedError("QARepVGGBlock: groups/dilation != 1 have no sm_100a kernel")
+            raise NotImplementedError("QARepVGGBlock: groups/dilation != 1 have no sm_90a kernel")
         if se_type is not nn.Identity:
             raise NotImplementedError("QARepVGGBlock: SE blocks are not on the YOLO-NAS path (se_type must be nn.Identity)")
         activation_kwargs = activation_kwargs or {}

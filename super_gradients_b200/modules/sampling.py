@@ -18,5 +18,5 @@ class ConvTranspose2x2(nn.ConvTranspose2d):
 def make_upsample_module_with_explicit_channels(in_channels: int, out_channels: int, scale_factor: int, upsample_mode="conv_transpose", align_corners=None) -> nn.Module:
     mode = getattr(upsample_mode, "value", upsample_mode)
     if str(mode).lower() not in ("conv_transpose",) or scale_factor != 2:
-        raise NotImplementedError(f"upsample mode {upsample_mode} (x{scale_factor}) has no sm_100a kernel; YOLO-NAS uses conv_transpose x2")
+        raise NotImplementedError(f"upsample mode {upsample_mode} (x{scale_factor}) has no sm_90a kernel; YOLO-NAS uses conv_transpose x2")
     return ConvTranspose2x2(in_channels, out_channels)

@@ -1,4 +1,4 @@
-"""PPYoloELoss (reference: training/losses/ppyolo_loss.py:640-1084) on the sm_100a path.
+"""PPYoloELoss (reference: training/losses/ppyolo_loss.py:640-1084) on the sm_90a path.
 
 forward(outputs, targets) -> (loss, log_items[4]) with the reference's semantics (task-aligned assigner, varifocal +
 GIoU + DFL, normalisation by max(sum(assigned_scores), 1), weights 1.0 / 2.5 / 0.5).  Target padding is done on the
@@ -8,7 +8,7 @@ assigner (3 small kernels) and the fused loss forward+backward (1 kernel) replac
 Both assigners of the reference are served: the task-aligned one (`use_static_assigner=False`, the YOLO-NAS recipes) by
 `sgb_tal_assign`, the ATSS static one (`use_static_assigner=True`, the constructor default as in the reference) by `sgb_atss_assign`;
 `use_varifocal_loss=False` swaps the classification term for the focal pass (`sgb_focal_cls_fwd_bwd`).  All of them are parity-tested on
-B200 against the reference's recorded values (tests/test_zz_pose_train_gpu.py).  Deviation (DESIGN.md section 4): under DDP the
+the GPU against the reference's recorded values (tests/test_zz_pose_train_gpu.py).  Deviation (DESIGN.md section 4): under DDP the
 normaliser is per rank unless `sync_normaliser=True` (SURVEY.md D4).
 """
 from typing import Optional, Tuple, Union

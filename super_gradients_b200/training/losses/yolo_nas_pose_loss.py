@@ -1,4 +1,4 @@
-"""YoloNASPoseLoss (reference: training/losses/yolo_nas_pose_loss.py:280-682) on the sm_100a path.
+"""YoloNASPoseLoss (reference: training/losses/yolo_nas_pose_loss.py:280-682) on the sm_90a path.
 
 forward(outputs, targets) -> (loss, log_items[6] = cls, iou, dfl, pose_cls, pose_reg, total) with the reference's
 semantics: OKS-aware task-aligned assigner with crowd handling, focal / BCE person classification normalised by

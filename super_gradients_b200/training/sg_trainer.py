@@ -1,5 +1,5 @@
 """Trainer with the reference's entry points -- Trainer(experiment_name, ckpt_root_dir).train(model, training_params,
-train_loader, valid_loader) / .test() -- driving the sm_100a hot path (reference: training/sg_trainer/sg_trainer.py).
+train_loader, valid_loader) / .test() -- driving the sm_90a hot path (reference: training/sg_trainer/sg_trainer.py).
 
 What is kept: the per-batch order of SURVEY.md Appendix B (H2D -> forward+loss -> backward -> optimizer -> EMA -> LR
 step), named training_params of the reference recipes (max_epochs, initial_lr, lr_mode, cosine_final_lr_ratio,
@@ -151,7 +151,7 @@ def setup_device(device: Optional[str] = None):
     """torchrun-launched jobs (LOCAL_RANK set) are data parallel over NCCL, one process per GPU
     (reference: training/utils/distributed_training_utils.py:173-311, env:// rendezvous)."""
     if not torch.cuda.is_available():
-        raise RuntimeError("super_gradients_b200 needs a CUDA device (sm_100a); there is no CPU execution path")
+        raise RuntimeError("super_gradients_b200 needs a CUDA device (sm_90a); there is no CPU execution path")
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local_rank)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 and not torch.distributed.is_initialized():

@@ -897,9 +897,33 @@ def golden_droppath():
     torch.save(out, os.path.join(HERE, "droppath.pt"))
 
 
+def golden_glue_outputs():
+    """The reference's DetectionCollateFN / YoloNASPoseCollateFN and export decoding modules on the seeded inputs of
+    tests/test_host_logic.py (what its collate / decoding tests compare against)."""
+    import numpy as np
+
+    sys.path.insert(0, os.path.dirname(HERE))
+    import test_host_logic as T
+    from super_gradients.training.datasets.pose_estimation_datasets.yolo_nas_pose_collate_fn import YoloNASPoseCollateFN
+    from super_gradients.training.models.detection_models.yolo_nas.yolo_nas_variants import YoloNASDecodingModule
+    from super_gradients.training.models.pose_estimation_models.yolo_nas_pose.yolo_nas_pose_variants import YoloNASPoseDecodingModule
+    from super_gradients.training.utils.collate_fn.detection_collate_fn import DetectionCollateFN
+
+    gen = np.random.RandomState(0)
+    data = [(gen.rand(16, 24, 3).astype(np.float32), gen.rand(n, 5).astype(np.float32) * 10) for n in (3, 0, 2)]
+    det = DetectionCollateFN()(data)
+    pa, (pb, pj, pc), _ = YoloNASPoseCollateFN()(T._pose_samples(1))
+    g = torch.Generator().manual_seed(0)
+    boxes, scores = torch.rand(3, 400, 4, generator=g), torch.rand(3, 400, 80, generator=g)
+    dec = YoloNASDecodingModule(100)(((boxes, scores), None))
+    conf, coords, js = torch.rand(3, 400, 1, generator=g), torch.rand(3, 400, 17, 2, generator=g), torch.rand(3, 400, 17, generator=g)
+    pose_dec = YoloNASPoseDecodingModule(64)(((boxes, conf, coords, js), None))
+    torch.save(dict(det_collate=tuple(det), pose_collate=(pa, pb, pj, pc), det_decode=tuple(dec), pose_decode=tuple(pose_dec)), os.path.join(HERE, "glue_outputs.pt"))
+
+
 if __name__ == "__main__":
     ref_shim.install()
-    which = sys.argv[1:] or ["qarepvgg", "conv_blocks", "loss", "atss", "nms", "yolox_nms", "processing", "detection_metrics", "lr_schedules", "param_groups", "pose_nms", "pose", "tiny_yolo_nas", "tiny_yolo_nas_pose", "tiny_yolo_nas_pose_train", "state_keys", "resnet_cifar_train", "other_configs", "port_fidelity"]
+    which = sys.argv[1:] or ["qarepvgg", "conv_blocks", "loss", "atss", "nms", "yolox_nms", "processing", "detection_metrics", "lr_schedules", "param_groups", "pose_nms", "pose", "tiny_yolo_nas", "tiny_yolo_nas_pose", "tiny_yolo_nas_pose_train", "state_keys", "resnet_cifar_train", "other_configs", "port_fidelity", "glue_outputs"]
     for w in which:
         print("generating", w, flush=True)
         globals()["golden_" + w]()

@@ -1,7 +1,7 @@
 """Every kernel call the OTHER benchmark configurations make (BASELINE.json configs 3-5: YOLO-NAS-M / -L training, ResNet-50 training,
 YOLO-NAS-POSE-L predict) is accepted by the C-ABI's host-side argument validation.
 
-Only YOLO-NAS-S, the tiny fixtures and resnet18_cifar have run on a B200 so far.  Here the models run on the CPU stand-in backend,
+Only YOLO-NAS-S, the tiny fixtures and resnet18_cifar have run on the GPU so far.  Here the models run on the CPU stand-in backend,
 and every kernel wrapper call is ALSO forwarded to the real wrapper and the real libsgb200.so entry point with the host tensors'
 addresses: without a GPU the entry point either rejects the descriptor (SGB_E_INVALID / SGB_E_UNSUPPORTED -- a shape this
 library cannot serve, which would be the first thing to fail on hardware) or gets as far as the first CUDA call and returns

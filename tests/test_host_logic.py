@@ -284,7 +284,7 @@ def _pose_samples(seed):
 def test_collate_functions_produce_the_reference_target_formats():
     """DetectionCollateFN (detection_collate_fn.py:10-49) and YoloNASPoseCollateFN / flat_collate_tensors_with_batch_index
     (yolo_nas_pose_collate_fn.py:14-123): the producers of the flat target tensors rows L1 / L7 consume -- equal to the reference's
-    outputs when /root/reference is present, and accepted by the product's target padding either way."""
+    recorded outputs, and accepted by the product's target padding."""
     from super_gradients_b200.common.registry import COLLATE_FUNCTIONS
     from super_gradients_b200.training.datasets.pose_estimation_datasets import YoloNASPoseCollateFN, flat_collate_tensors_with_batch_index, undo_flat_collate_tensors_with_batch_index
     from super_gradients_b200.training.losses.ppyolo_loss import pad_targets_host
@@ -315,33 +315,18 @@ def test_collate_functions_produce_the_reference_target_formats():
     padded = pad_pose_targets_host((b.float(), j.float(), c), 3, 4)
     assert padded[-1].sum(1).tolist() == [2, 0, 3]
 
-    # against the reference itself, in a child process (the import shim installs module stubs that must not leak into this one)
-    if not os.path.isdir("/root/reference/src/super_gradients"):
-        return
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    child = (
-        "import sys, torch, numpy as np; sys.path[:0] = [%r, %r]\n"
-        "import test_host_logic as T\n"
-        "from oracle import ref_shim; ref_shim.install()\n"
-        "from super_gradients.training.datasets.pose_estimation_datasets.yolo_nas_pose_collate_fn import YoloNASPoseCollateFN as RefPose\n"
-        "from super_gradients.training.utils.collate_fn.detection_collate_fn import DetectionCollateFN as RefDet\n"
-        "from super_gradients_b200.training.datasets.pose_estimation_datasets import YoloNASPoseCollateFN\n"
-        "from super_gradients_b200.training.utils.collate_fn import DetectionCollateFN\n"
-        "gen = np.random.RandomState(0)\n"
-        "data = [(gen.rand(16, 24, 3).astype(np.float32), gen.rand(n, 5).astype(np.float32) * 10) for n in (3, 0, 2)]\n"
-        "(ri, rt), (pi, pt) = RefDet()(data), DetectionCollateFN()(data)\n"
-        "assert torch.equal(ri, pi) and torch.equal(rt, pt) and rt.dtype == pt.dtype\n"
-        "ra, (rb, rj, rc), _ = RefPose()(T._pose_samples(1)); pa, (pb, pj, pc), _ = YoloNASPoseCollateFN()(T._pose_samples(1))\n"
-        "assert torch.equal(ra, pa) and torch.equal(rb, pb) and torch.equal(rj, pj) and torch.equal(rc, pc) and rb.dtype == pb.dtype and rc.dtype == pc.dtype\n"
-        "print('same as the reference')\n"
-    ) % (root, os.path.join(root, "tests"))
-    out = subprocess.run([sys.executable, "-c", child], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0 and "same as the reference" in out.stdout, out.stdout[-2000:] + out.stderr[-2000:]
+    # against the reference's outputs on the same inputs (tests/golden/make_goldens.py: glue_outputs)
+    ref = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "glue_outputs.pt"), weights_only=False)
+    for r, p in zip(ref["det_collate"], DetectionCollateFN()(data)):
+        assert torch.equal(r, p) and r.dtype == p.dtype
+    pa, (pb, pj, pc), _ = YoloNASPoseCollateFN()(_pose_samples(1))
+    for r, p in zip(ref["pose_collate"], (pa, pb, pj, pc)):
+        assert torch.equal(r, p) and r.dtype == p.dtype
 
 
 def test_export_decoding_modules_match_the_reference():
     """Row N4: YoloNASDecodingModule (yolo_nas_variants.py:53-72) and YoloNASPoseDecodingModule (yolo_nas_pose_variants.py:54-90),
-    the pre-NMS top-k of the export graph, against the reference's modules on the same random head outputs (child process)."""
+    the pre-NMS top-k of the export graph, against the reference's modules' recorded outputs on the same random head outputs."""
     from super_gradients_b200.training.models.detection_models.yolo_nas import YoloNASDecodingModule
     from super_gradients_b200.training.models.pose_estimation_models.yolo_nas_pose.yolo_nas_pose_variants import YoloNASPoseDecodingModule
 
@@ -354,25 +339,15 @@ def test_export_decoding_modules_match_the_reference():
     assert pb.shape == (2, 8, 4) and pc.shape == (2, 8, 1) and pj.shape == (2, 8, 5, 3) and (pc[:, :, 0].diff(dim=1) <= 0).all()
     k = int(conf[0, :, 0].argmax())
     assert torch.equal(pb[0, 0], boxes[0, k]) and torch.equal(pj[0, 0, :, :2], coords[0, k]) and torch.equal(pj[0, 0, :, 2], js[0, k])
-    if not os.path.isdir("/root/reference/src/super_gradients"):
-        return
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    child = (
-        "import sys, torch; sys.path[:0] = [%r]\n"
-        "from oracle import ref_shim; ref_shim.install()\n"
-        "from super_gradients.training.models.detection_models.yolo_nas.yolo_nas_variants import YoloNASDecodingModule as RD\n"
-        "from super_gradients.training.models.pose_estimation_models.yolo_nas_pose.yolo_nas_pose_variants import YoloNASPoseDecodingModule as RP\n"
-        "from super_gradients_b200.training.models.detection_models.yolo_nas import YoloNASDecodingModule as PD\n"
-        "from super_gradients_b200.training.models.pose_estimation_models.yolo_nas_pose.yolo_nas_pose_variants import YoloNASPoseDecodingModule as PP\n"
-        "gen = torch.Generator().manual_seed(0)\n"
-        "boxes, scores = torch.rand(3, 400, 4, generator=gen), torch.rand(3, 400, 80, generator=gen)\n"
-        "for a, b in zip(RD(100)(((boxes, scores), None)), PD(100)(((boxes, scores), None))): assert torch.equal(a, b)\n"
-        "conf, coords, js = torch.rand(3, 400, 1, generator=gen), torch.rand(3, 400, 17, 2, generator=gen), torch.rand(3, 400, 17, generator=gen)\n"
-        "for a, b in zip(RP(64)(((boxes, conf, coords, js), None)), PP(64)(((boxes, conf, coords, js), None))): assert torch.equal(a, b)\n"
-        "print('same as the reference')\n"
-    ) % (root,)
-    out = subprocess.run([sys.executable, "-c", child], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0 and "same as the reference" in out.stdout, out.stdout[-2000:] + out.stderr[-2000:]
+    # against the reference's modules on the same inputs (tests/golden/make_goldens.py: glue_outputs)
+    ref = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "glue_outputs.pt"), weights_only=False)
+    gen = torch.Generator().manual_seed(0)
+    boxes, scores = torch.rand(3, 400, 4, generator=gen), torch.rand(3, 400, 80, generator=gen)
+    for a, b in zip(ref["det_decode"], YoloNASDecodingModule(100)(((boxes, scores), None))):
+        assert torch.equal(a, b)
+    conf, coords, js = torch.rand(3, 400, 1, generator=gen), torch.rand(3, 400, 17, 2, generator=gen), torch.rand(3, 400, 17, generator=gen)
+    for a, b in zip(ref["pose_decode"], YoloNASPoseDecodingModule(64)(((boxes, conf, coords, js), None))):
+        assert torch.equal(a, b)
 
 
 def test_flat_state_adjacency_requests_and_checkpoint_remap(tmp_path):

@@ -67,7 +67,7 @@ def main():
             dw = torch.zeros(k, r, r, c, device="cuda")
             us = bench(lambda: K.conv_wgrad(x, y, r, r, s, pad, dw_krsc=dw), flush)
         used = lib.load().sgb_sm100_launches() > n0
-        print(f"{which} C={c:4d} {h}x{w} K={k:4d} r={r} s={s}: {us:8.1f} us  {flops / us / 1e6:7.1f} TFLOP/s  {bytes_ / us / 1e3:7.1f} GB/s(min traffic)  tcgen05={used}")
+        print(f"{which} C={c:4d} {h}x{w} K={k:4d} r={r} s={s}: {us:8.1f} us  {flops / us / 1e6:7.1f} TFLOP/s  {bytes_ / us / 1e3:7.1f} GB/s(min traffic)  wgmma={used}")
 
 
 if __name__ == "__main__":

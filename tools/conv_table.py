@@ -46,7 +46,7 @@ def main():
         step.set_hyper_params(2e-4, 0.9997)
         step._step_eager(x, t)
     torch.cuda.synchronize()
-    # which engine served each convolution call: the library counts launches of the im2col (umma) and halo-tile kernels
+    # which engine served each convolution call: the library counts launches of the wgmma / TMA kernels
     lib = K.L.load()
     engines = []
     orig_call = K.L.call
@@ -54,10 +54,10 @@ def main():
     def call(name, *a):
         if not name.startswith("sgb_conv_"):
             return orig_call(name, *a)
-        u0, h0 = lib.sgb_sm100_launches(), lib.sgb_sm100_halo_launches()
+        u0 = lib.sgb_sm100_launches()
         rc = orig_call(name, *a)
-        u1, h1 = lib.sgb_sm100_launches(), lib.sgb_sm100_halo_launches()
-        engines.append("halo" if h1 > h0 else ("umma" if u1 > u0 else "mma.sync"))
+        u1 = lib.sgb_sm100_launches()
+        engines.append("wgmma" if u1 > u0 else "mma.sync")
         return rc
 
     K.L.call = call
