@@ -407,6 +407,22 @@ int sgb_detection_matching(const SgbMatchDesc* d, const float* preds, const int3
                            const int32_t* target_count, const float* crowd, const int32_t* crowd_count, const float* thresholds,
                            uint8_t* matched, uint8_t* ignore, void* stream);
 
+/* ---- PoseEstimationMetrics matching (training/metrics/pose_estimation_metrics.py:237-314, pose_estimation_utils.py:35-263) ---- */
+/* poses [B, max_preds, n_joints, 3] f32 (x, y, joint score; only x, y are read), scores [B, max_preds] f32, pred_count [B] (rows
+ * in any order; the top_k by score are used); gt_joints [B, max_targets, n_joints, 3] f32 (x, y, visibility), gt_boxes
+ * [B, max_targets, 4] f32 XYWH, gt_areas [B, max_targets] f32, gt_flags [B, max_targets] u8 (1: is_crowd, 2: box given, 4: area
+ * given; missing ones are derived from the visible joints), gt_count [B]; sigmas [n_joints] f32; thresholds [n_thresholds] f32.
+ * With K = min(top_k, max_preds): matched / ignore [B, K, n_thresholds] u8 and used_scores [B, K] f32 in score order (rows past
+ * used_count[b] are zero), used_count [B], n_targets [B] (targets neither crowd nor fully invisible) =
+ * compute_img_keypoint_matching's preds_matched / preds_to_ignore / preds_scores / num_targets.  oks_out (NULL: not written)
+ * [B, K, max_targets] f32 receives the OKS of every used prediction against every target.  One CTA per image, one warp per
+ * threshold; an image's working set must fit in 200 KB of shared memory (pose_match.cu states the formula). */
+int sgb_pose_keypoint_matching(const float* poses, const float* scores, const int32_t* pred_count, const float* gt_joints,
+                               const float* gt_boxes, const float* gt_areas, const uint8_t* gt_flags, const int32_t* gt_count,
+                               const float* sigmas, const float* thresholds, int32_t B, int32_t max_preds, int32_t max_targets,
+                               int32_t n_joints, int32_t n_thresholds, int32_t top_k, uint8_t* matched, uint8_t* ignore,
+                               float* used_scores, int32_t* used_count, int32_t* n_targets, float* oks_out, void* stream);
+
 /* ---- fused predict() pre-processing (SURVEY section 8(f) N3: training/processing/processing.py:205-590, pipelines.py:192-216) ---- */
 typedef struct SgbPreprocDesc {
   int32_t src_h, src_w, src_c; /* uint8 H x W x C source image (C <= 4) */

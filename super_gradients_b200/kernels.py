@@ -425,6 +425,44 @@ def detection_matching(preds, pred_count, targets, target_count, crowd, crowd_co
     return matched, ignore
 
 
+def pose_keypoint_matching(poses, scores, pred_count, gt_joints, gt_boxes, gt_areas, gt_flags, gt_count, sigmas, thresholds, top_k, oks_out=False):
+    """PoseEstimationMetrics matching of one batch.  poses [B, P, J, 3] f32 (x, y, joint score), scores [B, P] f32, pred_count [B]
+    int32; gt_joints [B, M, J, 3] f32 (x, y, visibility), gt_boxes [B, M, 4] f32 XYWH, gt_areas [B, M] f32, gt_flags [B, M] uint8
+    (1: crowd, 2: box given, 4: area given), gt_count [B] int32; sigmas [J] f32; thresholds [T] f32.  Returns (matched, ignore
+    [B, K, T] uint8, used_scores [B, K] f32, used_count [B] int32, n_targets [B] int32) with K = min(top_k, P), rows in score order,
+    plus the OKS matrix [B, K, M] f32 of the used predictions against every target when `oks_out`."""
+    require_cuda(poses, "poses")
+    for name, t, dt in (("poses", poses, torch.float32), ("scores", scores, torch.float32), ("pred_count", pred_count, torch.int32), ("gt_joints", gt_joints, torch.float32),
+                        ("gt_boxes", gt_boxes, torch.float32), ("gt_areas", gt_areas, torch.float32), ("gt_flags", gt_flags, torch.uint8), ("gt_count", gt_count, torch.int32),
+                        ("sigmas", sigmas, torch.float32), ("thresholds", thresholds, torch.float32)):  # fmt: skip
+        if t.dtype != dt or not t.is_contiguous() or t.device != poses.device:
+            raise L.SgbError(f"{name} must be a contiguous {dt} tensor on {poses.device}")
+    if poses.dim() != 4 or poses.shape[3] != 3:
+        raise L.SgbError(f"poses must be [B, P, J, 3], got {tuple(poses.shape)}")
+    B, P, J, _ = poses.shape
+    M = gt_joints.shape[1] if gt_joints.dim() == 4 else -1
+    T = thresholds.numel()
+    shapes = ((scores, (B, P)), (pred_count, (B,)), (gt_joints, (B, M, J, 3)), (gt_boxes, (B, M, 4)), (gt_areas, (B, M)), (gt_flags, (B, M)), (gt_count, (B,)), (sigmas, (J,)))
+    if M < 1 or any(tuple(t.shape) != s for t, s in shapes) or thresholds.dim() != 1:
+        raise L.SgbError("pose matching expects scores [B, P], pred_count [B], gt_joints [B, M >= 1, J, 3], gt_boxes [B, M, 4], gt_areas / gt_flags [B, M], gt_count [B], sigmas [J], thresholds [T]")
+    if not 1 <= T <= 32 or int(top_k) < 1:
+        raise L.SgbError(f"pose matching needs 1..32 thresholds (got {T}) and top_k >= 1 (got {top_k})")
+    K = min(int(top_k), P)
+    dev = poses.device
+    matched = torch.empty((B, K, T), dtype=torch.uint8, device=dev)
+    ignore = torch.empty_like(matched)
+    used_scores = torch.empty((B, K), dtype=torch.float32, device=dev)
+    used_count = torch.empty(B, dtype=torch.int32, device=dev)
+    n_targets = torch.empty(B, dtype=torch.int32, device=dev)
+    oks = torch.empty((B, K, M), dtype=torch.float32, device=dev) if oks_out else None
+    if oks is not None:
+        oks.fill_(float("nan"))  # entries of prediction rows past the used count stay NaN
+    _timed("sgb_pose_keypoint_matching", _ptr(poses), _ptr(scores), _ptr(pred_count), _ptr(gt_joints), _ptr(gt_boxes), _ptr(gt_areas), _ptr(gt_flags), _ptr(gt_count), _ptr(sigmas),
+           _ptr(thresholds), B, P, M, J, T, int(top_k), _ptr(matched), _ptr(ignore), _ptr(used_scores), _ptr(used_count), _ptr(n_targets), _ptr(oks), _stream())  # fmt: skip
+    out = (matched, ignore, used_scores, used_count, n_targets)
+    return out + (oks,) if oks_out else out
+
+
 # ------------------------------------------------------------------------------------------------ batch norm
 def bn_desc(x, y, eps, momentum, act, residual=None, stats_repl=STATS_REPL, sample_scale=None) -> L.BnDesc:
     n, c, h, w = x.shape

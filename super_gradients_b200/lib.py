@@ -201,6 +201,7 @@ _SIGNATURES = {
     "sgb_loss_finalize": (c_int, [POINTER(LossDesc), P, P, P]),
     "sgb_preprocess_u8": (c_int, [POINTER(PreprocDesc), P, P, P]),
     "sgb_detection_matching": (c_int, [POINTER(MatchDesc), P, P, P, P, P, P, P, P, P, P]),
+    "sgb_pose_keypoint_matching": (c_int, [P] * 10 + [_I] * 6 + [P] * 7),
     "sgb_pose_tal_workspace_bytes": (c_int64, [POINTER(PoseLossDesc)]),
     "sgb_pose_tal_assign": (c_int, [POINTER(PoseLossDesc)] + [P] * 14 + [_L, P]),
     "sgb_pose_loss_fwd_bwd": (c_int, [POINTER(PoseLossDesc)] + [P] * 12 + [_F] + [P] * 5),
