@@ -166,6 +166,14 @@ typedef struct SgbBnDesc {
    * GEMM with concatenated output channels): channels [dy2_split, C) of dy come from a second tensor.  dy2 == NULL: one source. */
   int32_t dy2_split, dy2_pitch, dy2_off, dy2_reserved;
   const void* dy2;
+  /* cross-rank statistics (torch.nn.SyncBatchNorm under data parallelism), two-pass entry points only: `count` is a device pointer to
+   * the element count of the layer over all ranks, read by the forward and backward apply passes in place of M (means, variance,
+   * unbiased running variance).  `param_scale` multiplies the dgamma / dbeta the backward apply pass accumulates from all-reduced
+   * sums: 1 / (ranks in the group), so that the data-parallel average of the per-rank gradients equals the average of torch's
+   * per-rank SyncBatchNorm gradients.  count == NULL: local statistics, param_scale unused. */
+  const double* count;
+  float param_scale;
+  int32_t count_reserved;
 } SgbBnDesc;
 /* Reduces stats -> mean / rstd (saved for backward), updates running stats, writes y = act(bn(x) + residual). */
 int sgb_bn_act_fwd(const SgbBnDesc* d, const sgb_bf16* x, const double* stats, const float* gamma, const float* beta,
@@ -204,6 +212,11 @@ typedef struct SgbQarepDesc {
   int32_t pitchr, offr;
   const void* res;
   const float* res_alpha;
+  /* cross-rank statistics, exactly as SgbBnDesc.count / param_scale: the forward apply pass takes the all-reduced moments and the
+   * global count, the backward apply pass the all-reduced sums; both BatchNorms of the block follow from them. */
+  const double* count;
+  float param_scale;
+  int32_t count_reserved;
 } SgbQarepDesc;
 int sgb_qarep_moments(const SgbQarepDesc* d, const sgb_bf16* y3, const sgb_bf16* u, double* moments, void* stream);
 /* coef out: [9][C] floats = mu3, rstd3, mu_u, rstd_z, a3 (coefficient of y3), au (of u), c0 (constant),

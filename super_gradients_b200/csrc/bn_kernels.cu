@@ -57,6 +57,17 @@ __device__ __forceinline__ V8 unpack8(const uint4& r) {
   }
   return o;
 }
+// Element count the statistics are taken over: the layer's pixels on every rank (SgbBnDesc / SgbQarepDesc .count, written by the
+// all-reduce that also summed the statistics) or the local M; and the factor on the parameter gradients an apply pass accumulates.
+template <class D>
+__device__ __forceinline__ double stat_count(const D& d) {
+  return d.count ? *d.count : (double)d.M;
+}
+template <class D>
+__device__ __forceinline__ double param_scale(const D& d) {
+  return d.count ? (double)d.param_scale : 1.0;
+}
+
 template <class Op>
 constexpr size_t chan_ring_bytes() {
   return sgb_ring::bytes<Op::NIN, Op::UNROLL, Op::DEPTH, TPB>();
@@ -246,14 +257,15 @@ struct BnFwdOp {
   int out_stride = 0;
   __device__ void prologue(float* sc) const {
     const int C = d.C;
+    const double M = stat_count(d);
     for (int c = threadIdx.x; c < C; c += TPB) {
       double s1 = 0, s2 = 0;
       for (int r = 0; r < d.stats_repl; ++r) {  // L2 reads: in the fused launch other CTAs produced the sums just before the grid barrier
         s1 += __ldcg(stats + (int64_t)r * 2 * C + c);
         s2 += __ldcg(stats + (int64_t)r * 2 * C + C + c);
       }
-      const double mean = s1 / (double)d.M;
-      double var = s2 / (double)d.M - mean * mean;
+      const double mean = s1 / M;
+      double var = s2 / M - mean * mean;
       if (var < 0) var = 0;
       const float rstd = (float)(1.0 / sqrt(var + (double)d.eps));
       const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
@@ -263,7 +275,7 @@ struct BnFwdOp {
         save_mean[c] = (float)mean;
         save_rstd[c] = rstd;
         if (rmean) {
-          const double unb = d.M > 1 ? var * (double)d.M / (double)(d.M - 1) : var;
+          const double unb = M > 1.0 ? var * M / (M - 1.0) : var;
           rmean[c] = (1.f - d.momentum) * rmean[c] + d.momentum * (float)mean;
           rvar[c] = (1.f - d.momentum) * rvar[c] + d.momentum * (float)unb;
         }
@@ -395,6 +407,7 @@ struct BnBwdApplyOp {
   int out_stride = 0;
   __device__ void prologue(float* sc) const {
     const int C = d.C;
+    const double M = stat_count(d), ps = param_scale(d);
     for (int c = threadIdx.x; c < C; c += TPB) {
       const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
       sc[c] = mean[c];
@@ -402,11 +415,11 @@ struct BnBwdApplyOp {
       sc[2 * C + c] = g * rstd[c];
       sc[3 * C + c] = b - mean[c] * g * rstd[c];
       const double S0 = __ldcg(sums + c), S1 = __ldcg(sums + C + c);  // L2 reads: in the fused launch other CTAs just wrote them
-      sc[4 * C + c] = (float)(S0 / (double)d.M);
-      sc[5 * C + c] = (float)(S1 / (double)d.M);
+      sc[4 * C + c] = (float)(S0 / M);
+      sc[5 * C + c] = (float)(S1 / M);
       if (blockIdx.x == 0) {
-        if (dgamma) dgamma[c] += (float)S1;
-        if (dbeta) dbeta[c] += (float)S0;
+        if (dgamma) dgamma[c] += (float)(S1 * ps);
+        if (dbeta) dbeta[c] += (float)(S0 * ps);
       }
     }
   }
@@ -488,7 +501,7 @@ struct QarepFwdOpT {
   int out_stride = 0;
   __device__ void prologue(float* sc) const {
     const int C = d.C;
-    const double M = (double)d.M;
+    const double M = stat_count(d);
     for (int c = threadIdx.x; c < C; c += TPB) {
       // L2 reads: in the fused launch other CTAs produced the sums just before the grid barrier
       const double S3 = __ldcg(mom + c), S33 = __ldcg(mom + C + c), Su = __ldcg(mom + 2 * C + c), Suu = __ldcg(mom + 3 * C + c), S3u = __ldcg(mom + 4 * C + c);
@@ -531,7 +544,7 @@ struct QarepFwdOpT {
         coef[6 * C + c] = (float)c0;
         coef[7 * C + c] = (float)czy;
         coef[8 * C + c] = (float)s3;
-        const double unb = d.M > 1 ? M / (M - 1.0) : 1.0;
+        const double unb = M > 1.0 ? M / (M - 1.0) : 1.0;
         if (rm3) {
           rm3[c] = (1.f - d.momentum) * rm3[c] + d.momentum * (float)mu3;
           rv3[c] = (1.f - d.momentum) * rv3[c] + d.momentum * (float)(var3 * unb);
@@ -624,7 +637,7 @@ struct QarepBwdApplyOp {
   int out_stride = 0;
   __device__ void prologue(float* sc) const {
     const int C = d.C;
-    const double M = (double)d.M;
+    const double M = stat_count(d), ps = param_scale(d);
     for (int c = threadIdx.x; c < C; c += TPB) {
       const float rstdz = coef[3 * C + c], czy = coef[7 * C + c];
       const double T0 = __ldcg(sums + c), T1 = __ldcg(sums + C + c), T2 = __ldcg(sums + 2 * C + c);  // L2 reads (fused launch)
@@ -652,14 +665,14 @@ struct QarepBwdApplyOp {
       sc[11 * C + c] = q;
       if (blockIdx.x == 0) {
         if (d.use_post_bn) {
-          if (dgamma_p) dgamma_p[c] += (float)T1;
-          if (dbeta_p) dbeta_p[c] += (float)T0;
-          if (dgamma3) dgamma3[c] += (float)(M * (double)q);
+          if (dgamma_p) dgamma_p[c] += (float)(T1 * ps);
+          if (dbeta_p) dbeta_p[c] += (float)(T0 * ps);
+          if (dgamma3) dgamma3[c] += (float)(M * (double)q * ps);
           // dbeta3 and d(alpha*b1) are exactly zero: post_bn removes any per-channel constant.
         } else {
-          if (dgamma3) dgamma3[c] += (float)T2;
-          if (dbeta3) dbeta3[c] += (float)T0;
-          if (dab) dab[c] += (float)T0;
+          if (dgamma3) dgamma3[c] += (float)(T2 * ps);
+          if (dbeta3) dbeta3[c] += (float)(T0 * ps);
+          if (dab) dab[c] += (float)(T0 * ps);
         }
       }
     }
@@ -706,6 +719,7 @@ int check_bn(const SgbBnDesc* d) {
   SGB_REQUIRE(!d->dy2 || (d->dy2_split > 0 && d->dy2_split < d->C && d->dy2_split % 8 == 0 && d->dy2_pitch % 8 == 0 && d->dy2_off % 8 == 0 &&
                           d->dy2_pitch >= d->dy2_off + d->C - d->dy2_split && ((uintptr_t)d->dy2 & 15) == 0),
               "second dy source layout");
+  SGB_REQUIRE(!d->count || (((uintptr_t)d->count & 7) == 0 && d->param_scale > 0.f && d->param_scale <= 1.f), "cross-rank count / param_scale");
   return SGB_OK;
 }
 int check_qarep(const SgbQarepDesc* d) {
@@ -716,6 +730,7 @@ int check_qarep(const SgbQarepDesc* d) {
   SGB_REQUIRE(d->pitchd == 0 || d->pitchd >= d->offd + d->C, "dout slice layout");
   SGB_REQUIRE(!d->res || (d->res_alpha && d->pitchr % 8 == 0 && d->offr % 8 == 0 && d->pitchr >= d->offr + d->C && ((uintptr_t)d->res & 15) == 0),
               "shortcut tensor layout");
+  SGB_REQUIRE(!d->count || (((uintptr_t)d->count & 7) == 0 && d->param_scale > 0.f && d->param_scale <= 1.f), "cross-rank count / param_scale");
   return SGB_OK;
 }
 
@@ -737,6 +752,7 @@ extern "C" int sgb_bn_act_fwd_fused(const SgbBnDesc* d, const sgb_bf16* x, doubl
                                     float* running_mean, float* running_var, const sgb_bf16* residual, sgb_bf16* y, float* save_mean,
                                     float* save_rstd, void* stream) {
   if (int rc = check_bn(d)) return rc;
+  SGB_REQUIRE(!d->count, "cross-rank statistics need the two-pass entry points (a collective between the passes)");
   SGB_REQUIRE(x && stats && y && save_mean && save_rstd, "null pointer");
   SGB_REQUIRE(d->stats_repl >= 1, "stats_repl");
   BnStatsOp so{*d, (const bf16*)x, stats, d->C};
@@ -778,6 +794,7 @@ extern "C" int sgb_bn_act_bwd_fused(const SgbBnDesc* d, const sgb_bf16* dy, cons
                                     const float* beta, const float* save_mean, const float* save_rstd, double* sums, sgb_bf16* dx,
                                     sgb_bf16* dresidual, float* dgamma, float* dbeta, void* stream) {
   if (int rc = check_bn(d)) return rc;
+  SGB_REQUIRE(!d->count, "cross-rank statistics need the two-pass entry points (a collective between the passes)");
   SGB_REQUIRE(dy && x && save_mean && save_rstd && sums && dx, "null pointer");
   SGB_REQUIRE(!d->sample_scale || y, "drop-path backward needs the forward output (the mask cannot be recomputed from x alone)");
   BnBwdRedOp ra{*d, (const bf16*)dy, (const bf16*)x, (const bf16*)y, save_mean, save_rstd, gamma, beta, sums, d->C};
@@ -804,6 +821,7 @@ extern "C" int sgb_qarep_fwd_fused(const SgbQarepDesc* d, const sgb_bf16* y3, co
                                    const float* beta3, const float* bias1_alpha, const float* gamma_p, const float* beta_p, float* rm3, float* rv3,
                                    float* rm_p, float* rv_p, sgb_bf16* out, float* coef, void* stream) {
   if (int rc = check_qarep(d)) return rc;
+  SGB_REQUIRE(!d->count, "cross-rank statistics need the two-pass entry points (a collective between the passes)");
   SGB_REQUIRE(y3 && u && moments && gamma3 && beta3 && out && coef, "null pointer");
   SGB_REQUIRE(!d->use_post_bn || (gamma_p && beta_p), "post_bn parameters missing");
   QarepMomOp mo{*d, (const bf16*)y3, (const bf16*)u, moments, d->C};
@@ -842,6 +860,7 @@ extern "C" int sgb_qarep_bwd_fused(const SgbQarepDesc* d, const sgb_bf16* dout, 
                                    double* sums, const float* gamma3, const float* gamma_p, sgb_bf16* dy3, sgb_bf16* du, float* dgamma3,
                                    float* dbeta3, float* dbias1a, float* dgamma_p, float* dbeta_p, void* stream) {
   if (int rc = check_qarep(d)) return rc;
+  SGB_REQUIRE(!d->count, "cross-rank statistics need the two-pass entry points (a collective between the passes)");
   SGB_REQUIRE(dout && y3 && u && coef && sums && gamma3 && dy3 && du, "null pointer");
   SGB_REQUIRE(!d->use_post_bn || gamma_p, "gamma_p missing");
   QarepBwdRedOp ra{*d, (const bf16*)dout, (const bf16*)y3, (const bf16*)u, coef, sums, d->C};

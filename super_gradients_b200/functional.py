@@ -442,6 +442,47 @@ def _defer_finish(tok, dx):
     return dx
 
 
+# ------------------------------------------------------------------------------------------------ cross-rank BatchNorm statistics
+class BnSync:
+    """torch.nn.SyncBatchNorm semantics for one train-mode call of a fused block (reference: sg_trainer.py:449-456 converts the model
+    under DDP): the kernel wrappers take the split path (statistics pass, sync(buffer), apply pass) and sync(buffer) sums the buffer
+    over the module's process group -- one collective per layer in the forward (sums + element count) and one in the backward.
+
+    Parameter gradients: the backward apply pass sees the all-reduced sums on every rank; it scales its gamma / beta gradients by
+    param_scale = 1 / (ranks in the group), so that after the flat gradient all-reduce and the 1 / world average they equal the DDP
+    average of torch's per-rank SyncBatchNorm gradients (which are computed from local sums).  `count` is the device tensor of the
+    global element count the forward pass reduced; the backward pass of the same call reads it.
+    A group of one rank sums nothing: the collective is skipped, the split path still runs."""
+
+    __slots__ = ("group", "size", "param_scale", "count")
+
+    def __init__(self, group):
+        self.group = group
+        self.size = torch.distributed.get_world_size(group)
+        self.param_scale = 1.0 / self.size
+        self.count = None
+
+    def __call__(self, buf):
+        SYNC_CALLS[0] += 1
+        if self.size > 1:
+            torch.distributed.all_reduce(buf, group=self.group)
+
+
+SYNC_CALLS = [0]  # BnSync reductions issued so far (tools/time_sync_bn.py reports them per step)
+
+
+def bn_sync(bn) -> Optional[BnSync]:
+    """A BnSync when `bn` is a train-mode torch.nn.SyncBatchNorm and torch.distributed is initialised (process_group None: WORLD),
+    else None: local statistics through the fused launches, exactly as for nn.BatchNorm2d."""
+    if not (isinstance(bn, torch.nn.SyncBatchNorm) and bn.training and torch.distributed.is_available() and torch.distributed.is_initialized()):
+        return None
+    return BnSync(bn.process_group)
+
+
+def _sync_kw(sync) -> dict:
+    return {"sync": sync} if sync is not None else {}
+
+
 def _mg(p):
     """Flat-buffer gradient slot of a parameter (training/flat_state.py) or None under plain autograd."""
     return getattr(p, "main_grad", None) if p is not None else None
@@ -549,11 +590,13 @@ class _ConvBnAct(torch.autograd.Function):
         kout, _, r, s = w.shape
         p_out = (x.shape[2] + 2 * cfg.pad - r) // cfg.stride + 1, (x.shape[3] + 2 * cfg.pad - s) // cfg.stride + 1
         # wide layers: no statistics in the GEMM epilogue, the BatchNorm launch computes them (kernels.stats_in_bn)
-        stats = None if K.stats_in_bn(kout, x.shape[0] * p_out[0] * p_out[1]) else K.new_stats(kout, x.device)
+        pixels = x.shape[0] * p_out[0] * p_out[1]
+        sync = getattr(cfg, "sync", None)
+        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if sync is not None else {}))
         y_raw = K.conv_fprop(x, krsc, kout, r, s, cfg.stride, cfg.pad, stats=stats)
         res = K.as_nhwc(residual) if residual is not None else None
         ss = getattr(cfg, "sample_scale", None)
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, res, **({"sample_scale": ss} if ss is not None else {}))
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, res, **({"sample_scale": ss} if ss is not None else {}), **_sync_kw(sync))
         if cfg.num_batches_tracked is not None and not _NBT_DEFERRED[0]:
             cfg.num_batches_tracked += 1
         ctx.save_for_backward(x, y_raw, out, gamma, mean, rstd, beta)
@@ -568,7 +611,7 @@ class _ConvBnAct(torch.autograd.Function):
         kout, cin, r, s = ctx.wshape
         sw, sg, sb = ctx.slots
         ss = getattr(cfg, "sample_scale", None)
-        dy, dres, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, out, gamma, mean, rstd, cfg.eps, cfg.act, want_residual_grad=ctx.has_res, dgamma=sg, dbeta=sb, beta=beta, **({"sample_scale": ss} if ss is not None else {}))
+        dy, dres, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, out, gamma, mean, rstd, cfg.eps, cfg.act, want_residual_grad=ctx.has_res, dgamma=sg, dbeta=sb, beta=beta, **({"sample_scale": ss} if ss is not None else {}), **_sync_kw(getattr(cfg, "sync", None)))
         dx = None
         if ctx.needs_input_grad[0]:
             dx = _share_dx(
@@ -580,14 +623,15 @@ class _ConvBnAct(torch.autograd.Function):
         return dx, dw, (None if sg is not None else dgamma), (None if sb is not None else dbeta), dres, None
 
 
-def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracked, *, stride, pad, eps, momentum, act, training, cache: WeightCache, residual=None, sample_scale=None):
+def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracked, *, stride, pad, eps, momentum, act, training, cache: WeightCache, residual=None, sample_scale=None, sync=None):
     """Conv2d(bias=False) -> BatchNorm2d -> (* drop-path scale per image) -> (+ residual) -> activation.   reference:
     modules/conv_bn_act_block.py:92-93, training/models/classification_models/resnet.py:53-84 (the residual form),
-    training/utils/regularization_utils.py:4-15 (drop_path; `sample_scale` = bernoulli(keep) / keep per image, training only)."""
+    training/utils/regularization_utils.py:4-15 (drop_path; `sample_scale` = bernoulli(keep) / keep per image, training only).
+    sync: bn_sync(bn) -- cross-rank statistics (SyncBatchNorm)."""
     K.require_cuda(x, "x")
     if training:
         cfg = SimpleNamespace(stride=stride, pad=pad, eps=eps, momentum=momentum, act=act, cache=cache, running_mean=running_mean, running_var=running_var, num_batches_tracked=num_batches_tracked, sample_scale=sample_scale,
-                              share=_share_pickup(x))  # fmt: skip
+                              share=_share_pickup(x), sync=sync)  # fmt: skip
         return _ConvBnAct.apply(x, w, gamma, beta, residual, cfg)
     # inference: BN folded into the GEMM epilogue (one kernel)
     with torch.no_grad():
@@ -659,9 +703,10 @@ class _ConvBnActStem(torch.autograd.Function):
         c_out = ((cin * r * s + 31) // 32) * 32
         xp = K.stem_patches(x, r, cfg.stride, cfg.pad, c_out)
         kf, _ = cfg.cache.get(w, c_out)
-        stats = None if K.stats_in_bn(kout, xp.shape[0] * xp.shape[2] * xp.shape[3]) else K.new_stats(kout, x.device)
+        pixels = xp.shape[0] * xp.shape[2] * xp.shape[3]
+        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if cfg.sync is not None else {}))
         y_raw = K.conv_fprop(xp, kf, kout, 1, 1, 1, 0, stats=stats)
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act)
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, **_sync_kw(cfg.sync))
         if cfg.num_batches_tracked is not None and not _NBT_DEFERRED[0]:
             cfg.num_batches_tracked += 1
         ctx.save_for_backward(xp, y_raw, gamma, mean, rstd, beta)
@@ -675,7 +720,7 @@ class _ConvBnActStem(torch.autograd.Function):
         cfg = ctx.cfg
         kout, cin, r, s = ctx.geom
         sw, sg, sb = ctx.slots
-        dy, _, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, None, gamma, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=beta)
+        dy, _, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, None, gamma, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=beta, **_sync_kw(cfg.sync))
         c = _CTX[0]
         if c is not None and c.side_stream is not None and sw is not None:
             dwf = _side_wgrad(c, xp, dy, 1, 1, 1, 0)
@@ -694,7 +739,7 @@ def conv_bn_act_stem(x, conv, bn, *, act, cache: PatchWeightCache):
     stride = conv.stride[0] if isinstance(conv.stride, (tuple, list)) else conv.stride
     pad = conv.padding[0] if isinstance(conv.padding, (tuple, list)) else conv.padding
     cfg = SimpleNamespace(stride=int(stride), pad=int(pad), eps=bn.eps, momentum=0.1 if bn.momentum is None else bn.momentum, act=act, cache=cache,
-                          running_mean=bn.running_mean, running_var=bn.running_var, num_batches_tracked=bn.num_batches_tracked)  # fmt: skip
+                          running_mean=bn.running_mean, running_var=bn.running_var, num_batches_tracked=bn.num_batches_tracked, sync=bn_sync(bn))  # fmt: skip
     return _ConvBnActStem.apply(x, conv.weight, bn.weight, bn.bias, cfg)
 
 
@@ -724,6 +769,8 @@ def dual_conv_bn_act_ready(conv1, bn1, conv2, bn2) -> bool:
         return False
     if not (bn1.training and bn2.training):  # a frozen BatchNorm (eval() on the sub-module) normalises with its running statistics
         return False
+    if type(bn1) is not type(bn2) or getattr(bn1, "process_group", None) is not getattr(bn2, "process_group", None):  # one collective serves both
+        return False
     pairs = [(bn1.weight, bn2.weight), (bn1.bias, bn2.bias), (bn1.running_mean, bn2.running_mean), (bn1.running_var, bn2.running_var)]
     if not all(_follows(a, b) for a, b in pairs):
         return False
@@ -740,10 +787,12 @@ class _DualConvBnAct(torch.autograd.Function):
         krsc, crsk = cfg.cache.get(w1, w2, x.shape[1])
         kout = k1 + k2
         p_out = (x.shape[2] + 2 * cfg.pad - r) // cfg.stride + 1, (x.shape[3] + 2 * cfg.pad - s) // cfg.stride + 1
-        stats = None if K.stats_in_bn(kout, x.shape[0] * p_out[0] * p_out[1]) else K.new_stats(kout, x.device)
+        pixels = x.shape[0] * p_out[0] * p_out[1]
+        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if cfg.sync is not None else {}))
         y_raw = K.conv_fprop(x, krsc, kout, r, s, cfg.stride, cfg.pad, stats=stats)
-        # gamma / beta / running statistics of the second layer follow the first's in memory: the pointers of the first serve K1 + K2 channels
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, g1, b1, cfg.rm1, cfg.rv1, cfg.eps, cfg.momentum, cfg.act)
+        # gamma / beta / running statistics of the second layer follow the first's in memory: the pointers of the first serve K1 + K2
+        # channels (and one collective carries the statistics of both layers)
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, g1, b1, cfg.rm1, cfg.rv1, cfg.eps, cfg.momentum, cfg.act, **_sync_kw(cfg.sync))
         if not _NBT_DEFERRED[0]:
             for nbt in cfg.nbt:
                 if nbt is not None:
@@ -763,7 +812,7 @@ class _DualConvBnAct(torch.autograd.Function):
             n, _, h, w = y_raw.shape
             d1 = d1 if d1 is not None else torch.zeros((n, k1, h, w), dtype=torch.bfloat16, device=x.device).contiguous(memory_format=torch.channels_last)
             d2 = d2 if d2 is not None else torch.zeros((n, k2, h, w), dtype=torch.bfloat16, device=x.device).contiguous(memory_format=torch.channels_last)
-        dy, _, _, _ = K.bn_act_bwd(d1, y_raw, None, g1, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=b1, dy2=d2)
+        dy, _, _, _ = K.bn_act_bwd(d1, y_raw, None, g1, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=b1, dy2=d2, **_sync_kw(cfg.sync))
         dx = K.conv_dgrad(dy, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad) if ctx.needs_input_grad[0] else None
         c = _CTX[0]
         if c is not None:
@@ -784,7 +833,7 @@ def dual_conv_bn_act(x, conv1, bn1, conv2, bn2, *, act, cache: ConcatWeightCache
     stride = conv1.stride[0] if isinstance(conv1.stride, (tuple, list)) else conv1.stride
     pad = conv1.padding[0] if isinstance(conv1.padding, (tuple, list)) else conv1.padding
     cfg = SimpleNamespace(stride=int(stride), pad=int(pad), eps=bn1.eps, momentum=0.1 if bn1.momentum is None else bn1.momentum, act=act, cache=cache,
-                          rm1=bn1.running_mean, rv1=bn1.running_var, nbt=(bn1.num_batches_tracked, bn2.num_batches_tracked))  # fmt: skip
+                          rm1=bn1.running_mean, rv1=bn1.running_var, nbt=(bn1.num_batches_tracked, bn2.num_batches_tracked), sync=bn_sync(bn1))  # fmt: skip
     return _DualConvBnAct.apply(x, conv1.weight, bn1.weight, bn1.bias, conv2.weight, bn2.weight, bn2.bias, cfg)
 
 
@@ -921,7 +970,7 @@ class _QARepVGG(torch.autograd.Function):
             ab = bias1 * alpha if alpha is not None else bias1
         sc = getattr(cfg, "shortcut", None)  # (x_s, alpha_s, token): out += alpha_s * x_s in the apply pass (a bottleneck's shortcut)
         skw = {"residual": sc[0], "res_alpha": sc[1]} if sc is not None else {}
-        out, coef = K.qarep_fwd(y3, u, g3, b3, ab, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, cfg.use_post_bn, **skw)
+        out, coef = K.qarep_fwd(y3, u, g3, b3, ab, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, cfg.use_post_bn, **skw, **_sync_kw(getattr(cfg, "sync", None)))
         ctx.shortcut = sc
         if not _NBT_DEFERRED[0]:
             for nbt in cfg.nbt:
@@ -953,7 +1002,7 @@ class _QARepVGG(torch.autograd.Function):
             dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
         dy3, du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(
             dout, out, y3, u, coef, g3, gp if has_post else None, cfg.eps, cfg.eps, cfg.act, cfg.use_post_bn, acc=(sg3, sb3, direct_bias, sgp, sbp),
-            out_grads=(dcat[:, :kout], dcat[:, kout:]) if dcat is not None else None,
+            out_grads=(dcat[:, :kout], dcat[:, kout:]) if dcat is not None else None, **_sync_kw(getattr(cfg, "sync", None)),
         )  # fmt: skip
         dx = None
         dw1f = None
@@ -1113,7 +1162,7 @@ class _QARepVGGStem(torch.autograd.Function):
         kf, _ = cfg.cache_stem.get(w3, w1, c_out)
         ycat = K.conv_fprop(xp, kf, 2 * kout, 1, 1, 1, 0)
         y3, u = ycat[:, :kout], ycat[:, kout:]
-        out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True)
+        out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True, **_sync_kw(getattr(cfg, "sync", None)))
         if not _NBT_DEFERRED[0]:
             for nbt in cfg.nbt:
                 if nbt is not None:
@@ -1132,7 +1181,7 @@ class _QARepVGGStem(torch.autograd.Function):
         n, _, h, w = y3.shape
         dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
         _dy3, _du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(dout, out, y3, u, coef, g3, gp, cfg.eps, cfg.eps, cfg.act, True, acc=(sg3, sb3, sbias, sgp, sbp),
-                                                         out_grads=(dcat[:, :kout], dcat[:, kout:]))  # fmt: skip
+                                                         out_grads=(dcat[:, :kout], dcat[:, kout:]), **_sync_kw(getattr(cfg, "sync", None)))  # fmt: skip
         c = _CTX[0]
         dw3 = dw1 = None
         if c is not None and sw3 is not None and sw1 is not None:

@@ -174,8 +174,24 @@ def conv_desc(x: torch.Tensor, K: int, R: int, S: int, stride: int, pad: int, y:
     return d
 
 
-def new_stats(C: int, device, nacc=2) -> torch.Tensor:
-    return zeros((STATS_REPL, nacc, C), torch.float64, device)
+def new_stats(C: int, device, nacc=2, count=None) -> torch.Tensor:
+    """[STATS_REPL, nacc, C] fp64 accumulators of a GEMM epilogue.  count (cross-rank statistics, bn_act_fwd(sync=...)): the local
+    element count is stored right after the sums, so that ONE all-reduce of the buffer yields the global sums and count."""
+    if count is None:
+        return zeros((STATS_REPL, nacc, C), torch.float64, device)
+    return new_sync_sums(STATS_REPL * nacc * C, count, device)[:-1].view(STATS_REPL, nacc, C)
+
+
+def new_sync_sums(n: int, count, device) -> torch.Tensor:
+    """fp64 [n + 1]: n zeroed sums followed by the element count (one fill launch; zeros() is a memset inside a step)."""
+    buf = zeros((n + 1,), torch.float64, device)
+    buf[n:].fill_(float(count))
+    return buf
+
+
+def _with_count(sums: torch.Tensor) -> torch.Tensor:
+    """The flat buffer of sums allocated with their element count behind them (new_stats(count=...), new_sync_sums)."""
+    return torch.as_strided(sums, (sums.numel() + 1,), (1,), sums.storage_offset())
 
 
 # ------------------------------------------------------------------------------------------------ conv family
@@ -498,13 +514,31 @@ def stats_in_bn(kout: int, pixels: int) -> bool:
     return STATS_IN_BN[0] and kout not in _EPILOGUE_STATS_CHANNELS and kout % 8 == 0 and 2 * kout * pixels <= STATS_IN_BN_MAX_BYTES[0]
 
 
-def bn_act_fwd(x, stats, gamma, beta, running_mean, running_var, eps, momentum, act, residual=None, sample_scale=None):
+def bn_act_fwd(x, stats, gamma, beta, running_mean, running_var, eps, momentum, act, residual=None, sample_scale=None, sync=None):
     """stats: [repl, 2, C] fp64 sums from the producing GEMM's epilogue, or None: the launch computes them itself (cooperative:
-    sums, grid-wide barrier, apply)."""
+    sums, grid-wide barrier, apply).
+
+    sync (functional.BnSync): cross-rank statistics in two passes -- the sums (epilogue sums from new_stats(count=...), or
+    sgb_channel_stats) and the local count are all-reduced by ONE sync(buffer) call, then sgb_bn_act_fwd divides by the global
+    count.  The reduced count is left in sync.count for the backward pass."""
     n, c, h, w = x.shape
     y = empty_nhwc(n, c, h, w, x.device)
     mean = torch.empty(c, dtype=torch.float32, device=x.device)
     rstd = torch.empty(c, dtype=torch.float32, device=x.device)
+    if sync is not None:
+        if stats is None:
+            buf = new_sync_sums(2 * c, n * h * w, x.device)
+            stats = buf[:-1].view(1, 2, c)
+            _timed("sgb_channel_stats", _ptr(x), n * h * w, c, nhwc_pitch(x), 0, _ptr(stats), _stream())
+        else:
+            buf = _with_count(stats)
+        sync(buf)
+        sync.count = buf[-1:]
+        d = bn_desc(x, y, eps, momentum, act, residual, stats.shape[0], sample_scale=sample_scale)
+        d.count = sync.count.data_ptr()
+        d.param_scale = sync.param_scale
+        _timed("sgb_bn_act_fwd", ctypes.byref(d), _ptr(x), _ptr(stats), _ptr(gamma), _ptr(beta), _ptr(running_mean), _ptr(running_var), _ptr(residual), _ptr(y), _ptr(mean), _ptr(rstd), _stream())
+        return y, mean, rstd
     if stats is None:
         stats = zeros((1, 2, c), torch.float64, x.device)
         d = bn_desc(x, y, eps, momentum, act, residual, 1, sample_scale=sample_scale)
@@ -523,10 +557,12 @@ def bn_act_infer(x, gamma, beta, running_mean, running_var, eps, act, residual=N
     return y
 
 
-def bn_act_bwd(dy, x, y, gamma, mean, rstd, eps, act, want_residual_grad=False, dgamma=None, dbeta=None, beta=None, sample_scale=None, dy2=None):
+def bn_act_bwd(dy, x, y, gamma, mean, rstd, eps, act, want_residual_grad=False, dgamma=None, dbeta=None, beta=None, sample_scale=None, dy2=None, sync=None):
     """Returns (dx, dresidual or None, dgamma, dbeta); dgamma / dbeta are accumulated into when given.
     dy2: the gradient arrives as TWO tensors, dy for channels [0, dy.shape[1]) and dy2 for the rest (two layers that shared one GEMM,
-    functional._DualConvBnAct); both are read in place (SgbBnDesc.dy2).  y may be None when the mask is recomputed from x."""
+    functional._DualConvBnAct); both are read in place (SgbBnDesc.dy2).  y may be None when the mask is recomputed from x.
+    sync: the forward's functional.BnSync -- the reduction pass's sums are all-reduced by sync(sums) before the apply pass, which
+    divides by sync.count and scales the parameter gradients by sync.param_scale."""
     n, c, h, w = x.shape
     dy = as_nhwc(dy)
     if act_code(act) not in (ACT_NONE, ACT_RELU):
@@ -554,9 +590,12 @@ def bn_act_bwd(dy, x, y, gamma, mean, rstd, eps, act, want_residual_grad=False, 
     sums = zeros((2, c), torch.float64, x.device)
     # the forward output is only read when a residual entered the activation; otherwise the mask is recomputed from x
     y_arg = y if (want_residual_grad or beta is None or sample_scale is not None) else None
-    fused = FUSED_BWD[0] and nhwc_pitch(x) == c
+    fused = FUSED_BWD[0] and nhwc_pitch(x) == c and sync is None
     if not fused:
         _timed("sgb_bn_act_bwd_reduce", ctypes.byref(d), _ptr(dy), _ptr(x), _ptr(y_arg), _ptr(gamma), _ptr(beta), _ptr(mean), _ptr(rstd), _ptr(sums), _stream())
+    if sync is not None:
+        sync(sums)
+        d.count, d.param_scale = sync.count.data_ptr(), sync.param_scale
     dx = torch.empty_like(x, memory_format=torch.channels_last) if nhwc_pitch(x) == c else torch.zeros_like(x)
     d.x_pitch = nhwc_pitch(dx)
     # x and dx must share a pitch for the kernel: re-describe x if it is a slice
@@ -596,8 +635,11 @@ def qarep_desc(y3, u, out, eps3, eps_post, momentum, act, use_post_bn) -> L.Qare
     return d
 
 
-def qarep_fwd(y3, u, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp, eps3, eps_post, momentum, act, use_post_bn=True, residual=None, res_alpha=None):
-    """residual / res_alpha: out = act(...) + res_alpha * residual (device scalar): a bottleneck's learnable shortcut in the same pass."""
+def qarep_fwd(y3, u, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp, eps3, eps_post, momentum, act, use_post_bn=True, residual=None, res_alpha=None, sync=None):
+    """residual / res_alpha: out = act(...) + res_alpha * residual (device scalar): a bottleneck's learnable shortcut in the same pass.
+    sync (functional.BnSync): the five moments and the local count are all-reduced by ONE sync(buffer) call between
+    sgb_qarep_moments and sgb_qarep_fwd, which gives both BatchNorms of the block their global statistics; the reduced count is left
+    in sync.count for the backward pass."""
     n, c, h, w = y3.shape
     out = empty_nhwc(n, c, h, w, y3.device)
     d = qarep_desc(y3, u, out, eps3, eps_post, momentum, act, use_post_bn)
@@ -607,6 +649,16 @@ def qarep_fwd(y3, u, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp,
             raise L.SgbError("qarep_fwd: the shortcut must have the output's shape and a one-element fp32 device scale")
         require_cuda(res_alpha, "res_alpha")
         d.pitchr, d.offr, d.res, d.res_alpha = nhwc_pitch(residual), 0, residual.data_ptr(), res_alpha.data_ptr()
+    if sync is not None:
+        coef = torch.empty((9, c), dtype=torch.float32, device=y3.device)
+        buf = new_sync_sums(5 * c, n * h * w, y3.device)
+        mom = buf[:-1].view(5, c)
+        _timed("sgb_qarep_moments", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _stream())
+        sync(buf)
+        sync.count = buf[-1:]
+        d.count, d.param_scale = sync.count.data_ptr(), sync.param_scale
+        _timed("sgb_qarep_fwd", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _ptr(gamma3), _ptr(beta3), _ptr(bias1a), _ptr(gamma_p), _ptr(beta_p), _ptr(rm3), _ptr(rv3), _ptr(rmp), _ptr(rvp), _ptr(out), _ptr(coef), _stream())
+        return out, coef
     mom = zeros((5, c), torch.float64, y3.device)
     coef = torch.empty((9, c), dtype=torch.float32, device=y3.device)
     if FUSED_FWD[0]:  # moments, grid barrier, apply in one cooperative launch
@@ -617,11 +669,12 @@ def qarep_fwd(y3, u, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp,
     return out, coef
 
 
-def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_post_bn=True, acc=None, out_grads=None):
+def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_post_bn=True, acc=None, out_grads=None, sync=None):
     """Returns dy3, du, dgamma3, dbeta3, dbias1a, dgamma_p, dbeta_p.  `acc` optionally supplies existing fp32 tensors
     (dgamma3, dbeta3, dbias1a, dgamma_p, dbeta_p) to accumulate into (None entries are allocated).  The kernel writes dy3 / du
     with the channel pitch of y3 / u: `out_grads` = (dy3, du) buffers of those pitches (e.g. channel slices of one tensor when
-    y3 / u are slices); by default dense tensors are allocated, which requires dense y3 / u."""
+    y3 / u are slices); by default dense tensors are allocated, which requires dense y3 / u.
+    sync: the forward's functional.BnSync -- the three sums are all-reduced by sync(sums) between the two passes."""
     n, c, h, w = y3.shape
     dout = as_nhwc(dout)
     if act_code(act) not in (ACT_NONE, ACT_RELU):
@@ -633,8 +686,12 @@ def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_
         else:
             dout = dout.contiguous(memory_format=torch.channels_last)
     sums = zeros((3, c), torch.float64, y3.device)
-    if not FUSED_BWD[0]:
+    fused = FUSED_BWD[0] and sync is None
+    if not fused:
         _timed("sgb_qarep_bwd_reduce", ctypes.byref(d), _ptr(dout), _ptr(out), _ptr(y3), _ptr(u), _ptr(coef), _ptr(sums), _stream())
+    if sync is not None:
+        sync(sums)
+        d.count, d.param_scale = sync.count.data_ptr(), sync.param_scale
     if out_grads is not None:
         dy3, du = out_grads
         if nhwc_pitch(dy3) != nhwc_pitch(y3) or nhwc_pitch(du) != nhwc_pitch(u):
@@ -644,7 +701,7 @@ def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_
     z = lambda: zeros((c,), torch.float32, y3.device)  # noqa: E731
     acc = acc or (None,) * 5
     dg3, db3, dab, dgp, dbp = [a if a is not None else z() for a in acc]
-    if FUSED_BWD[0]:  # one cooperative launch: reduction, grid barrier, apply
+    if fused:  # one cooperative launch: reduction, grid barrier, apply
         _timed("sgb_qarep_bwd_fused", ctypes.byref(d), _ptr(dout), _ptr(y3), _ptr(u), _ptr(coef), _ptr(sums), _ptr(gamma3), _ptr(gamma_p), _ptr(dy3), _ptr(du), _ptr(dg3), _ptr(db3), _ptr(dab), _ptr(dgp), _ptr(dbp), _stream())
     else:
         _timed("sgb_qarep_bwd_apply", ctypes.byref(d), _ptr(dout), _ptr(out), _ptr(y3), _ptr(u), _ptr(coef), _ptr(sums), _ptr(gamma3), _ptr(gamma_p), _ptr(dy3), _ptr(du), _ptr(dg3), _ptr(db3), _ptr(dab), _ptr(dgp), _ptr(dbp), _stream())

@@ -68,6 +68,9 @@ class BnDesc(Structure):
         ("dy2_off", c_int32),
         ("dy2_reserved", c_int32),
         ("dy2", c_void_p),
+        ("count", c_void_p),
+        ("param_scale", c_float),
+        ("count_reserved", c_int32),
     ]
 
 
@@ -92,6 +95,9 @@ class QarepDesc(Structure):
         ("offr", c_int32),
         ("res", c_void_p),
         ("res_alpha", c_void_p),
+        ("count", c_void_p),
+        ("param_scale", c_float),
+        ("count_reserved", c_int32),
     ]
 
 

@@ -39,6 +39,7 @@ class _FusedConvBN:
         return SF.conv_bn_act(
             x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked,
             stride=stride, pad=pad, eps=bn.eps, momentum=momentum, act=act_code, training=self.training and bn.training, cache=cache, residual=residual, sample_scale=sample_scale,
+            sync=SF.bn_sync(bn),
         )  # fmt: skip
 
 

@@ -104,6 +104,7 @@ class QARepVGGBlock(nn.Module):
                 cfg = SimpleNamespace(
                     stride=self.stride, act=self._act_code, eps=bn3.eps, momentum=0.1 if bn3.momentum is None else bn3.momentum, cache_stem=self._cache_stem,
                     rm3=bn3.running_mean, rv3=bn3.running_var, rmp=pbn.running_mean, rvp=pbn.running_var, nbt=(bn3.num_batches_tracked, pbn.num_batches_tracked),
+                    sync=self._bn_sync(bn3, pbn),
                 )  # fmt: skip
                 if pbn.eps != bn3.eps:
                     raise NotImplementedError("branch and post BatchNorm must share eps")
@@ -114,7 +115,7 @@ class QARepVGGBlock(nn.Module):
                 stride=self.stride, residual=self.identity is not None, act=self._act_code, eps=bn3.eps, momentum=0.1 if bn3.momentum is None else bn3.momentum,
                 use_post_bn=self.use_post_bn, cache3=self._cache3, cache1=self._cache1, cache_fold=self._cache_fold, rm3=bn3.running_mean, rv3=bn3.running_var,
                 rmp=pbn.running_mean if pbn is not None else None, rvp=pbn.running_var if pbn is not None else None,
-                nbt=(bn3.num_batches_tracked, pbn.num_batches_tracked if pbn is not None else None),
+                nbt=(bn3.num_batches_tracked, pbn.num_batches_tracked if pbn is not None else None), sync=self._bn_sync(bn3, pbn),
             )  # fmt: skip
             if pbn is not None and pbn.eps != bn3.eps:
                 raise NotImplementedError("branch and post BatchNorm must share eps")
@@ -143,6 +144,15 @@ class QARepVGGBlock(nn.Module):
                 self._eval_fold = (key, krsc, scale, shift)
             _, krsc, scale, shift = self._eval_fold
             return K.conv_fprop(x, krsc, self.out_channels, 3, 3, self.stride, 1, scale=scale, shift=shift, act=self._act_code)
+
+    @staticmethod
+    def _bn_sync(bn3, pbn):
+        """Cross-rank statistics for the block: the branch BN and post_bn follow from the same five moments, so they are synced
+        together (one collective per direction) and must agree on it."""
+        sync = SF.bn_sync(bn3)
+        if pbn is not None and (sync is None) != (SF.bn_sync(pbn) is None):
+            raise NotImplementedError("QARepVGGBlock: branch BatchNorm and post_bn must both be SyncBatchNorm or both not")
+        return sync
 
     def _eval_source_key(self):
         """Identity + version of every tensor the folded eval kernel is computed from.  The folded kernel itself is a temporary

@@ -438,14 +438,17 @@ class Trainer:
     # ------------------------------------------------------------------------------------------------ train
     def train(self, model: nn.Module, training_params: Mapping[str, Any], train_loader, valid_loader=None, test_loaders=None, additional_configs_to_log=None):
         tp = {**DEFAULT_TRAINING_PARAMS, **dict(training_params or {})}
-        if tp["sync_bn"] and is_distributed():  # on one GPU SyncBatchNorm is plain BatchNorm (the shipped YOLO-NAS recipe sets sync_bn: True)
-            raise NotImplementedError("sync_bn needs per-layer collectives; the data-parallel path uses ONE gradient all-reduce (SURVEY.md D4): set sync_bn=False")
         ckpt = None
         if tp["resume"] or tp["resume_path"]:
             path = tp["resume_path"] or os.path.join(self.checkpoints_dir_path, tp["ckpt_name"])
             ckpt = torch.load(path, map_location="cpu", weights_only=False)
             model.load_state_dict(ckpt["net"], strict=bool(tp["resume_strict_load"]))
         self.net = model.to(self.device)
+        if tp["sync_bn"] and is_distributed():
+            # reference sg_trainer.py:449-456.  The conversion swaps module objects only: the Parameters and buffers (so the state-dict
+            # keys, the flat-buffer layout and the adjacency requests) stay the same objects; the fused blocks see SyncBatchNorm modules
+            # and reduce their statistics across ranks (functional.bn_sync).  On one rank SyncBatchNorm is plain BatchNorm, as in torch.
+            self.net = torch.nn.SyncBatchNorm.convert_sync_batchnorm(self.net)
         torch.manual_seed(int(tp["seed"]) + (torch.distributed.get_rank() if is_distributed() else 0))
         criterion = tp["loss"]
         if isinstance(criterion, (str, Mapping)):
