@@ -55,7 +55,7 @@ class StepContext:
         self.wgrad_table = None
         self.wgrad_key = None
         self.alpha_pending = []   # QARepVGG alpha chain rule of every block, finished by one batched launch (flush_wgrads)
-        self.stem_pending = []    # patch-stem weight gradients, unpacked into the two filters' slots after the join
+        self.stem_pending = []    # patch-stem weight gradients, unpacked into the filters' slots after the join
         self.alpha_table = None
         self.alpha_key = None
         # Weight gradients are off the critical path of backward (nothing consumes them before the optimizer): with a side
@@ -79,44 +79,84 @@ def set_step_context(ctx: Optional["StepContext"]):
         ctx.side_used = False
 
 
+def _tensor_key(t):
+    return None if t is None else (t.data_ptr(), t._version)
+
+
 class WeightCache:
-    """bf16 KRSC / CRSK copies of an fp32 OIHW conv weight, refreshed when the parameter changes."""
+    """bf16 KRSC / CRSK copies of fp32 OIHW filters, refreshed when a source changes.
+
+    get(): one filter, re-laid-out by sgb_weight_prepare.  get_blocks(): several filters applied to the same input, written in
+    place as row blocks of ONE destination by entries of the batched filter re-layout (SgbWeightItem kp / koff / etaps / etap);
+    outside a train step the cache launches its own table.  Inside a train step every cache the model touched contributes its
+    entries to the step's ONE sgb_weight_prepare_batch launch (refresh_weight_caches)."""
 
     def __init__(self, batched: bool = True):
         self.key = None
         self.krsc = None
         self.crsk = None
-        self.args = None  # (w, scale, add_identity, extra_key, c_pad) of the last prepare
+        # (sources, c_pad) of the last get: (w fp32 OIHW, scale or None, add_identity, rows or None, (etaps, etap)) per source
+        self.args = ((), None)
+        self.table = None   # own work table of a multi-source cache, and the batch_ident() it was built for
+        self.table_ident = None
         self.batched = batched  # False: never part of a TrainStep's batched refresh (its source is staged during the forward)
 
     @staticmethod
-    def _key(w, scale, add_identity, extra_key, c_pad):
-        return (w.data_ptr(), w._version, None if scale is None else (scale.data_ptr(), scale._version), add_identity, extra_key, c_pad, _WEIGHT_EPOCH[0])
+    def _key(srcs, c_pad):
+        return tuple((w.data_ptr(), w._version, _tensor_key(scale), add_identity) for w, scale, add_identity, _, _ in srcs) + (c_pad, _WEIGHT_EPOCH[0])
 
-    def get(self, w: torch.Tensor, scale: Optional[torch.Tensor] = None, add_identity=False, extra_key=None, c_pad=None):
+    def get(self, w: torch.Tensor, scale: Optional[torch.Tensor] = None, add_identity=False, c_pad=None):
         """c_pad: channel count of the activation the filter is applied to (>= w.shape[1]; the extra channels are zero)."""
-        key = self._key(w, scale, add_identity, extra_key, c_pad)
+        self.args = (((w, scale, add_identity, None, None),), c_pad)
+        key = self._key(*self.args)
         if key != self.key:
             self.krsc, self.crsk = K.weight_prepare(w, c_pad=c_pad, scale=scale, add_identity=add_identity, out=(self.krsc, self.crsk))
             self.key = key
-            self.args = (w, scale, add_identity, extra_key, c_pad)
+        return self._enrol()
+
+    def get_blocks(self, srcs, r, s, c_pad):
+        """srcs: (w, scale, add_identity, rows, (etaps, etap)) per filter.  The filter is written into rows `rows` (a slice) of the
+        destination KRSC [K, r, s, c_pad] / CRSK [c_pad, r, s, K] (K: the filters' output channels together); etaps > 0 places a 1x1
+        filter at tap `etap` of the destination's etaps taps.  Entries no source writes stay zero from the allocation."""
+        kout, dev = sum(src[0].shape[0] for src in srcs), srcs[0][0].device
+        self.args = (srcs, c_pad)
+        if self.krsc is None or tuple(self.krsc.shape) != (kout, r, s, c_pad) or self.krsc.device != dev:
+            self.krsc = torch.zeros((kout, r, s, c_pad), dtype=torch.bfloat16, device=dev)
+            self.crsk = torch.zeros((c_pad, r, s, kout), dtype=torch.bfloat16, device=dev)
+            self.key = None
+        key = self._key(*self.args)
+        if key != self.key:
+            ident = self.batch_ident()
+            if self.table_ident != ident:
+                self.table = K.weight_prepare_batch(self.batch_entries(), dev)
+                self.table_ident = ident
+            K.run_weight_prepare_batch(*self.table)
+            self.key = key
+        return self._enrol()
+
+    def _enrol(self):
         if _CTX[0] is not None and self.batched:
             _CTX[0].caches.setdefault(id(self), self)
         return self.krsc, self.crsk
 
-    # -- the train step's batched refresh (refresh_weight_caches): one work-table entry per filter
+    # -- the train step's batched refresh (refresh_weight_caches)
     def batch_ready(self, dev) -> bool:
-        return self.args is not None and self.krsc is not None and self.args[0].device == dev and self.args[0].dtype == torch.float32 and self.args[0].is_contiguous()
+        return self.krsc is not None and all(w.device == dev and w.dtype == torch.float32 and w.is_contiguous() for w, *_ in self.args[0])
 
     def batch_ident(self):
-        a = self.args
-        return (a[0].data_ptr(), self.krsc.data_ptr(), None if self.crsk is None else self.crsk.data_ptr(), None if a[1] is None else a[1].data_ptr(), a[2], a[4])
+        srcs, c_pad = self.args
+        srcs = tuple((w.data_ptr(), None if scale is None else scale.data_ptr(), add_identity) for w, scale, add_identity, _, _ in srcs)
+        return (srcs, c_pad, self.krsc.data_ptr(), None if self.crsk is None else self.crsk.data_ptr())
 
     def batch_entries(self):
-        return [(self.args[0], self.args[1], self.krsc, self.crsk, self.krsc.shape[3], self.args[2])]
-
-    def mark_current(self):
-        self.key = WeightCache._key(*self.args)
+        """The sources as weight_prepare_batch entries, one per filter."""
+        srcs, c_pad = self.args
+        if srcs[0][3] is None:  # one filter: the whole destination
+            w, scale, add_identity, _, _ = srcs[0]
+            return [(w, scale, self.krsc, self.crsk, self.krsc.shape[3], add_identity)]
+        kout = self.krsc.shape[0]
+        return [(w, scale, self.krsc[rows], self.crsk, c_pad, bool(add_identity), (kout, rows.start or 0) + taps)
+                for w, scale, add_identity, rows, taps in srcs]  # fmt: skip
 
 
 def refresh_weight_caches(ctx: StepContext, device) -> int:
@@ -134,7 +174,7 @@ def refresh_weight_caches(ctx: StepContext, device) -> int:
     table, n, total = ctx.weight_table
     K.run_weight_prepare_batch(table, n, total)
     for c in live:
-        c.mark_current()
+        c.key = c._key(*c.args)
     return n
 
 
@@ -146,8 +186,9 @@ def flush_wgrads(ctx: StepContext, device) -> int:
         torch.cuda.current_stream().wait_event(ev)
         ctx.side_used = False
     ctx.keep.clear()
-    for dwf, kout, cin, r, s, sw3, sw1 in ctx.stem_pending:
-        _unpack_stem_wgrad(dwf, kout, cin, r, s, sw3, sw1)
+    for dwf, cin, kout, r, s, slots in ctx.stem_pending:
+        for slot, g in zip(slots, _stem_filter_grads(dwf, cin, kout, r, s, len(slots))):
+            slot.add_(g)
     ctx.stem_pending.clear()
     if ctx.alpha_pending:
         ident = tuple(tuple(None if t is None else (t.data_ptr() if torch.is_tensor(t) else t) for t in e) for e in ctx.alpha_pending)
@@ -179,209 +220,29 @@ def flush_wgrads(ctx: StepContext, device) -> int:
     return n + len(rest)
 
 
-# Folded QARepVGG (default; SGB_QAREP_FOLD=0 restores the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
-# of ONE 3x3 convolution with 2K output channels (rows [0, K) = the 3x3 filters, rows [K, 2K) = alpha * K1 + I embedded at the centre),
-# so y3 and u come out of one convolution launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
-# epilogue) and wgrad produces both gradients in one launch (for K <= 64 inside the M = 128 padding the 3x3 weight gradient pays
-# for anyway).  The folded filters are written in place by the step's batched re-layout launch (FoldedWeightCache) and the weight
-# gradient goes to the side stream.
-QAREP_FOLD = [__import__("os").environ.get("SGB_QAREP_FOLD", "1") != "0"]
-QAREP_FOLD_MAXPIX = [int(__import__("os").environ.get("SGB_QAREP_FOLD_MAXPIX", "0"))]  # > 0: fold only maps of at most this many pixels (N*H*W)
-_FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS stride-1 blocks that fold
-
-
-def qarep_fold_supported(cin: int, x_channels: int, kout: int, stride: int) -> bool:
-    return stride == 1 and cin == x_channels and cin in _FOLD_CHANNELS and 2 * kout in _FOLD_CHANNELS
-
-
-class FoldedWeightCache:
-    """bf16 KRSC [2K, 3, 3, C] / CRSK [C, 3, 3, 2K] of the folded filter (K3 ; centre(alpha * K1 + I)), written in place from the two
-    fp32 parameters by two work-table entries of the batched filter re-layout (SgbWeightItem kp / koff / etaps / etap): inside a
-    train step they ride in the step's ONE sgb_weight_prepare_batch launch, outside one the cache launches its own two-entry
-    table.  The destination's never-written entries (the eight outer taps of rows [K, 2K)) stay zero from the allocation."""
+class StagedWeightCache:
+    """A filter the kernels cannot take as it is, staged by torch copies into an fp32 filter they can (patch-channel order, output
+    channels padded), plus the bf16 copies of that stage (an inner WeightCache outside the step's batched refresh: the stage is
+    written during the forward).  The stage is rewritten when a source changes."""
 
     def __init__(self):
         self.key = None
-        self.krsc = None
-        self.crsk = None
-        self.src = None    # (w3, w1, alpha, add_identity, c_pad)
-        self.table = None  # own two-entry table (and the identity it was built for)
-        self.table_ident = None
+        self.stages = None  # fp32 staging tensors, zero-initialised: what fill() does not write stays zero
+        self.inner = WeightCache(batched=False)
 
-    def _key(self):
-        w3, w1, alpha, add_identity, c_pad = self.src
-        return (WeightCache._key(w3, None, False, None, c_pad), WeightCache._key(w1, alpha, add_identity, None, c_pad))
-
-    def get(self, w3, w1, alpha, add_identity, c_pad):
-        self.src = (w3, w1, alpha, add_identity, c_pad)
-        kout, cin = w3.shape[0], w3.shape[1]
-        if c_pad != cin:
-            raise K.L.SgbError("folded QARepVGG filter: the input tensor must have exactly the filter's channel count")
-        if self.krsc is None or tuple(self.krsc.shape) != (2 * kout, 3, 3, c_pad) or self.krsc.device != w3.device:
-            self.krsc = torch.zeros((2 * kout, 3, 3, c_pad), dtype=torch.bfloat16, device=w3.device)
-            self.crsk = torch.zeros((cin, 3, 3, 2 * kout), dtype=torch.bfloat16, device=w3.device)
-            self.key = None
-        key = self._key()
+    def get(self, srcs, shapes, c_pad, fill):
+        """srcs: the tensors the stage is computed from (None entries allowed); shapes: of the staging tensors; fill(*stages) writes
+        them.  Returns the inner cache's (KRSC, CRSK) of the first stage."""
+        key = tuple(_tensor_key(t) for t in srcs) + (tuple(shapes), c_pad, _WEIGHT_EPOCH[0])
         if key != self.key:
-            ident = self.batch_ident()
-            if self.table_ident != ident:
-                self.table = K.weight_prepare_batch(self.batch_entries(), w3.device)
-                self.table_ident = ident
-            K.run_weight_prepare_batch(*self.table)
+            dev = srcs[0].device
+            with torch.no_grad():
+                if self.stages is None or [tuple(t.shape) for t in self.stages] != list(shapes) or self.stages[0].device != dev:
+                    self.stages = [torch.zeros(shape, dtype=torch.float32, device=dev) for shape in shapes]
+                    self.inner.key = None  # a new stage may sit at the old one's address with the same version
+                fill(*self.stages)
             self.key = key
-        if _CTX[0] is not None:
-            _CTX[0].caches.setdefault(id(self), self)
-        return self.krsc, self.crsk
-
-    def batch_ready(self, dev) -> bool:
-        if self.src is None or self.krsc is None:
-            return False
-        w3, w1 = self.src[0], self.src[1]
-        return all(t.device == dev and t.dtype == torch.float32 and t.is_contiguous() for t in (w3, w1))
-
-    def batch_ident(self):
-        w3, w1, alpha, add_identity, c_pad = self.src
-        return (w3.data_ptr(), w1.data_ptr(), None if alpha is None else alpha.data_ptr(), add_identity, self.krsc.data_ptr(), self.crsk.data_ptr())
-
-    def batch_entries(self):
-        w3, w1, alpha, add_identity, c_pad = self.src
-        kout = w3.shape[0]
-        w1_4d = w1 if w1.dim() == 4 else w1.view(w1.shape[0], w1.shape[1], 1, 1)
-        return [
-            (w3, None, self.krsc[:kout], self.crsk, c_pad, False, (2 * kout, 0, 0, 0)),                # rows [0, K): the 3x3 filter
-            (w1_4d, alpha, self.krsc[kout:], self.crsk, c_pad, bool(add_identity), (2 * kout, kout, 9, 4)),  # rows [K, 2K): centre tap
-        ]
-
-    def mark_current(self):
-        self.key = self._key()
-
-
-class ConcatWeightCache:
-    """bf16 KRSC [K1 + K2, R, S, C] / CRSK [C, R, S, K1 + K2] of two filters applied to the same input (the two 1x1 convolutions of a
-    CSP layer as ONE GEMM), written in place from the two fp32 parameters by two entries of the batched filter re-layout, exactly like
-    FoldedWeightCache (SgbWeightItem kp / koff)."""
-
-    def __init__(self):
-        self.key = None
-        self.krsc = None
-        self.crsk = None
-        self.src = None    # (w1, w2, c_pad)
-        self.table = None
-        self.table_ident = None
-
-    def _key(self):
-        w1, w2, c_pad = self.src
-        return (WeightCache._key(w1, None, False, None, c_pad), WeightCache._key(w2, None, False, None, c_pad))
-
-    def get(self, w1, w2, c_pad):
-        self.src = (w1, w2, c_pad)
-        k1, cin, r, s_ = w1.shape
-        k2 = w2.shape[0]
-        if tuple(w2.shape[1:]) != (cin, r, s_) or k1 % 8 != 0 or k2 % 8 != 0:
-            raise K.L.SgbError("concatenated filters need equal input channels / taps and multiples of 8 output channels")
-        if self.krsc is None or tuple(self.krsc.shape) != (k1 + k2, r, s_, c_pad) or self.krsc.device != w1.device:
-            self.krsc = torch.zeros((k1 + k2, r, s_, c_pad), dtype=torch.bfloat16, device=w1.device)
-            self.crsk = torch.zeros((c_pad, r, s_, k1 + k2), dtype=torch.bfloat16, device=w1.device)
-            self.key = None
-        key = self._key()
-        if key != self.key:
-            ident = self.batch_ident()
-            if self.table_ident != ident:
-                self.table = K.weight_prepare_batch(self.batch_entries(), w1.device)
-                self.table_ident = ident
-            K.run_weight_prepare_batch(*self.table)
-            self.key = key
-        if _CTX[0] is not None:
-            _CTX[0].caches.setdefault(id(self), self)
-        return self.krsc, self.crsk
-
-    def batch_ready(self, dev) -> bool:
-        if self.src is None or self.krsc is None:
-            return False
-        return all(t.device == dev and t.dtype == torch.float32 and t.is_contiguous() for t in self.src[:2])
-
-    def batch_ident(self):
-        w1, w2, c_pad = self.src
-        return (w1.data_ptr(), w2.data_ptr(), c_pad, self.krsc.data_ptr(), self.crsk.data_ptr())
-
-    def batch_entries(self):
-        w1, w2, c_pad = self.src
-        k1, k2 = w1.shape[0], w2.shape[0]
-        return [
-            (w1, None, self.krsc[:k1], self.crsk, c_pad, False, (k1 + k2, 0, 0, 0)),
-            (w2, None, self.krsc[k1:], self.crsk, c_pad, False, (k1 + k2, k1, 0, 0)),
-        ]
-
-    def mark_current(self):
-        self.key = self._key()
-
-
-# ------------------------------------------------------------------------------------------------ shared input gradients
-# An activation consumed by several fused blocks (the two 1 x 1 convolutions of a CSP layer, a bottleneck's first block and its
-# shortcut, a backbone feature feeding the next stage and the neck, a head stem feeding the cls / reg branches) receives one
-# gradient per consumer, which autograd sums with an ATen add per extra consumer: 39 full-tensor read-read-write passes per
-# YOLO-NAS-S step (0.78 ms at batch 32).  Every input-gradient kernel here can instead ACCUMULATE into an existing tensor in its
-# epilogue (sgb_conv_dgrad's `accumulate`, sgb_scale_add's in-place form), so the consumers of one tensor object share a token:
-# the first to run backward produces the gradient buffer, the others add into it and return None to autograd, the last returns
-# the buffer.  Autograd's sum is unchanged whatever else consumes the tensor (non-participating consumers are added by autograd
-# as before).  It relies on every registered consumer running in the same backward pass; a pass that reaches only some of them
-# (part of the outputs unused) is detected by a callback at the end of the pass and raises instead of returning wrong gradients
-# The ATen adds disappear, but the accumulating convolution epilogues read the residual row with dependent loads; the mechanism is
-# OFF by default (SGB_SHARE_GRADS=1 turns it on) until those epilogues prefetch the residual through TMA.
-SHARE_GRADS = [__import__("os").environ.get("SGB_SHARE_GRADS", "0") == "1"]
-
-
-class _GradShare:
-    __slots__ = ("n", "arrived", "buf", "queued")
-
-    def __init__(self):
-        self.n = 0          # consumers registered by the forward pass
-        self.arrived = 0    # consumers whose backward ran in the current backward pass
-        self.buf = None     # the gradient accumulated so far
-        self.queued = False
-
-
-def _share_pickup(x):
-    """Called by a block's wrapper with the tensor object the caller passed in; returns the tensor's token (or None)."""
-    if not SHARE_GRADS[0] or not torch.is_tensor(x) or not torch.is_grad_enabled() or not x.requires_grad or x.grad_fn is None:
-        return None
-    tok = x.__dict__.get("_sgb_share") if hasattr(x, "__dict__") else None
-    if tok is None:
-        tok = _GradShare()
-        x._sgb_share = tok
-    tok.n += 1
-    return tok
-
-
-def _share_check(tok):
-    n, a = tok.n, tok.arrived
-    tok.arrived, tok.buf, tok.queued = 0, None, False
-    if a != n:
-        raise RuntimeError(
-            f"shared input gradient: {a} of the {n} fused blocks consuming one activation ran in this backward pass; the gradient of that "
-            "activation would be incomplete.  Backward passes that reach only part of a model's outputs need SGB_SHARE_GRADS=0."
-        )
-
-
-def _share_dx(tok, fresh, accumulate):
-    """The input gradient a backward returns to autograd.  fresh() -> new tensor; accumulate(buf) adds this consumer's gradient
-    into buf in place."""
-    if tok is None or tok.n <= 1:
-        return fresh()
-    if not tok.queued:
-        tok.queued = True
-        torch.autograd.Variable._execution_engine.queue_callback(lambda: _share_check(tok))
-    tok.arrived += 1
-    if tok.buf is None:
-        buf = fresh()
-    else:
-        buf = tok.buf
-        accumulate(buf)
-    if tok.arrived == tok.n:
-        tok.buf = None
-        return buf
-    tok.buf = buf
-    return None
+        return self.inner.get(self.stages[0], c_pad=c_pad)
 
 
 # ------------------------------------------------------------------------------------------------ deferred shortcut gradient
@@ -389,7 +250,7 @@ def _share_dx(tok, fresh, accumulate):
 # ... cv1's dgrad (writes the main-path gradient), then autograd's ATen add of the two (reads both, writes dx): 6 tensor passes and two
 # launches per bottleneck around the dgrad.  With a token the shortcut's backward only parks (dout, alpha, x); cv1's backward runs its
 # dgrad as before and then ONE pass dx = alpha * dout + dx, dot = sum(dout * x) in place (reads dout, x, dx; writes dx): 4 passes, one
-# launch, no ATen add (20 bottlenecks per YOLO-NAS-S step).  Unlike SGB_SHARE_GRADS nothing accumulates inside a GEMM epilogue.
+# launch, no ATen add (20 bottlenecks per YOLO-NAS-S step).
 DEFER_SHORTCUT = [__import__("os").environ.get("SGB_DEFER_SHORTCUT", "1") != "0"]
 
 
@@ -403,7 +264,7 @@ class _DeferTok:
 
 def defer_shortcut_offer(x, alpha):
     """Called by the bottleneck before cv1(x): attaches a token to x for the block that consumes x next (or returns None)."""
-    if not DEFER_SHORTCUT[0] or SHARE_GRADS[0] or not torch.is_grad_enabled() or not torch.is_tensor(x) or not x.requires_grad:
+    if not DEFER_SHORTCUT[0] or not torch.is_grad_enabled() or not torch.is_tensor(x) or not x.requires_grad:
         return None
     if not torch.is_tensor(alpha) or getattr(alpha, "main_grad", None) is None:
         return None
@@ -479,8 +340,9 @@ def bn_sync(bn) -> Optional[BnSync]:
     return BnSync(bn.process_group)
 
 
-def _sync_kw(sync) -> dict:
-    return {"sync": sync} if sync is not None else {}
+def _kw(**kw) -> dict:
+    """The optional keyword arguments that are set (a wrapper's default stands for the others)."""
+    return {k: v for k, v in kw.items() if v is not None}
 
 
 def _mg(p):
@@ -496,54 +358,112 @@ def _deliver(slot, grad):
     return None
 
 
-def _side_wgrad(ctx, x, dy, r, s, stride, pad):
-    """conv_wgrad on the context's side stream (after everything queued so far on the current stream); the result may only
-    be read after flush_wgrads() joined the streams."""
-    dw = K.zeros((dy.shape[1], r, s, x.shape[1]), torch.float32, x.device)  # arena (host-side) or a fill on the current stream
-    main, side = torch.cuda.current_stream(), ctx.side_stream
-    ev = torch.cuda.Event()
-    ev.record(main)
-    with torch.cuda.stream(side):
-        side.wait_event(ev)
-        K.conv_wgrad(x, dy, r, s, stride, pad, dw_krsc=dw)
-    ctx.keep.append((x, dy, dw))
-    ctx.side_used = True
-    return dw
+def _unless_slot(slot, grad):
+    """A gradient a kernel has already accumulated into the parameter's slot when there is one: autograd gets it only without."""
+    return None if slot is not None else grad
 
 
-def _wgrad_raw(x, dy, r, s, stride, pad):
-    """fp32 KRSC weight gradient; on the step's side stream when there is one (readable after flush_wgrads() joined)."""
+def _scalar(v) -> int:
+    """A conv module's stride / padding as one int (the callers checked that it is symmetric)."""
+    return int(v[0]) if isinstance(v, (tuple, list)) else int(v)
+
+
+def _gemm_stats(kout, pixels, device, sync):
+    """BatchNorm statistics buffer for the producing GEMM's epilogue, or None for wide layers: the BatchNorm launch computes them
+    (kernels.stats_in_bn).  With cross-rank statistics the buffer carries the local element count too."""
+    return None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, device, **({"count": pixels} if sync is not None else {}))
+
+
+def _bump_batches_tracked(*nbts):
+    """num_batches_tracked += 1 per BatchNorm, unless a TrainStep bumps every counter at once after the step."""
+    if not _NBT_DEFERRED[0]:
+        for nbt in nbts:
+            if nbt is not None:
+                nbt += 1
+
+
+def _stem_filter_grads(dwf, cin, kout, r, s, n):
+    """Gradient of a staged patch filter (fp32 [n * K, 1, 1, c_out], StagedWeightCache) -> OIHW views of the gradients of its n
+    filters: K3 from the patch channels (r, s, c), then K1 from the centre tap's channels."""
+    g = dwf.reshape(dwf.shape[0], dwf.shape[3])
+    out = [g[:kout, : cin * r * s].reshape(kout, r, s, cin).permute(0, 3, 1, 2)]
+    if n > 1:
+        ctr = ((r // 2) * s + s // 2) * cin
+        out.append(g[kout:, ctr : ctr + cin].reshape(kout, cin, 1, 1))
+    return out
+
+
+def _has_slots(dest) -> bool:
+    kind, slot = dest[0], dest[2]
+    if kind == "stem":
+        return all(t is not None for t in slot)
+    if kind == "alpha":
+        _w1, _alpha, dab, _bias1, sbias, salpha = dest[3]
+        return slot is not None and salpha is not None and (dab is None or sbias is not None)
+    return slot is not None
+
+
+def _wgrad(x, dy, r, s, stride, pad, cin, *dests):
+    """The weight gradient of one convolution, dw = fp32 KRSC conv_wgrad(x, dy), delivered to `dests`:
+      ("oihw", rows, slot)                 dw[rows] -> that filter's OIHW gradient
+      ("alpha", rows, slot, chain)         dw[rows] is the gradient of a QARepVGG block's alpha * K1 + I; chain = (w1, alpha, dab, bias1,
+                                           bias1's slot, alpha's slot) (dab, bias1 None without a 1x1 bias): the chain rule through alpha
+                                           gives the gradients of K1, the bias and alpha
+      ("stem", (kout, r, s), slots)        dw is the gradient of a staged patch filter: the gradients of its len(slots) filters
+    A slot is the parameter's flat gradient slot, or None: the gradient goes to autograd.  Inside a train step, when every
+    destination has its slots, nothing reads the result before flush_wgrads(): the launch goes to the step's side stream (when it
+    has one) and the deliveries wait for the batched passes there.  Otherwise the gradient is computed and delivered now.
+    Returns per destination what autograd receives: a tensor or None ("oihw"), (dK1, dbias, dalpha) ("alpha"), a list ("stem")."""
     ctx = _CTX[0]
-    if ctx is not None and ctx.side_stream is not None:
-        return _side_wgrad(ctx, x, dy, r, s, stride, pad)
-    return K.conv_wgrad(x, dy, r, s, stride, pad)
-
-
-def _wgrad_finish(dw, cin, slot):
-    """fp32 KRSC gradient (rows of dw) -> the parameter's flat gradient slot (deferred to the batched pass inside a step) or OIHW."""
-    ctx = _CTX[0]
-    if slot is not None and ctx is not None:
-        ctx.pending.append((dw, cin, slot))  # dw (step arena or a plain tensor) stays referenced until flush_wgrads()
-        return None
-    if ctx is not None and ctx.side_used:  # no slot: the caller reads the result now
-        torch.cuda.current_stream().wait_stream(ctx.side_stream)
-    if slot is not None:
-        K.wgrad_to_oihw(dw, cin, out=slot, accumulate=True)
-        return None
-    return K.wgrad_to_oihw(dw, cin)
-
-
-def _wgrad(x, dy, r, s, stride, pad, cin, slot):
-    ctx = _CTX[0]
-    if slot is not None and ctx is not None:
-        dw = _side_wgrad(ctx, x, dy, r, s, stride, pad) if ctx.side_stream is not None else K.conv_wgrad(x, dy, r, s, stride, pad)
-        ctx.pending.append((dw, cin, slot))  # dw (step arena or a plain tensor) stays referenced until flush_wgrads()
-        return None
+    if ctx is not None and all(_has_slots(d) for d in dests):
+        if ctx.side_stream is not None:
+            dw = K.zeros((dy.shape[1], r, s, x.shape[1]), torch.float32, x.device)  # arena (host-side) or a fill on the current stream
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream())
+            with torch.cuda.stream(ctx.side_stream):
+                ctx.side_stream.wait_event(ev)
+                K.conv_wgrad(x, dy, r, s, stride, pad, dw_krsc=dw)
+            ctx.keep.append((x, dy, dw))
+            ctx.side_used = True
+        else:
+            dw = K.conv_wgrad(x, dy, r, s, stride, pad)
+        out = []
+        for kind, rows, slot, *chain in dests:  # the queued tensors (step arena or plain) stay referenced until flush_wgrads()
+            if kind == "oihw":
+                ctx.pending.append((dw[rows], cin, slot))
+                out.append(None)
+            elif kind == "alpha":
+                w1, alpha, dab, bias1, sbias, salpha = chain[0]
+                ctx.alpha_pending.append((dw[rows], cin, w1, alpha, dab, bias1, slot, sbias, salpha))
+                out.append((None, None, None))
+            else:
+                ctx.stem_pending.append((dw, cin, *rows, slot))
+                out.append([None] * len(slot))
+        return out
     dw = K.conv_wgrad(x, dy, r, s, stride, pad)
-    if slot is not None:
-        K.wgrad_to_oihw(dw, cin, out=slot, accumulate=True)
-        return None
-    return K.wgrad_to_oihw(dw, cin)
+    out = []
+    for kind, rows, slot, *chain in dests:
+        if kind == "stem":
+            out.append([_deliver(sl, g.contiguous()) for sl, g in zip(slot, _stem_filter_grads(dw, cin, *rows, len(slot)))])
+            continue
+        v = dw[rows]
+        if not v.is_contiguous():  # one tap of a wider filter (a folded QARepVGG's centre tap): [K, C, 1, 1] by a torch copy
+            g = v[:, 0, 0, :cin].reshape(v.shape[0], cin, 1, 1).contiguous()
+        elif kind == "oihw" and slot is not None:
+            K.wgrad_to_oihw(v, cin, out=slot, accumulate=True)
+            out.append(None)
+            continue
+        else:
+            g = K.wgrad_to_oihw(v, cin)
+        if kind == "oihw":
+            out.append(_deliver(slot, g))
+            continue
+        w1, alpha, dab, bias1, sbias, salpha = chain[0]
+        dalpha = (g * w1).sum().reshape(1)
+        if dab is not None:
+            dalpha = dalpha + (dab * bias1).sum().reshape(1)
+        out.append((_deliver(slot, g * alpha), _deliver(sbias, dab * alpha) if dab is not None else None, _deliver(salpha, dalpha)))
+    return out
 
 
 def _chan_sum(dy: torch.Tensor) -> torch.Tensor:
@@ -589,16 +509,11 @@ class _ConvBnAct(torch.autograd.Function):
         krsc, crsk = cfg.cache.get(w, c_pad=x.shape[1])
         kout, _, r, s = w.shape
         p_out = (x.shape[2] + 2 * cfg.pad - r) // cfg.stride + 1, (x.shape[3] + 2 * cfg.pad - s) // cfg.stride + 1
-        # wide layers: no statistics in the GEMM epilogue, the BatchNorm launch computes them (kernels.stats_in_bn)
-        pixels = x.shape[0] * p_out[0] * p_out[1]
-        sync = getattr(cfg, "sync", None)
-        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if sync is not None else {}))
+        stats = _gemm_stats(kout, x.shape[0] * p_out[0] * p_out[1], x.device, cfg.sync)
         y_raw = K.conv_fprop(x, krsc, kout, r, s, cfg.stride, cfg.pad, stats=stats)
         res = K.as_nhwc(residual) if residual is not None else None
-        ss = getattr(cfg, "sample_scale", None)
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, res, **({"sample_scale": ss} if ss is not None else {}), **_sync_kw(sync))
-        if cfg.num_batches_tracked is not None and not _NBT_DEFERRED[0]:
-            cfg.num_batches_tracked += 1
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, res, **_kw(sample_scale=cfg.sample_scale, sync=cfg.sync))
+        _bump_batches_tracked(cfg.num_batches_tracked)
         ctx.save_for_backward(x, y_raw, out, gamma, mean, rstd, beta)
         ctx.cfg, ctx.crsk, ctx.wshape, ctx.has_res = cfg, crsk, tuple(w.shape), residual is not None
         ctx.slots = (_mg(w), _mg(gamma), _mg(beta))
@@ -610,17 +525,10 @@ class _ConvBnAct(torch.autograd.Function):
         cfg = ctx.cfg
         kout, cin, r, s = ctx.wshape
         sw, sg, sb = ctx.slots
-        ss = getattr(cfg, "sample_scale", None)
-        dy, dres, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, out, gamma, mean, rstd, cfg.eps, cfg.act, want_residual_grad=ctx.has_res, dgamma=sg, dbeta=sb, beta=beta, **({"sample_scale": ss} if ss is not None else {}), **_sync_kw(getattr(cfg, "sync", None)))
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = _share_dx(
-                getattr(cfg, "share", None),
-                lambda: K.conv_dgrad(dy, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad),
-                lambda buf: K.conv_dgrad(dy, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad, out=buf, accumulate=True),
-            )
-        dw = _wgrad(x, dy, r, s, cfg.stride, cfg.pad, cin, sw)
-        return dx, dw, (None if sg is not None else dgamma), (None if sb is not None else dbeta), dres, None
+        dy, dres, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, out, gamma, mean, rstd, cfg.eps, cfg.act, want_residual_grad=ctx.has_res, dgamma=sg, dbeta=sb, beta=beta, **_kw(sample_scale=cfg.sample_scale, sync=cfg.sync))
+        dx = K.conv_dgrad(dy, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad) if ctx.needs_input_grad[0] else None
+        (dw,) = _wgrad(x, dy, r, s, cfg.stride, cfg.pad, cin, ("oihw", ..., sw))
+        return dx, dw, _unless_slot(sg, dgamma), _unless_slot(sb, dbeta), dres, None
 
 
 def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracked, *, stride, pad, eps, momentum, act, training, cache: WeightCache, residual=None, sample_scale=None, sync=None):
@@ -631,7 +539,7 @@ def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracke
     K.require_cuda(x, "x")
     if training:
         cfg = SimpleNamespace(stride=stride, pad=pad, eps=eps, momentum=momentum, act=act, cache=cache, running_mean=running_mean, running_var=running_var, num_batches_tracked=num_batches_tracked, sample_scale=sample_scale,
-                              share=_share_pickup(x), sync=sync)  # fmt: skip
+                              sync=sync)  # fmt: skip
         return _ConvBnAct.apply(x, w, gamma, beta, residual, cfg)
     # inference: BN folded into the GEMM epilogue (one kernel)
     with torch.no_grad():
@@ -667,33 +575,13 @@ def conv_stem_patches_supported(conv, bn, x, training) -> bool:
         return False
     w = conv.weight
     r, s = w.shape[2], w.shape[3]
-    stride = conv.stride[0] if isinstance(conv.stride, (tuple, list)) else conv.stride
     if isinstance(conv.stride, (tuple, list)) and len(set(conv.stride)) != 1:
         return False
+    stride = _scalar(conv.stride)
     # the gather stages C * R input rows of (128 - 1) * stride + R pixels in shared memory (sgb_stem_patches_f32: 48 KB)
-    staged = w.shape[1] * r * ((128 - 1) * int(stride) + r) * 4 + (((w.shape[1] * r * s + 31) // 32) * 32) * 4
+    staged = w.shape[1] * r * ((128 - 1) * stride + r) * 4 + (((w.shape[1] * r * s + 31) // 32) * 32) * 4
     return bool(conv.bias is None and conv.groups == 1 and r == s and r > 1 and x.shape[1] == w.shape[1] and w.shape[1] % 8 != 0
                 and w.shape[1] * r * s <= STEM_PATCH_MAX_CHANNELS and w.shape[0] % 8 == 0 and staged + 64 <= 48 * 1024)  # fmt: skip
-
-
-class PatchWeightCache:
-    """fp32 [K, c_out, 1, 1] staging of a first-layer filter in patch-channel order (r, s, c) plus its bf16 KRSC copy."""
-
-    def __init__(self):
-        self.key = None
-        self.stage = None
-        self.inner = WeightCache(batched=False)
-
-    def get(self, w, c_out):
-        key = WeightCache._key(w, None, False, None, c_out)
-        if key != self.key:
-            kout, cin, r, s = w.shape
-            with torch.no_grad():
-                if self.stage is None or tuple(self.stage.shape) != (kout, c_out, 1, 1) or self.stage.device != w.device:
-                    self.stage = torch.zeros((kout, c_out, 1, 1), dtype=torch.float32, device=w.device)
-                self.stage.view(kout, c_out)[:, : cin * r * s].copy_(w.detach().permute(0, 2, 3, 1).reshape(kout, r * s * cin))
-            self.key = key
-        return self.inner.get(self.stage, c_pad=c_out, extra_key=key)
 
 
 class _ConvBnActStem(torch.autograd.Function):
@@ -702,13 +590,12 @@ class _ConvBnActStem(torch.autograd.Function):
         kout, cin, r, s = w.shape
         c_out = ((cin * r * s + 31) // 32) * 32
         xp = K.stem_patches(x, r, cfg.stride, cfg.pad, c_out)
-        kf, _ = cfg.cache.get(w, c_out)
-        pixels = xp.shape[0] * xp.shape[2] * xp.shape[3]
-        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if cfg.sync is not None else {}))
+        # the staged filter [K, c_out, 1, 1]: w in patch-channel order (r, s, c)
+        kf, _ = cfg.cache.get((w,), [(kout, c_out, 1, 1)], c_out, lambda st: st.view(kout, c_out)[:, : cin * r * s].copy_(w.detach().permute(0, 2, 3, 1).reshape(kout, r * s * cin)))
+        stats = _gemm_stats(kout, xp.shape[0] * xp.shape[2] * xp.shape[3], x.device, cfg.sync)
         y_raw = K.conv_fprop(xp, kf, kout, 1, 1, 1, 0, stats=stats)
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, **_sync_kw(cfg.sync))
-        if cfg.num_batches_tracked is not None and not _NBT_DEFERRED[0]:
-            cfg.num_batches_tracked += 1
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, gamma, beta, cfg.running_mean, cfg.running_var, cfg.eps, cfg.momentum, cfg.act, **_kw(sync=cfg.sync))
+        _bump_batches_tracked(cfg.num_batches_tracked)
         ctx.save_for_backward(xp, y_raw, gamma, mean, rstd, beta)
         ctx.cfg, ctx.geom = cfg, (kout, cin, r, s)
         ctx.slots = (_mg(w), _mg(gamma), _mg(beta))
@@ -720,25 +607,16 @@ class _ConvBnActStem(torch.autograd.Function):
         cfg = ctx.cfg
         kout, cin, r, s = ctx.geom
         sw, sg, sb = ctx.slots
-        dy, _, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, None, gamma, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=beta, **_sync_kw(cfg.sync))
-        c = _CTX[0]
-        if c is not None and c.side_stream is not None and sw is not None:
-            dwf = _side_wgrad(c, xp, dy, 1, 1, 1, 0)
-            c.stem_pending.append((dwf, kout, cin, r, s, sw, None))  # unpacked in flush_wgrads(), after the side stream joined
-            dw = None
-        else:
-            dwf = K.conv_wgrad(xp, dy, 1, 1, 1, 0)
-            dw = _deliver(sw, dwf.reshape(kout, dwf.shape[3])[:, : cin * r * s].reshape(kout, r, s, cin).permute(0, 3, 1, 2).contiguous())
-        return None, dw, (None if sg is not None else dgamma), (None if sb is not None else dbeta), None
+        dy, _, dgamma, dbeta = K.bn_act_bwd(dout, y_raw, None, gamma, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=beta, **_kw(sync=cfg.sync))
+        ((dw,),) = _wgrad(xp, dy, 1, 1, 1, 0, cin, ("stem", (kout, r, s), (sw,)))
+        return None, dw, _unless_slot(sg, dgamma), _unless_slot(sb, dbeta), None
 
 
-def conv_bn_act_stem(x, conv, bn, *, act, cache: PatchWeightCache):
+def conv_bn_act_stem(x, conv, bn, *, act, cache: StagedWeightCache):
     """act(bn_train(conv(x))) of a first layer over a raw fp32 NCHW image as a 1 x 1 GEMM over gathered patches; the caller checked
     conv_stem_patches_supported()."""
     K.require_cuda(x, "x")
-    stride = conv.stride[0] if isinstance(conv.stride, (tuple, list)) else conv.stride
-    pad = conv.padding[0] if isinstance(conv.padding, (tuple, list)) else conv.padding
-    cfg = SimpleNamespace(stride=int(stride), pad=int(pad), eps=bn.eps, momentum=0.1 if bn.momentum is None else bn.momentum, act=act, cache=cache,
+    cfg = SimpleNamespace(stride=_scalar(conv.stride), pad=_scalar(conv.padding), eps=bn.eps, momentum=0.1 if bn.momentum is None else bn.momentum, act=act, cache=cache,
                           running_mean=bn.running_mean, running_var=bn.running_var, num_batches_tracked=bn.num_batches_tracked, sync=bn_sync(bn))  # fmt: skip
     return _ConvBnActStem.apply(x, conv.weight, bn.weight, bn.bias, cfg)
 
@@ -784,19 +662,18 @@ class _DualConvBnAct(torch.autograd.Function):
         x = K.as_nhwc(x)
         k1, cin, r, s = w1.shape
         k2 = w2.shape[0]
-        krsc, crsk = cfg.cache.get(w1, w2, x.shape[1])
+        if tuple(w2.shape[1:]) != (cin, r, s) or k1 % 8 != 0 or k2 % 8 != 0:
+            raise K.L.SgbError("concatenated filters need equal input channels / taps and multiples of 8 output channels")
+        # one filter [K1 + K2, R, S, C]: rows [0, K1) = w1, rows [K1, K1 + K2) = w2
+        krsc, crsk = cfg.cache.get_blocks([(w1, None, False, slice(None, k1), (0, 0)), (w2, None, False, slice(k1, None), (0, 0))], r, s, x.shape[1])
         kout = k1 + k2
         p_out = (x.shape[2] + 2 * cfg.pad - r) // cfg.stride + 1, (x.shape[3] + 2 * cfg.pad - s) // cfg.stride + 1
-        pixels = x.shape[0] * p_out[0] * p_out[1]
-        stats = None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, x.device, **({"count": pixels} if cfg.sync is not None else {}))
+        stats = _gemm_stats(kout, x.shape[0] * p_out[0] * p_out[1], x.device, cfg.sync)
         y_raw = K.conv_fprop(x, krsc, kout, r, s, cfg.stride, cfg.pad, stats=stats)
         # gamma / beta / running statistics of the second layer follow the first's in memory: the pointers of the first serve K1 + K2
         # channels (and one collective carries the statistics of both layers)
-        out, mean, rstd = K.bn_act_fwd(y_raw, stats, g1, b1, cfg.rm1, cfg.rv1, cfg.eps, cfg.momentum, cfg.act, **_sync_kw(cfg.sync))
-        if not _NBT_DEFERRED[0]:
-            for nbt in cfg.nbt:
-                if nbt is not None:
-                    nbt += 1
+        out, mean, rstd = K.bn_act_fwd(y_raw, stats, g1, b1, cfg.rm1, cfg.rv1, cfg.eps, cfg.momentum, cfg.act, **_kw(sync=cfg.sync))
+        _bump_batches_tracked(*cfg.nbt)
         ctx.save_for_backward(x, y_raw, g1, b1, mean, rstd)
         ctx.cfg, ctx.crsk, ctx.shape = cfg, crsk, (k1, k2, cin, r, s)
         ctx.slots = (_mg(w1), _mg(w2), _mg(g1), _mg(b1))
@@ -812,52 +689,19 @@ class _DualConvBnAct(torch.autograd.Function):
             n, _, h, w = y_raw.shape
             d1 = d1 if d1 is not None else torch.zeros((n, k1, h, w), dtype=torch.bfloat16, device=x.device).contiguous(memory_format=torch.channels_last)
             d2 = d2 if d2 is not None else torch.zeros((n, k2, h, w), dtype=torch.bfloat16, device=x.device).contiguous(memory_format=torch.channels_last)
-        dy, _, _, _ = K.bn_act_bwd(d1, y_raw, None, g1, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=b1, dy2=d2, **_sync_kw(cfg.sync))
+        dy, _, _, _ = K.bn_act_bwd(d1, y_raw, None, g1, mean, rstd, cfg.eps, cfg.act, dgamma=sg, dbeta=sb, beta=b1, dy2=d2, **_kw(sync=cfg.sync))
         dx = K.conv_dgrad(dy, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad) if ctx.needs_input_grad[0] else None
-        c = _CTX[0]
-        if c is not None:
-            dwf = _wgrad_raw(x, dy, r, s, cfg.stride, cfg.pad)  # fp32 [K1 + K2, R, S, C]: rows of the two filters
-            c.pending.append((dwf[:k1], cin, sw1))
-            c.pending.append((dwf[k1:], cin, sw2))
-        else:
-            dwf = K.conv_wgrad(x, dy, r, s, cfg.stride, cfg.pad)
-            K.wgrad_to_oihw(dwf[:k1], cin, out=sw1, accumulate=True)
-            K.wgrad_to_oihw(dwf[k1:], cin, out=sw2, accumulate=True)
+        _wgrad(x, dy, r, s, cfg.stride, cfg.pad, cin, ("oihw", slice(None, k1), sw1), ("oihw", slice(k1, None), sw2))  # both slots exist (dual_conv_bn_act_ready)
         return dx, None, None, None, None, None, None, None
 
 
-def dual_conv_bn_act(x, conv1, bn1, conv2, bn2, *, act, cache: ConcatWeightCache):
+def dual_conv_bn_act(x, conv1, bn1, conv2, bn2, *, act, cache: WeightCache):
     """(act(bn1(conv1(x))), act(bn2(conv2(x)))) in training mode as one GEMM + one BatchNorm launch; the caller checked
     dual_conv_bn_act_ready().  Reference: modules/conv_bn_act_block.py:92-93 applied twice (training/models/detection_models/yolo_nas/yolo_stages.py:134-135, 144-147)."""
     K.require_cuda(x, "x")
-    stride = conv1.stride[0] if isinstance(conv1.stride, (tuple, list)) else conv1.stride
-    pad = conv1.padding[0] if isinstance(conv1.padding, (tuple, list)) else conv1.padding
-    cfg = SimpleNamespace(stride=int(stride), pad=int(pad), eps=bn1.eps, momentum=0.1 if bn1.momentum is None else bn1.momentum, act=act, cache=cache,
+    cfg = SimpleNamespace(stride=_scalar(conv1.stride), pad=_scalar(conv1.padding), eps=bn1.eps, momentum=0.1 if bn1.momentum is None else bn1.momentum, act=act, cache=cache,
                           rm1=bn1.running_mean, rv1=bn1.running_var, nbt=(bn1.num_batches_tracked, bn2.num_batches_tracked), sync=bn_sync(bn1))  # fmt: skip
     return _DualConvBnAct.apply(x, conv1.weight, bn1.weight, bn1.bias, conv2.weight, bn2.weight, bn2.bias, cfg)
-
-
-class PaddedOutCache:
-    def __init__(self):
-        self.key = None
-        self.stage = None
-        self.bias = None
-        self.inner = WeightCache(batched=False)
-
-    def get(self, w4, b, kp, c_pad):
-        key = (WeightCache._key(w4, None, False, None, c_pad), None if b is None else (b.data_ptr(), b._version), kp)
-        if key != self.key:
-            kout = w4.shape[0]
-            with torch.no_grad():
-                if self.stage is None or tuple(self.stage.shape) != (kp,) + tuple(w4.shape[1:]) or self.stage.device != w4.device:
-                    self.stage = torch.zeros((kp,) + tuple(w4.shape[1:]), dtype=torch.float32, device=w4.device)
-                    self.bias = torch.zeros((kp,), dtype=torch.float32, device=w4.device)
-                self.stage[:kout].copy_(w4.detach())
-                if b is not None:
-                    self.bias[:kout].copy_(b.detach())
-            self.key = key
-        krsc, crsk = self.inner.get(self.stage, c_pad=c_pad, extra_key=key)
-        return krsc, crsk, (self.bias if b is not None else None)
 
 
 def _padded_view(t, kp):
@@ -881,12 +725,18 @@ class _ConvBias(torch.autograd.Function):
             kp = ((kout + 15) // 16) * 16
             pc = cfg.cache.__dict__.get("_kpad")
             if pc is None:
-                pc = cfg.cache._kpad = PaddedOutCache()
-            krsc, crsk, bpad = pc.get(w4, b, kp, x.shape[1])
+                pc = cfg.cache._kpad = StagedWeightCache()
+
+            def fill(stage, bias):  # the filter and bias with zero rows / entries for the padding channels
+                stage[:kout].copy_(w4.detach())
+                if b is not None:
+                    bias[:kout].copy_(b.detach())
+
+            krsc, crsk = pc.get((w4, b), [(kp,) + tuple(w4.shape[1:]), (kp,)], x.shape[1], fill)
             n, _, h, wd = x.shape
             P, Q = (h + 2 * cfg.pad - r) // cfg.stride + 1, (wd + 2 * cfg.pad - s) // cfg.stride + 1
             ybuf = K.empty_nhwc(n, kp, P, Q, x.device)
-            K.conv_fprop(x, krsc, kp, r, s, cfg.stride, cfg.pad, shift=bpad, act=cfg.act, out=ybuf)
+            K.conv_fprop(x, krsc, kp, r, s, cfg.stride, cfg.pad, shift=pc.stages[1] if b is not None else None, act=cfg.act, out=ybuf)
             y = ybuf[:, :kout].detach()  # a plain alias: autograd must not treat the output as a view of a tensor made inside forward
             ctx.kp = kp
         else:
@@ -916,18 +766,9 @@ class _ConvBias(torch.autograd.Function):
                     K.axpby(dy, 1.0, out=dyk[:, :kout])
                 else:
                     dyk[:, :kout].copy_(dy)  # ragged channel count from a producer that did not mark its padding: plain strided copy
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = _share_dx(
-                getattr(cfg, "share", None),
-                lambda: K.conv_dgrad(dyk, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad),
-                lambda buf: K.conv_dgrad(dyk, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad, out=buf, accumulate=True),
-            )
-        if ctx.kp:
-            dwf = _wgrad_raw(x, dyk, r, s, cfg.stride, cfg.pad)  # fp32 [kp, r, s, c]; rows [0, kout) are the filter's gradient
-            dw = _wgrad_finish(dwf[:kout], cin, ctx.slots[0])
-        else:
-            dw = _wgrad(x, dyk, r, s, cfg.stride, cfg.pad, cin, ctx.slots[0])
+        dx = K.conv_dgrad(dyk, ctx.crsk, x.shape, r, s, cfg.stride, cfg.pad) if ctx.needs_input_grad[0] else None
+        # with K padded, rows [0, kout) of the fp32 [kp, r, s, c] gradient are the filter's
+        (dw,) = _wgrad(x, dyk, r, s, cfg.stride, cfg.pad, cin, ("oihw", slice(None, kout) if ctx.kp else ..., ctx.slots[0]))
         if dw is not None:
             dw = dw.reshape(ctx.w_orig_shape)
         db = _deliver(ctx.slots[1], _chan_sum(dy)) if ctx.has_bias else None
@@ -937,11 +778,26 @@ class _ConvBias(torch.autograd.Function):
 def conv_bias(x, w, b, *, stride, pad, cache: WeightCache, act=None):
     """Plain Conv2d (+ bias), e.g. the cls/reg prediction convs (yolo_nas/dfl_heads.py:65-66) and nn.Linear as 1x1."""
     K.require_cuda(x, "x")
-    cfg = SimpleNamespace(stride=stride, pad=pad, cache=cache, act=act, share=_share_pickup(x))
+    cfg = SimpleNamespace(stride=stride, pad=pad, cache=cache, act=act)
     return _ConvBias.apply(x, w, b, cfg)
 
 
 # ------------------------------------------------------------------------------------------------------------ QARepVGG
+# Folded QARepVGG (default; SGB_QAREP_FOLD=0 restores the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
+# of ONE 3x3 convolution with 2K output channels (rows [0, K) = the 3x3 filters, rows [K, 2K) = alpha * K1 + I embedded at the centre),
+# so y3 and u come out of one convolution launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
+# epilogue) and wgrad produces both gradients in one launch (for K <= 64 inside the M = 128 padding the 3x3 weight gradient pays
+# for anyway).  The folded filters are written in place by the step's batched re-layout launch (WeightCache.get_blocks) and the weight
+# gradient goes to the side stream.
+QAREP_FOLD = [__import__("os").environ.get("SGB_QAREP_FOLD", "1") != "0"]
+QAREP_FOLD_MAXPIX = [int(__import__("os").environ.get("SGB_QAREP_FOLD_MAXPIX", "0"))]  # > 0: fold only maps of at most this many pixels (N*H*W)
+_FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS stride-1 blocks that fold
+
+
+def qarep_fold_supported(cin: int, x_channels: int, kout: int, stride: int) -> bool:
+    return stride == 1 and cin == x_channels and cin in _FOLD_CHANNELS and 2 * kout in _FOLD_CHANNELS
+
+
 class _QARepVGG(torch.autograd.Function):
     """Train-mode QARepVGG block (modules/qarepvgg_block.py:184-204) as
         y3 = conv3x3(x);  u = conv1x1_{alpha*K1 + I}(x);  out = act(a3*y3 + au*u + c0)
@@ -953,11 +809,13 @@ class _QARepVGG(torch.autograd.Function):
     def forward(ctx, x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg):
         x = K.as_nhwc(x)
         kout = w3.shape[0]
-        fold = QAREP_FOLD[0] and getattr(cfg, "cache_fold", None) is not None and qarep_fold_supported(w3.shape[1], x.shape[1], kout, cfg.stride)
+        fold = QAREP_FOLD[0] and qarep_fold_supported(w3.shape[1], x.shape[1], kout, cfg.stride)
         if fold and QAREP_FOLD_MAXPIX[0] > 0 and x.shape[0] * x.shape[2] * x.shape[3] > QAREP_FOLD_MAXPIX[0]:
             fold = False
         if fold:
-            kf, cf = cfg.cache_fold.get(w3, w1, alpha, cfg.residual, x.shape[1])
+            # one filter [2K, 3, 3, C]: rows [0, K) = K3, rows [K, 2K) = alpha * K1 + I at the centre tap (tap 4 of 9)
+            srcs = [(w3, None, False, slice(None, kout), (0, 0)), (w1, alpha, cfg.residual, slice(kout, None), (9, 4))]
+            kf, cf = cfg.cache_fold.get_blocks(srcs, 3, 3, x.shape[1])
             ycat = K.conv_fprop(x, kf, 2 * kout, 3, 3, 1, 1)
             y3, u, c3, c1 = ycat[:, :kout], ycat[:, kout:], cf, None
         else:
@@ -968,18 +826,14 @@ class _QARepVGG(torch.autograd.Function):
         ab = None
         if bias1 is not None:
             ab = bias1 * alpha if alpha is not None else bias1
-        sc = getattr(cfg, "shortcut", None)  # (x_s, alpha_s, token): out += alpha_s * x_s in the apply pass (a bottleneck's shortcut)
+        sc = cfg.shortcut  # (x_s, alpha_s, token): out += alpha_s * x_s in the apply pass (a bottleneck's shortcut)
         skw = {"residual": sc[0], "res_alpha": sc[1]} if sc is not None else {}
-        out, coef = K.qarep_fwd(y3, u, g3, b3, ab, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, cfg.use_post_bn, **skw, **_sync_kw(getattr(cfg, "sync", None)))
+        out, coef = K.qarep_fwd(y3, u, g3, b3, ab, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, cfg.use_post_bn, **skw, **_kw(sync=cfg.sync))
         ctx.shortcut = sc
-        if not _NBT_DEFERRED[0]:
-            for nbt in cfg.nbt:
-                if nbt is not None:
-                    nbt += 1
+        _bump_batches_tracked(*cfg.nbt)
         ctx.save_for_backward(x, y3, u, out, coef, g3, gp if gp is not None else g3, w1, bias1 if bias1 is not None else g3, alpha if alpha is not None else g3)
         ctx.cfg, ctx.c3, ctx.c1, ctx.fold = cfg, c3, c1, fold
-        ctx.share = getattr(cfg, "share_tok", None)
-        ctx.defer = getattr(cfg, "defer_tok", None)
+        ctx.defer = cfg.defer_tok
         ctx.flags = (bias1 is not None, alpha is not None, gp is not None, w3.shape[1])
         ctx.slots = (_mg(w3), _mg(g3), _mg(b3), _mg(w1), _mg(bias1), _mg(alpha), _mg(gp), _mg(bp))
         return out
@@ -1002,87 +856,31 @@ class _QARepVGG(torch.autograd.Function):
             dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
         dy3, du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(
             dout, out, y3, u, coef, g3, gp if has_post else None, cfg.eps, cfg.eps, cfg.act, cfg.use_post_bn, acc=(sg3, sb3, direct_bias, sgp, sbp),
-            out_grads=(dcat[:, :kout], dcat[:, kout:]) if dcat is not None else None, **_sync_kw(getattr(cfg, "sync", None)),
+            out_grads=(dcat[:, :kout], dcat[:, kout:]) if dcat is not None else None, **_kw(sync=cfg.sync),
         )  # fmt: skip
+        # the gradient of the 1x1 filter alpha * K1 + I: with a learnable alpha the chain rule gives those of K1, its bias and alpha
+        chain = (w1, alpha, dab if has_bias else None, bias1 if has_bias else None, sbias if has_bias else None, salpha)
+        dest1 = lambda rows: ("alpha", rows, sw1, chain) if has_alpha else ("oihw", rows, sw1)  # noqa: E731
         dx = None
-        dw1f = None
-        tok = ctx.share
-        if dcat is not None:
+        if ctx.fold:
             if ctx.needs_input_grad[0]:
-                dx = _share_dx(tok, lambda: K.conv_dgrad(dcat, ctx.c3, x.shape, 3, 3, 1, 1), lambda buf: K.conv_dgrad(dcat, ctx.c3, x.shape, 3, 3, 1, 1, out=buf, accumulate=True))
+                dx = K.conv_dgrad(dcat, ctx.c3, x.shape, 3, 3, 1, 1)
             dx = _defer_finish(ctx.defer, dx)
-            c = _CTX[0]
-            batched = c is not None and sw3 is not None and sw1 is not None and (not has_alpha or (salpha is not None and (sbias is not None or not has_bias)))
-            # fp32 [2K, 3, 3, C]: rows [0, K) = dW3, rows [K, 2K) centre tap = d(alpha * K1 + I)
-            dwf = _wgrad_raw(x, dcat, 3, 3, 1, 1) if batched else K.conv_wgrad(x, dcat, 3, 3, 1, 1)
-            if batched:
-                # inside a train step nothing reads the gradient before flush_wgrads(): the launch goes to the side stream and both
-                # filters' gradients are delivered by the batched passes (the 1x1 filter's is the centre-tap view of the buffer)
-                c.pending.append((dwf[:kout], cin, sw3))
-                dw1v = dwf[kout:, 1:2, 1:2, :]  # [K, 1, 1, c] view, row pitch 9 * c
-                if has_alpha:
-                    c.alpha_pending.append((dw1v, cin, w1, alpha, dab if has_bias else None, bias1 if has_bias else None, sw1, sbias if has_bias else None, salpha))
-                else:
-                    c.pending.append((dw1v, cin, sw1))
-                dw3 = dw1 = dbias1 = dalpha = None
-                if has_bias and not has_alpha and sbias is None:
-                    dbias1 = dab
-                ret = lambda slot, v: None if slot is not None else v  # noqa: E731
-                return dx, dw3, ret(sg3, dg3), ret(sb3, db3), dw1, dbias1, dalpha, (ret(sgp, dgp) if has_post else None), (ret(sbp, dbp) if has_post else None), None
-            if sw3 is not None and _CTX[0] is not None:
-                _CTX[0].pending.append((dwf[:kout], cin, sw3))
-                dw3 = None
-            elif sw3 is not None:
-                K.wgrad_to_oihw(dwf[:kout], cin, out=sw3, accumulate=True)
-                dw3 = None
-            else:
-                dw3 = K.wgrad_to_oihw(dwf[:kout], cin)
-            dw1f = dwf[kout:, 1, 1, :cin].reshape(kout, cin, 1, 1).contiguous()
+            # fp32 [2K, 3, 3, C]: rows [0, K) = dW3, the centre tap of rows [K, 2K) = d(alpha * K1 + I)
+            dw3, d1 = _wgrad(x, dcat, 3, 3, 1, 1, cin, ("oihw", slice(None, kout), sw3), dest1((slice(kout, None), slice(1, 2), slice(1, 2))))
         else:
             if ctx.needs_input_grad[0]:
-
-                def _fresh():
-                    d = K.conv_dgrad(dy3, ctx.c3, x.shape, 3, 3, cfg.stride, 1)
-                    return K.conv_dgrad(du, ctx.c1, x.shape, 1, 1, cfg.stride, 0, out=d, accumulate=True)
-
-                def _acc(buf):
-                    K.conv_dgrad(dy3, ctx.c3, x.shape, 3, 3, cfg.stride, 1, out=buf, accumulate=True)
-                    K.conv_dgrad(du, ctx.c1, x.shape, 1, 1, cfg.stride, 0, out=buf, accumulate=True)
-
-                dx = _share_dx(tok, _fresh, _acc)
+                dx = K.conv_dgrad(dy3, ctx.c3, x.shape, 3, 3, cfg.stride, 1)
+                K.conv_dgrad(du, ctx.c1, x.shape, 1, 1, cfg.stride, 0, out=dx, accumulate=True)
             dx = _defer_finish(ctx.defer, dx)
-            dw3 = _wgrad(x, dy3, 3, 3, cfg.stride, 1, cin, sw3)
-        dalpha = None
-        if has_alpha and dcat is not None and sw1 is not None and salpha is not None and (sbias is not None or not has_bias):
-            # fold path with flat gradient slots: the same quantities with one launch each (dot / addcmul_) instead of mul + sum + add
-            dalpha_v = torch.dot(dw1f.reshape(-1), w1.reshape(-1))
-            if has_bias:
-                dalpha_v = dalpha_v + torch.dot(dab, bias1)
-                sbias.addcmul_(dab, alpha)
-            sw1.addcmul_(dw1f, alpha)
-            salpha.add_(dalpha_v)
-            dw1 = dbias1 = dalpha = None
-        elif has_alpha and dw1f is None and _CTX[0] is not None and sw1 is not None and salpha is not None and (sbias is not None or not has_bias):
-            # batched plumbing: the 1x1 weight gradient goes to the side stream (when there is one) and the alpha chain rule of
-            # every block is finished by ONE launch in flush_wgrads() instead of ~7 small launches per block
-            c = _CTX[0]
-            dw1k = _side_wgrad(c, x, du, 1, 1, cfg.stride, 0) if c.side_stream is not None else K.conv_wgrad(x, du, 1, 1, cfg.stride, 0)
-            c.alpha_pending.append((dw1k, cin, w1, alpha, dab if has_bias else None, bias1 if has_bias else None, sw1, sbias if has_bias else None, salpha))
-            dw1 = dbias1 = dalpha = None
-        elif has_alpha:
-            if dw1f is None:
-                dw1f = K.wgrad_to_oihw(K.conv_wgrad(x, du, 1, 1, cfg.stride, 0), cin)  # grad of the folded alpha*K1 + I
-            dalpha = (dw1f * w1).sum().reshape(1)
-            if has_bias:
-                dalpha = dalpha + (dab * bias1).sum().reshape(1)
-            dw1 = _deliver(sw1, dw1f * alpha)
-            dbias1 = _deliver(sbias, dab * alpha) if has_bias else None
-            dalpha = _deliver(salpha, dalpha)
+            (dw3,) = _wgrad(x, dy3, 3, 3, cfg.stride, 1, cin, ("oihw", ..., sw3))
+            (d1,) = _wgrad(x, du, 1, 1, cfg.stride, 0, cin, dest1(...))
+        if has_alpha:
+            dw1, dbias1, dalpha = d1
         else:
-            dw1 = _deliver(sw1, dw1f) if dw1f is not None else _wgrad(x, du, 1, 1, cfg.stride, 0, cin, sw1)
-            dbias1 = (None if sbias is not None else dab) if has_bias else None
-        ret = lambda slot, v: None if slot is not None else v  # noqa: E731
-        return dx, dw3, ret(sg3, dg3), ret(sb3, db3), dw1, dbias1, dalpha, (ret(sgp, dgp) if has_post else None), (ret(sbp, dbp) if has_post else None), None
+            dw1, dbias1, dalpha = d1, (_unless_slot(sbias, dab) if has_bias else None), None
+        post = (_unless_slot(sgp, dgp), _unless_slot(sbp, dbp)) if has_post else (None, None)
+        return dx, dw3, _unless_slot(sg3, dg3), _unless_slot(sb3, db3), dw1, dbias1, dalpha, *post, None
 
 
 FUSE_SHORTCUT = [__import__("os").environ.get("SGB_FUSE_SHORTCUT", "1") != "0"]
@@ -1090,8 +888,7 @@ FUSE_SHORTCUT = [__import__("os").environ.get("SGB_FUSE_SHORTCUT", "1") != "0"]
 
 def qarepvgg_block(x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg):
     K.require_cuda(x, "x")
-    cfg.share_tok = _share_pickup(x)  # cfg is built per call by the module
-    cfg.defer_tok = _defer_pickup(x)
+    cfg.defer_tok = _defer_pickup(x)  # cfg is built per call by the module
     return _QARepVGG.apply(x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg)
 
 
@@ -1113,40 +910,6 @@ def stem_patches_supported(block, x) -> bool:
     )  # fmt: skip
 
 
-class StemPatchWeightCache:
-    """fp32 [2K, c_out, 1, 1] staging of the two stem filters in patch-channel order -- rows [0, K): K3 as (r, s, c); rows [K, 2K):
-    K1 at the centre tap's channels -- plus its bf16 KRSC copy, refreshed when a source changes."""
-
-    def __init__(self):
-        self.key = None
-        self.stage = None
-        self.inner = WeightCache(batched=False)
-
-    def get(self, w3, w1, c_out):
-        key = (WeightCache._key(w3, None, False, None, c_out), WeightCache._key(w1, None, False, None, c_out))
-        if key != self.key:
-            kout, cin, r, s = w3.shape
-            with torch.no_grad():
-                if self.stage is None or tuple(self.stage.shape) != (2 * kout, c_out, 1, 1) or self.stage.device != w3.device:
-                    self.stage = torch.zeros((2 * kout, c_out, 1, 1), dtype=torch.float32, device=w3.device)
-                st = self.stage.view(2 * kout, c_out)
-                st[:kout, : cin * r * s].copy_(w3.detach().permute(0, 2, 3, 1).reshape(kout, r * s * cin))
-                ctr = ((r // 2) * s + s // 2) * cin
-                st[kout:, ctr : ctr + cin].copy_(w1.detach()[:, :, 0, 0])
-            self.key = key
-        return self.inner.get(self.stage, c_pad=c_out, extra_key=key)
-
-
-def _unpack_stem_wgrad(dwf, kout, cin, r, s, sw3, sw1):
-    """dwf fp32 [2K, 1, 1, c_out] (gradient of the staged patch filter) -> += into the two OIHW gradient slots."""
-    g = dwf.reshape(dwf.shape[0], dwf.shape[3])
-    sw3.add_(g[:kout, : cin * r * s].reshape(kout, r, s, cin).permute(0, 3, 1, 2))
-    if sw1 is None:  # a plain conv + BN stem (functional._ConvBnActStem): one filter
-        return
-    ctr = ((r // 2) * s + s // 2) * cin
-    sw1.add_(g[kout:, ctr : ctr + cin].reshape(kout, cin, 1, 1))
-
-
 class _QARepVGGStem(torch.autograd.Function):
     """The train-mode QARepVGG stem as ONE 1 x 1 GEMM over gathered patches: y3 = conv3x3_s2(x) and u = conv1x1_s2(x) are the
     first / second K output channels of `patches(x) @ [K3 ; centre(K1)]`.  The im2col engine fetched the 16-channel-padded image
@@ -1159,14 +922,18 @@ class _QARepVGGStem(torch.autograd.Function):
         kout, cin, r, s = w3.shape
         c_out = stem_patch_channels(cin, r)
         xp = K.stem_patches(x, r, cfg.stride, 1, c_out)
-        kf, _ = cfg.cache_stem.get(w3, w1, c_out)
+
+        def fill(stage):  # [2K, c_out, 1, 1]: rows [0, K) = K3 in patch-channel order (r, s, c), rows [K, 2K) = K1 at the centre tap's channels
+            st = stage.view(2 * kout, c_out)
+            st[:kout, : cin * r * s].copy_(w3.detach().permute(0, 2, 3, 1).reshape(kout, r * s * cin))
+            ctr = ((r // 2) * s + s // 2) * cin
+            st[kout:, ctr : ctr + cin].copy_(w1.detach()[:, :, 0, 0])
+
+        kf, _ = cfg.cache_stem.get((w3, w1), [(2 * kout, c_out, 1, 1)], c_out, fill)
         ycat = K.conv_fprop(xp, kf, 2 * kout, 1, 1, 1, 0)
         y3, u = ycat[:, :kout], ycat[:, kout:]
-        out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True, **_sync_kw(getattr(cfg, "sync", None)))
-        if not _NBT_DEFERRED[0]:
-            for nbt in cfg.nbt:
-                if nbt is not None:
-                    nbt += 1
+        out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True, **_kw(sync=cfg.sync))
+        _bump_batches_tracked(*cfg.nbt)
         ctx.save_for_backward(xp, y3, u, out, coef, g3, gp)
         ctx.cfg, ctx.geom, ctx.has_bias = cfg, (kout, cin, r, s), bias1 is not None
         ctx.slots = (_mg(w3), _mg(g3), _mg(b3), _mg(w1), _mg(bias1), _mg(gp), _mg(bp))
@@ -1181,20 +948,9 @@ class _QARepVGGStem(torch.autograd.Function):
         n, _, h, w = y3.shape
         dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
         _dy3, _du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(dout, out, y3, u, coef, g3, gp, cfg.eps, cfg.eps, cfg.act, True, acc=(sg3, sb3, sbias, sgp, sbp),
-                                                         out_grads=(dcat[:, :kout], dcat[:, kout:]), **_sync_kw(getattr(cfg, "sync", None)))  # fmt: skip
-        c = _CTX[0]
-        dw3 = dw1 = None
-        if c is not None and sw3 is not None and sw1 is not None:
-            dwf = _side_wgrad(c, xp, dcat, 1, 1, 1, 0) if c.side_stream is not None else K.conv_wgrad(xp, dcat, 1, 1, 1, 0)
-            c.stem_pending.append((dwf, kout, cin, r, s, sw3, sw1))  # unpacked in flush_wgrads(), after the side stream joined
-        else:
-            dwf = K.conv_wgrad(xp, dcat, 1, 1, 1, 0)
-            g = dwf.reshape(2 * kout, dwf.shape[3])
-            dw3 = _deliver(sw3, g[:kout, : cin * r * s].reshape(kout, r, s, cin).permute(0, 3, 1, 2).contiguous())
-            ctr = ((r // 2) * s + s // 2) * cin
-            dw1 = _deliver(sw1, g[kout:, ctr : ctr + cin].reshape(kout, cin, 1, 1).contiguous())
-        ret = lambda slot, v: None if slot is not None else v  # noqa: E731
-        return None, dw3, ret(sg3, dg3), ret(sb3, db3), dw1, (ret(sbias, dab) if ctx.has_bias else None), ret(sgp, dgp), ret(sbp, dbp), None
+                                                         out_grads=(dcat[:, :kout], dcat[:, kout:]), **_kw(sync=cfg.sync))  # fmt: skip
+        ((dw3, dw1),) = _wgrad(xp, dcat, 1, 1, 1, 0, cin, ("stem", (kout, r, s), (sw3, sw1)))
+        return None, dw3, _unless_slot(sg3, dg3), _unless_slot(sb3, db3), dw1, (_unless_slot(sbias, dab) if ctx.has_bias else None), _unless_slot(sgp, dgp), _unless_slot(sbp, dbp), None
 
 
 def qarepvgg_stem_block(x, w3, g3, b3, w1, bias1, gp, bp, cfg):
@@ -1290,27 +1046,21 @@ def concat(xs):
 
 class _Add(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x1, x2, a, b, tok1, tok2):
+    def forward(ctx, x1, x2, a, b):
         x1, x2 = K.as_nhwc(x1), K.as_nhwc(x2)
         ctx.ab = (a, b)
-        ctx.toks = (tok1, tok2)
         return K.axpby(x1, a, x2, b)
 
     @staticmethod
     def backward(ctx, dy):
         a, b = ctx.ab
         dy = K.as_nhwc(dy)
-        # a scaled branch writes a new tensor anyway, so it can take part in the shared-gradient accumulation; an unscaled branch
-        # hands dy itself to autograd (no kernel) and stays out of it
-        d1 = dy if a == 1.0 else _share_dx(ctx.toks[0], lambda: K.axpby(dy, a), lambda buf: K.axpby(dy, a, buf, 1.0, out=buf))
-        d2 = dy if b == 1.0 else _share_dx(ctx.toks[1], lambda: K.axpby(dy, b), lambda buf: K.axpby(dy, b, buf, 1.0, out=buf))
-        return d1, d2, None, None, None, None
+        return (dy if a == 1.0 else K.axpby(dy, a)), (dy if b == 1.0 else K.axpby(dy, b)), None, None
 
 
 def add(x1, x2, a=1.0, b=1.0):
     """a*x1 + b*x2 (residual connections)."""
-    a, b = float(a), float(b)
-    return _Add.apply(x1, x2, a, b, _share_pickup(x1) if a != 1.0 else None, _share_pickup(x2) if b != 1.0 else None)
+    return _Add.apply(x1, x2, float(a), float(b))
 
 
 class _GlobalAvgPool(torch.autograd.Function):

@@ -77,8 +77,8 @@ class QARepVGGBlock(nn.Module):
         self.partially_fused = False
         self.fully_fused = False
         self._cache3, self._cache1, self._cache_eq = SF.WeightCache(), SF.WeightCache(), SF.WeightCache()
-        self._cache_fold = SF.FoldedWeightCache()
-        self._cache_stem = SF.StemPatchWeightCache()
+        self._cache_fold = SF.WeightCache()
+        self._cache_stem = SF.StagedWeightCache()
         self._eq = None
         self._eval_fold = None  # (key, bf16 KRSC filter, scale, shift) of the on-the-fly eval fold
         if not build_residual_branches:
@@ -115,12 +115,10 @@ class QARepVGGBlock(nn.Module):
                 stride=self.stride, residual=self.identity is not None, act=self._act_code, eps=bn3.eps, momentum=0.1 if bn3.momentum is None else bn3.momentum,
                 use_post_bn=self.use_post_bn, cache3=self._cache3, cache1=self._cache1, cache_fold=self._cache_fold, rm3=bn3.running_mean, rv3=bn3.running_var,
                 rmp=pbn.running_mean if pbn is not None else None, rvp=pbn.running_var if pbn is not None else None,
-                nbt=(bn3.num_batches_tracked, pbn.num_batches_tracked if pbn is not None else None), sync=self._bn_sync(bn3, pbn),
+                nbt=(bn3.num_batches_tracked, pbn.num_batches_tracked if pbn is not None else None), sync=self._bn_sync(bn3, pbn), shortcut=shortcut,
             )  # fmt: skip
             if pbn is not None and pbn.eps != bn3.eps:
                 raise NotImplementedError("branch and post BatchNorm must share eps")
-            if shortcut is not None:
-                cfg.shortcut = shortcut
             alpha = self.alpha if isinstance(self.alpha, torch.Tensor) else None
             return SF.qarepvgg_block(
                 inputs, self.branch_3x3.conv.weight, bn3.weight, bn3.bias, self.branch_1x1.weight, self.branch_1x1.bias, alpha,
@@ -166,10 +164,10 @@ class QARepVGGBlock(nn.Module):
             srcs += [self.post_bn.weight, self.post_bn.bias, self.post_bn.running_mean, self.post_bn.running_var]
         return tuple((t.data_ptr(), t._version) for t in srcs if t is not None)
 
-    def _forward_single_conv(self, x, weight, bias, extra_key=None):
+    def _forward_single_conv(self, x, weight, bias):
         """act(post_bn_eval(conv3x3(x, weight) + bias)) in one GEMM launch."""
         x = K.as_nhwc(x)
-        krsc, _ = self._cache_eq.get(weight, extra_key=extra_key, c_pad=x.shape[1])
+        krsc, _ = self._cache_eq.get(weight, c_pad=x.shape[1])
         if self.use_post_bn and not self.fully_fused:
             pbn = self.post_bn
             if self.training:

@@ -143,7 +143,7 @@ class ResNet(_Classifier):
         self.avgpool = nn.AdaptiveAvgPool2d(1)
         self.width_mult = width_mult
         self._stem_cache, self._fc_cache = SF.WeightCache(), SF.WeightCache()
-        self._stem_patch_cache = SF.PatchWeightCache()
+        self._stem_patch_cache = SF.StagedWeightCache()
 
     def forward(self, x):
         if SF.conv_stem_patches_supported(self.conv1, self.bn1, x, self.training and self.bn1.training):

@@ -42,7 +42,7 @@ class YoloNASDFLHead(BaseDetectionModule):
         self.prior_prob = 1e-2
         self._initialize_biases()
         self._cls_cache, self._reg_cache = SF.WeightCache(), SF.WeightCache()
-        self._cache_pair = SF.ConcatWeightCache()
+        self._cache_pair = SF.WeightCache()
 
     def _first_pair(self):
         """The first cls / reg convolutions read the same tensor (the stem's output; training/models/detection_models/yolo_nas/dfl_heads.py:86-92

@@ -44,7 +44,7 @@ class YoloNASBottleneck(nn.Module):
         if not self.add:
             return y
         if learnable:
-            return _ScaledAdd.apply(x, y, self.alpha, SF._share_pickup(x), tok)
+            return _ScaledAdd.apply(x, y, self.alpha, tok)
         return SF.add(x, y, self.alpha, 1.0)
 
 
@@ -52,13 +52,12 @@ class _ScaledAdd(torch.autograd.Function):
     """alpha * x + y with a learnable scalar alpha read on the device (yolo_stages.py:61-63)."""
 
     @staticmethod
-    def forward(ctx, x, y, alpha, share=None, defer=None):
+    def forward(ctx, x, y, alpha, defer=None):
         from ..... import kernels as K
 
         x, y = K.as_nhwc(x), K.as_nhwc(y)
         ctx.save_for_backward(x, alpha)
         ctx.slot = getattr(alpha, "main_grad", None)
-        ctx.share = share  # x also feeds the block's first convolution: both input gradients land in one buffer (functional._share_dx)
         ctx.defer = defer if ctx.slot is not None else None
         return K.scale_add(x, alpha, y)
 
@@ -72,23 +71,13 @@ class _ScaledAdd(torch.autograd.Function):
             # the block that consumes x (cv1) adds alpha * dy into its own input gradient and accumulates d(alpha) in ONE pass after its
             # dgrad: no gradient tensor for x from here, no ATen add afterwards
             ctx.defer.pending = (dy, alpha, x, ctx.slot)
-            return None, dy, None, None, None
-        dots = []  # alpha * dy (into the shared input-gradient buffer when there is one) and sum(dy * x) in one pass over dy
-
-        def fresh():
-            out, dot = K.scale_add_dot(dy, alpha, x)
-            dots.append(dot)
-            return out
-
-        def acc(buf):
-            dots.append(K.scale_add_dot(dy, alpha, x, buf, out=buf)[1])
-
-        dx = SF._share_dx(ctx.share, fresh, acc)
-        dalpha = dots[0].sum().float().reshape(1)
+            return None, dy, None, None
+        dx, dot = K.scale_add_dot(dy, alpha, x)  # alpha * dy and sum(dy * x) in one pass over dy
+        dalpha = dot.sum().float().reshape(1)
         if ctx.slot is not None:
             ctx.slot.add_(dalpha)
             dalpha = None
-        return dx, dy, dalpha, None, None
+        return dx, dy, dalpha, None
 
 
 class SequentialWithIntermediates(nn.Sequential):
@@ -135,7 +124,7 @@ class YoloNASCSPLayer(nn.Module):
         module_list = [YoloNASBottleneck(hidden_channels, hidden_channels, block_type, activation_type, shortcut, use_alpha, drop_path_rate=drop_path_rates[i]) for i in range(num_bottlenecks)]
         self.bottlenecks = SequentialWithIntermediates(concat_intermediates, *module_list)
         self.dropout = nn.Identity()
-        self._cache12 = SF.ConcatWeightCache()
+        self._cache12 = SF.WeightCache()
 
     def sgb_adjacent_tensors(self):
         """conv1 and conv2 read the same tensor: in training they run as ONE GEMM + ONE BatchNorm launch over the concatenated channels

@@ -915,65 +915,6 @@ def test_trainer_test_returns_loss_items_and_metrics(golden, monkeypatch, tmp_pa
     assert again["loss"] == raw["loss"]  # the EMA swap was undone
 
 
-def test_shared_input_gradients_are_the_same_sum(golden, monkeypatch):
-    """functional._share_dx: consumers of one activation accumulate their input gradients into one buffer instead of leaving the
-    sum to autograd.  (1) A YOLO-NAS CSP layer (two 1x1 convolutions on one input, bottlenecks whose shortcut and first block share
-    an input): output, input gradient and parameter gradients equal the autograd-summed ones up to one bf16 rounding of the sum.
-    (2) A whole train step of the tiny model stays on the same trajectory.  (3) A backward pass that reaches only one of two
-    registered consumers raises instead of returning an incomplete gradient."""
-    from super_gradients_b200 import functional as SF
-    from super_gradients_b200.modules import Conv, QARepVGGBlock
-    from super_gradients_b200.training.models.detection_models.yolo_nas.yolo_stages import YoloNASCSPLayer
-
-    cpu_backend.install_training(monkeypatch)
-
-    def run(share):
-        monkeypatch.setattr(SF, "SHARE_GRADS", [share])
-        torch.manual_seed(3)
-        pre = Conv(16, 32, 1, stride=1, activation_type=torch.nn.ReLU).train()
-        csp = YoloNASCSPLayer(32, 32, 2, QARepVGGBlock, torch.nn.ReLU, True, True, hidden_channels=16).train()
-        with torch.no_grad():
-            for p in list(pre.parameters()) + list(csp.parameters()):
-                p.add_(0.05 * torch.randn_like(p))
-        x = torch.randn(2, 16, 12, 12).bfloat16().contiguous(memory_format=torch.channels_last).requires_grad_(True)
-        y = csp(pre(x))
-        (y.float() * torch.linspace(-1, 1, y.numel()).reshape(y.shape)).sum().backward()
-        grads = {k: p.grad.clone() for k, p in list(pre.named_parameters()) + list(csp.named_parameters()) if p.grad is not None}
-        return y.detach().float(), x.grad.float(), grads
-
-    y0, dx0, g0 = run(False)
-    y1, dx1, g1 = run(True)
-    assert torch.equal(y0, y1)
-    assert l2rel(dx1, dx0) < 8e-3, l2rel(dx1, dx0)
-    assert set(g0) == set(g1)
-    scale = max(float(v.norm()) for v in g0.values())
-    for k in g0:
-        if float(g0[k].norm()) < 1e-4 * scale:  # analytically zero (a bias in front of a BatchNorm): rounding noise on both sides
-            assert float(g1[k].norm()) < 1e-4 * scale, k
-            continue
-        assert l2rel(g1[k], g0[k]) < 2e-2, (k, l2rel(g1[k], g0[k]))
-
-    g = golden("tiny_yolo_nas")
-    x, t = g["x"], _padded_targets(g)
-    res = {}
-    for share in (False, True):
-        monkeypatch.setattr(SF, "SHARE_GRADS", [share])
-        _, st = _train_step(g, monkeypatch)
-        res[share] = _run(st, x, t, 2)
-    assert abs(res[True][0][0] - res[False][0][0]) < 2e-2 * abs(res[False][0][0])
-    assert l2rel(res[True][1][3], res[False][1][3]) < 1e-3  # parameters after two steps
-
-    monkeypatch.setattr(SF, "SHARE_GRADS", [True])
-    torch.manual_seed(4)
-    pre = Conv(16, 16, 1, stride=1, activation_type=torch.nn.ReLU).train()
-    a, b = Conv(16, 16, 1, stride=1, activation_type=torch.nn.ReLU).train(), Conv(16, 16, 1, stride=1, activation_type=torch.nn.ReLU).train()
-    x = torch.randn(2, 16, 8, 8).bfloat16().contiguous(memory_format=torch.channels_last).requires_grad_(True)
-    h = pre(x)
-    ya, _yb = a(h), b(h)
-    with pytest.raises(RuntimeError, match="shared input gradient"):
-        ya.float().sum().backward()
-
-
 def test_k_padded_prediction_conv_is_the_same_conv(monkeypatch):
     """functional.KPAD: a 68-channel 1x1 prediction convolution run with K rounded up to 80 (zero filter rows / bias) returns the
     same output, input gradient, weight and bias gradients as the unpadded call -- both when the incoming gradient's producer
