@@ -454,6 +454,45 @@ typedef struct SgbPreprocDesc {
  * cv2.resize(INTER_LINEAR) + numpy padding / scaling of the reference pipeline followed by a round-to-nearest bf16 store. */
 int sgb_preprocess_u8(const SgbPreprocDesc* d, const uint8_t* src, sgb_bf16* out, void* stream);
 
+/* ---- ImageNet predict() pre-processing of a whole batch (processing.py:614-680 Resize + CenterCrop, transforms/utils.py:28-42
+ *      PIL.Image.resize(BILINEAR), processing.py:1142-1151 default_imagenet_processing_params) ---- */
+/* Per-image table: int64 [batch][SGB_RS_FIELDS] rows of (byte offset of the image's first row in src, source h, w, bytes per source
+ * row, size after Resize (resized_h, resized_w; == h, w: no resize), CenterCrop window origin (crop_top, crop_left)). */
+#define SGB_RS_OFFSET 0
+#define SGB_RS_H 1
+#define SGB_RS_W 2
+#define SGB_RS_PITCH 3
+#define SGB_RS_RESIZED_H 4
+#define SGB_RS_RESIZED_W 5
+#define SGB_RS_CROP_TOP 6
+#define SGB_RS_CROP_LEFT 7
+#define SGB_RS_FIELDS 8
+/* table_host: the table in host memory (validated here, sizes the launch); table: the same table in device memory.  src: device
+ * uint8 buffer of src_bytes holding every H x W x channels image (channels == 3); out: device bf16 [batch, out_h, out_w, out_pitch]
+ * (out_pitch >= channels, a multiple of 8; channels >= `channels` are written as 0).  reverse_channels: output channel c reads
+ * source channel channels - 1 - c (ReverseImageChannels); max_value > 0: v / max_value (StandardizeImage); mean_host / std_host
+ * (NULL: none): (v - mean[c]) / std[c] (NormalizeImage).  ONE launch for the batch: Pillow's antialiased bilinear resize evaluated
+ * only inside each crop window [crop_top, crop_top + out_h) x [crop_left, crop_left + out_w), then the standardisation and a
+ * round-to-nearest bf16 store, bit-exact with the reference pipeline.  A CTA stages the horizontally resized source rows of one
+ * output-row tile in shared memory; a batch whose rows cannot fit in 200 KB (a downscale factor of ~150 at a 224 crop) is
+ * refused with SGB_E_INVALID.  batch == 0 is a no-op. */
+int sgb_resample_crop_u8(const int64_t* table_host, const int64_t* table, const uint8_t* src, int64_t src_bytes, int32_t batch,
+                         int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t reverse_channels,
+                         double max_value, const float* mean_host, const float* std_host, sgb_bf16* out, void* stream);
+
+/* ---- row-wise classification decode (training/metrics/classification_metrics.py:40-78 Accuracy / Top5, utils.py accuracy(),
+ *      pipelines.py:516-531 torch.max(softmax(logits), 1)) ---- */
+/* logits [N, C] (row stride row_stride >= C elements; bf16 when logits_bf16, else f32).  One warp per row, one pass over the row.
+ * Ranking is (value desc, index asc) with NaN above every number: the top-1 index is the first maximum (torch.argmax), and the
+ * target is in the top k when fewer than k elements rank above it.  The target is target[N] (int64) or the argmax of the soft-label
+ * row soft_target[N, C] (row stride target_stride, bf16 when target_bf16, else f32); exactly one of the two when counters are given.
+ * counters[4] (int64, accumulated): top-1 correct, top-k correct (1 <= k <= C), rows, rows whose target is outside [0, C).
+ * label[N] int32 / confidence[N] f32 (each optional): the top-1 index and 1 / sum_j exp(x_j - max), the maximum of
+ * softmax(logits).  N == 0 is a no-op. */
+int sgb_classify_rows(const void* logits, int64_t N, int32_t C, int64_t row_stride, int32_t logits_bf16, const int64_t* target,
+                      const void* soft_target, int64_t target_stride, int32_t target_bf16, int32_t k, int64_t* counters,
+                      int32_t* label, float* confidence, void* stream);
+
 /* ---- optimizer over the flat parameter buffer (sg_trainer.py:634-644) --------------------------------------- */
 /* Hyper-parameters live in DEVICE memory (so a CUDA-graph-captured step follows the host-side LR schedule):
  *   sgd   hp[5] = {lr, momentum, weight_decay, grad_scale, nesterov}

@@ -69,6 +69,13 @@ SGB_HD int resized_u8(const uint8_t* img, int H, int W, int C, int pitch, int ds
   return (((cy.c0 * (d0 >> 4)) >> 16) + ((cy.c1 * (d1 >> 4)) >> 16) + 2) >> 2;
 }
 
+// StandardizeImage (max_value > 0) then NormalizeImage (normalize != 0) of one value of output channel c, in fp32
+SGB_HD float standardize(float v, double max_value, int normalize, float mean, float std) {
+  if (max_value > 0.0) v = (float)((double)v / max_value);  // numpy divides the uint8 image by a Python float (float64), then casts
+  if (normalize) v = (v - mean) / std;                      // float32 arrays in the reference
+  return v;
+}
+
 // value of output channel c at canvas position (oy, ox): resize -> pad -> [reverse] -> standardize -> [normalize], in fp32
 SGB_HD float sample_pixel(const SgbPreprocDesc& d, const uint8_t* src, int oy, int ox, int c) {
   const int sc = d.reverse_channels ? d.src_c - 1 - c : c;
@@ -76,9 +83,7 @@ SGB_HD float sample_pixel(const SgbPreprocDesc& d, const uint8_t* src, int oy, i
   float v;
   if (y >= 0 && y < d.dst_h && x >= 0 && x < d.dst_w) v = (float)resized_u8(src, d.src_h, d.src_w, d.src_c, d.src_pitch, d.dst_h, d.dst_w, y, x, sc);
   else v = d.pad_value;
-  if (d.max_value > 0.0) v = (float)((double)v / d.max_value);  // numpy divides the uint8 image by a Python float (float64), then casts
-  if (d.normalize) v = (v - d.mean[c]) / d.std[c];              // float32 arrays in the reference
-  return v;
+  return standardize(v, d.max_value, d.normalize, d.mean[c], d.std[c]);
 }
 
 }  // namespace sgb_prep

@@ -407,6 +407,56 @@ def preprocess_u8(src, out_slot, dst_hw, pad_tl, pad_value=114.0, max_value=255.
     return out_slot
 
 
+RS_FIELDS = 8  # SGB_RS_FIELDS: (offset, h, w, pitch, resized_h, resized_w, crop_top, crop_left) per image
+
+
+def resample_crop_u8(table_host, table, src, out, max_value=255.0, reverse_channels=False, mean=None, std=None):
+    """Resize + center-crop pre-processing of a whole batch in one launch.  table_host: int64 [B, 8] CPU tensor (offset into `src`,
+    h, w, row pitch, resized h, w, crop top, left), table: the same on the device; src: device uint8 buffer holding the HWC RGB images;
+    out: bf16 NHWC [B, c_pad, out_h, out_w] (channels >= 3 are zeroed)."""
+    require_cuda(src, "src")
+    if table_host.dtype != torch.int64 or table_host.dim() != 2 or table_host.shape[1] != RS_FIELDS or not table_host.is_contiguous() or table_host.is_cuda:
+        raise L.SgbError(f"table_host must be a contiguous int64 [B, {RS_FIELDS}] host tensor")
+    if table.dtype != torch.int64 or tuple(table.shape) != tuple(table_host.shape) or not table.is_contiguous() or src.dtype != torch.uint8:
+        raise L.SgbError("table must be the device copy of table_host and src a uint8 buffer")
+    B, pitch = table_host.shape[0], nhwc_pitch(out)
+    if out.dtype != torch.bfloat16 or out.shape[0] != B or out.shape[1] != pitch:
+        raise L.SgbError("out must be a dense bf16 NHWC batch [B, c_pad, out_h, out_w]")
+    m = s = None
+    if mean is not None:
+        m, s = (ctypes.c_float * 4)(*[float(v) for v in mean][:4]), (ctypes.c_float * 4)(*[float(v) for v in std][:4])
+    _timed("sgb_resample_crop_u8", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel(), B, 3, out.shape[2], out.shape[3], pitch,
+           1 if reverse_channels else 0, float(max_value) if max_value else 0.0, m, s, _ptr(out), _stream())  # fmt: skip
+    return out
+
+
+def classify_rows(logits, target=None, k=1, counters=None, label=None, confidence=None):
+    """Row-wise classification decode of fp32 / bf16 logits [N, C] (unit column stride).  target: int64 [N] class indices or a
+    float [N, C] soft-label tensor (argmax per row); counters: int64 [4] device accumulators (top-1 correct, top-k correct, rows,
+    invalid targets); label int32 [N] / confidence f32 [N]: the top-1 index and the softmax maximum."""
+    require_cuda(logits, "logits")
+    if logits.dim() != 2 or logits.dtype not in (torch.float32, torch.bfloat16) or (logits.shape[1] > 1 and logits.stride(1) != 1):
+        raise L.SgbError(f"logits must be a float32 / bfloat16 [N, C] tensor with unit column stride, got {tuple(logits.shape)} {logits.dtype}")
+    N, C = logits.shape
+    dev = logits.device
+    hard = soft = None
+    if target is not None:
+        if target.device != dev:
+            raise L.SgbError(f"target must live on {dev}")
+        if target.dim() == 1 and target.dtype == torch.int64 and target.shape[0] == N:
+            hard = target.contiguous()
+        elif target.dim() == 2 and tuple(target.shape) == (N, C) and target.dtype in (torch.float32, torch.bfloat16) and (C == 1 or target.stride(1) == 1):
+            soft = target
+        else:
+            raise L.SgbError(f"target must be int64 [N] or float32 / bfloat16 [N, C], got {tuple(target.shape)} {target.dtype} for logits {tuple(logits.shape)}")
+    for name, t, dt in (("counters", counters, torch.int64), ("label", label, torch.int32), ("confidence", confidence, torch.float32)):
+        if t is not None and (t.dtype != dt or not t.is_contiguous() or t.device != dev or t.numel() != (4 if name == "counters" else N)):
+            raise L.SgbError(f"{name} must be a contiguous {dt} tensor of {4 if name == 'counters' else N} elements on {dev}")
+    _timed("sgb_classify_rows", _ptr(logits), N, C, logits.stride(0) if N > 1 else C, 1 if logits.dtype == torch.bfloat16 else 0, _ptr(hard), _ptr(soft),
+           (soft.stride(0) if N > 1 else C) if soft is not None else 0, 1 if soft is not None and soft.dtype == torch.bfloat16 else 0, int(k), _ptr(counters),
+           _ptr(label), _ptr(confidence), _stream())  # fmt: skip
+
+
 # ------------------------------------------------------------------------------------------------ validation metrics
 def match_desc(preds, targets, crowd, n_thresholds, height, width, top_k, denormalize_targets) -> L.MatchDesc:
     d = L.MatchDesc()

@@ -206,6 +206,8 @@ _SIGNATURES = {
     "sgb_focal_cls_fwd_bwd": (c_int, [POINTER(LossDesc), P, P, P, P, c_float, c_float, P, P]),
     "sgb_loss_finalize": (c_int, [POINTER(LossDesc), P, P, P]),
     "sgb_preprocess_u8": (c_int, [POINTER(PreprocDesc), P, P, P]),
+    "sgb_resample_crop_u8": (c_int, [P, P, P, _L, _I, _I, _I, _I, _I, _I, c_double, P, P, P, P]),
+    "sgb_classify_rows": (c_int, [P, _L, _I, _L, _I, P, P, _L, _I, _I, P, P, P, P]),
     "sgb_detection_matching": (c_int, [POINTER(MatchDesc), P, P, P, P, P, P, P, P, P, P]),
     "sgb_pose_keypoint_matching": (c_int, [P] * 10 + [_I] * 6 + [P] * 7),
     "sgb_pose_tal_workspace_bytes": (c_int64, [POINTER(PoseLossDesc)]),

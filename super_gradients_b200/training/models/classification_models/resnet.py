@@ -1,12 +1,15 @@
 """ResNet / CifarResNet with the reference's constructors and state-dict keys
 (training/models/classification_models/resnet.py:26-379).  Every conv-bn(-add)-relu group is one fused call:
 GEMM with fused batch statistics + one normalise/add/ReLU pass (training) or a single GEMM (inference)."""
-from typing import Dict
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 
 from .... import functional as SF
+from .... import kernels as K
 from ....common.registry import register_model
 from ....modules.conv_bn_act_block import _FusedConvBN
 from ....modules.utils import width_multiplier
@@ -68,7 +71,58 @@ class Bottleneck(_Block):
         return self._fused(out, self.conv3, self.bn3, "relu" if self.final_relu else "none", self._caches[2], residual=self._shortcut(x), sample_scale=self.drop_path.sample_scale(x))
 
 
+@dataclass
+class ClassificationPrediction:
+    """One image's result of predict() (training/utils/predict/predictions.py:129-142, plus the class names)."""
+
+    confidence: float
+    label: int
+    image_shape: Tuple[int, ...]
+    class_names: Optional[Sequence[str]] = None
+
+    @property
+    def class_name(self) -> Optional[str]:
+        return self.class_names[self.label] if self.class_names is not None else None
+
+
 class _Classifier(SgModule, _FusedConvBN):
+    _class_names = None
+    _image_processor = None
+
+    def set_dataset_processing_params(self, class_names: Optional[List[str]] = None, image_processor=None) -> None:
+        """base_classifer.py:23-30."""
+        self._class_names = class_names or self._class_names
+        self._image_processor = image_processor or self._image_processor
+
+    @torch.no_grad()
+    def predict(self, images, batch_size: int = 32, fuse_model: bool = True, skip_image_resizing: bool = False, fp16: bool = True) -> List[ClassificationPrediction]:
+        """base_classifer.py:55-73 and the pipeline's decode (pipelines.py:516-531: torch.max(softmax(logits), 1)).  images: one uint8
+        H x W x 3 array or a list of them (any sizes; with skip_image_resizing the Resize / CenterCrop steps are dropped and the images
+        must share one shape), or a pre-processed [B, C, H, W] tensor.  Per batch: one pre-processing launch, one model pass, one decode
+        launch and one device -> host copy.  The compute is bf16 whatever `fp16` says; fuse_model is accepted for the signature."""
+        if self._image_processor is None:
+            raise RuntimeError("You must set the dataset processing parameters before calling predict.\n" "Please call `model.set_dataset_processing_params(...)` first.")
+        processor = self._image_processor.without_resizing() if skip_image_resizing else self._image_processor
+        device = next(self.parameters()).device
+        tensor_input = torch.is_tensor(images)
+        if not tensor_input:
+            images = [images] if isinstance(images, np.ndarray) else list(images)
+        was_training = self.training
+        self.eval()
+        out = []
+        for i in range(0, len(images), batch_size):
+            chunk = images[i : i + batch_size]
+            batch = chunk.to(device) if tensor_input else processor.preprocess_crop_batch(chunk, device)
+            logits = self(batch)
+            res = torch.empty((2, logits.shape[0]), dtype=torch.int32, device=device)  # row 0: label, row 1: confidence (f32 bits)
+            K.classify_rows(logits, label=res[0], confidence=res[1].view(torch.float32))
+            res = res.cpu()
+            labels, conf = res[0].tolist(), res[1].view(torch.float32).tolist()
+            shapes = [tuple(batch.shape[1:])] * len(labels) if tensor_input else [tuple(im.shape) for im in chunk]
+            out += [ClassificationPrediction(confidence=c, label=lb, image_shape=sh, class_names=self._class_names) for lb, c, sh in zip(labels, conf, shapes)]
+        self.train(was_training)
+        return out
+
     def _head(self, out):
         """avgpool -> Linear (as a 1x1 GEMM) -> fp32 logits [N, num_classes]."""
         out = SF.global_avg_pool(out)

@@ -57,6 +57,7 @@ DEFAULT_TRAINING_PARAMS = {
     "silent_mode": True,
     "sync_bn": False,
     "phase_callbacks": [],
+    "train_metrics_list": [],  # metrics updated with every train batch's outputs (sg_trainer.py:1729-1739); reported as train_<name>
     "valid_metrics_list": [],  # metric objects with update(...) / compute() / reset(), e.g. training.metrics.DetectionMetrics_050
     "metric_to_watch": None,  # None: the validation loss; else a key of the metrics' compute() dictionaries (fuzzy-matched like the reference)
     "greater_metric_to_watch_is_better": False,
@@ -160,6 +161,21 @@ def setup_device(device: Optional[str] = None):
     return torch.device("cuda", local_rank)
 
 
+def _update_metrics(metrics, fields: Mapping[str, Any]):
+    """Every metric's update() receives the batch fields it declares (MetricsUpdateCallback, callbacks.py:590-597)."""
+    for m in metrics:
+        accepted = inspect.signature(m.update).parameters
+        m.update(**{k: v for k, v in fields.items() if k in accepted})
+
+
+def _metric_values(metrics) -> Dict[str, float]:
+    values = {}
+    for m in metrics:
+        res = m.compute()
+        values.update({k: float(v) for k, v in res.items()} if isinstance(res, Mapping) else {type(m).__name__: float(res)})
+    return values
+
+
 class _SplitReplay:
     """replay() = graph A, an eagerly issued collective, graph B (TrainStep.capture under data parallelism)."""
 
@@ -178,8 +194,13 @@ class TrainStep:
 
     STAGING_SLOTS = 8  # pinned host slots of the per-step hyper-parameters (how far the host may run ahead of the device)
 
-    def __init__(self, model: nn.Module, criterion: Callable, optimizer: str, optimizer_params: Mapping[str, Any], zero_wd_on_bias_and_bn: bool, ema: bool = False, batch_accumulate: int = 1):
+    def __init__(self, model: nn.Module, criterion: Callable, optimizer: str, optimizer_params: Mapping[str, Any], zero_wd_on_bias_and_bn: bool, ema: bool = False, batch_accumulate: int = 1,
+                 keep_outputs: bool = False):  # fmt: skip
+        """keep_outputs: expose the detached model outputs of the last step as `last_outputs` (train metrics).  Under a captured graph
+        that is the graph's static output buffer, so work enqueued after run() reads the step just replayed."""
         self.model, self.criterion = model, criterion
+        self.keep_outputs = keep_outputs
+        self.last_outputs = None
         self.flat = FlatState(model, zero_wd_on_bias_and_bn)
         self.device = self.flat.params.device
         self.opt_name = optimizer
@@ -269,6 +290,7 @@ class TrainStep:
                 if SF.refresh_weight_caches(self.ctx, self.device):
                     self._filters_stale = False
             outputs = self.model(inputs)
+            self._keep(outputs)
             out = self.criterion(outputs, targets)
             loss, items = out if isinstance(out, tuple) else (out, out.detach().reshape(1))
             loss.backward()
@@ -291,6 +313,7 @@ class TrainStep:
         """The same step with every per-layer launch in place (batched_plumbing = False): the reference behaviour the
         batched path is tested against."""
         outputs = self.model(inputs)
+        self._keep(outputs)
         out = self.criterion(outputs, targets)
         loss, items = out if isinstance(out, tuple) else (out, out.detach().reshape(1))
         loss.backward()
@@ -299,6 +322,10 @@ class TrainStep:
                 p.main_grad.add_(p.grad)
                 p.grad = None
         return loss.detach(), items
+
+    def _keep(self, outputs):
+        if self.keep_outputs:
+            self.last_outputs = outputs.detach() if torch.is_tensor(outputs) else outputs
 
     def optimizer_step(self):
         if self.world > 1:
@@ -458,7 +485,11 @@ class Trainer:
         if isinstance(criterion, nn.Module):
             criterion = criterion.to(self.device)
         self.criterion = criterion
-        self.step = TrainStep(self.net, criterion, tp["optimizer"], tp["optimizer_params"], bool(tp["zero_weight_decay_on_bias_and_bn"]), ema=bool(tp["ema"]), batch_accumulate=int(tp["batch_accumulate"]))
+        from . import metrics as _registered_metrics  # noqa: F401  (fills the METRICS registry)
+
+        train_metrics = [MetricsFactory().get(m) for m in tp["train_metrics_list"] or []]
+        self.step = TrainStep(self.net, criterion, tp["optimizer"], tp["optimizer_params"], bool(tp["zero_weight_decay_on_bias_and_bn"]), ema=bool(tp["ema"]), batch_accumulate=int(tp["batch_accumulate"]),
+                              keep_outputs=bool(train_metrics))  # fmt: skip
         handler = CallbackHandler(tp["phase_callbacks"])
         context = PhaseContext(net=self.net, criterion=criterion, device=self.device, experiment_name=self.experiment_name, ckpt_dir=self.checkpoints_dir_path,
                                train_loader=train_loader, valid_loader=valid_loader, training_params=tp, optimizer=None, context_methods=self)  # fmt: skip
@@ -483,6 +514,8 @@ class Trainer:
             if hasattr(getattr(train_loader, "sampler", None), "set_epoch"):
                 train_loader.sampler.set_epoch(epoch)
             running, nb = None, 0
+            for m in train_metrics:
+                m.reset()
             for batch_idx, batch in enumerate(train_loader):
                 if batch_idx >= steps_per_epoch:
                     break
@@ -509,6 +542,8 @@ class Trainer:
                     handler.fire("on_train_batch_start", context)
                 loss, _items = self.step.run(inputs, targets, do_step)
                 running = loss.clone() if running is None else running + loss  # clone: with a captured graph `loss` is the static output buffer
+                if train_metrics:  # MetricsUpdateCallback at TRAIN_BATCH_END (sg_trainer.py:1264), enqueued behind the step: no sync
+                    _update_metrics(train_metrics, {"preds": self.step.last_outputs, "target": targets, "inputs": inputs, "device": self.device})
                 nb += 1
                 self.history["lr"].append(lr)
                 if handler.callbacks:  # the fused step is over: the reference's per-batch events, in its order
@@ -522,6 +557,7 @@ class Trainer:
             train_loss = float(running / max(nb, 1)) if running is not None else float("nan")
             self.history["train_loss"].append(train_loss)
             metrics = {"train_loss": train_loss}
+            metrics.update({f"train_{k}": v for k, v in _metric_values(train_metrics).items()})  # never collides with the validation keys
             context.update_context(metrics_dict=metrics)
             handler.fire("on_train_loader_end", context)
             if valid_loader is not None and (epoch + 1) % int(tp["run_validation_freq"]) == 0:
@@ -595,14 +631,8 @@ class Trainer:
             n += 1
             if valid_metrics:
                 extra = batch[2] if len(batch) > 2 and isinstance(batch[2], Mapping) else {}
-                fields = {"preds": preds, "target": targets, "inputs": inputs, "device": self.device, **extra}
-                for m in valid_metrics:
-                    accepted = inspect.signature(m.update).parameters
-                    m.update(**{k: v for k, v in fields.items() if k in accepted})
-        values = {}
-        for m in valid_metrics:
-            res = m.compute()
-            values.update({k: float(v) for k, v in res.items()} if isinstance(res, Mapping) else {type(m).__name__: float(res)})
+                _update_metrics(valid_metrics, {"preds": preds, "target": targets, "inputs": inputs, "device": self.device, **extra})
+        values = _metric_values(valid_metrics)
         self.net.train()
         return tot / max(n, 1), (items_tot / max(n, 1) if items_tot is not None else None), values
 
