@@ -399,6 +399,26 @@ int64_t sgb_nms_workspace_bytes(const SgbNmsDesc* d);
 int sgb_batched_nms(const SgbNmsDesc* d, const float* boxes, const float* scores, float* out, int32_t* out_idx,
                     int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- sliding-window detection (sliding_window_detection_forward_wrapper.py:107-166: tiles, per-image merge NMS) ---- */
+/* canvas: bf16 NHWC [B, H, W, pitch] (pitch a multiple of 8), tiles: int32 [T, 3] rows (image, y0, x0) in host (validated here)
+ * and device memory.  out: bf16 NHWC [T, tile, tile, pitch] = canvas[image, y0:y0+tile, x0:x0+tile], zero outside the canvas.
+ * One launch. */
+int sgb_sliding_window_gather(const sgb_bf16* canvas, int32_t B, int32_t H, int32_t W, int32_t pitch, const int32_t* tiles_host,
+                              const int32_t* tiles, int32_t T, int32_t tile, sgb_bf16* out, void* stream);
+/* image_tiles_host [B + 1]: image b owns tiles [image_tiles[b], image_tiles[b + 1]), ascending from 0 to T.  cap = P * the largest
+ * tile count of an image.  0 when the arguments are malformed. */
+int64_t sgb_sliding_window_merge_workspace_bytes(int32_t B, const int32_t* image_tiles_host, int32_t T, int32_t P, int32_t ncls);
+/* rows [T, P, 6] f32 / counts [T] int32: the per-tile NMS result in tile pixels (sgb_batched_nms with max_out P), tiles [T, 3] as
+ * above (device), image_tiles [B + 1] (host and device).  Per image: rows + (x0, y0, x0, y0) in fp32, concatenated in (tile, row)
+ * order, then torchvision's CPU batched_nms(boxes, score, label, iou_thr): the coordinate trick iff 4 n <= 4000, else per-class
+ * NMS.  out [B, cap, 6] f32 rows in (score desc, position asc) order, out_count [B]; a count outside [0, P] or a label outside
+ * [0, ncls) (or not integral) makes out_count[b] -1 / -2.  No host synchronisation; workspace linear in B * cap. */
+int sgb_sliding_window_merge(const float* rows, const int32_t* counts, const int32_t* tiles, const int32_t* image_tiles_host,
+                             const int32_t* image_tiles, int32_t B, int32_t T, int32_t P, int32_t ncls, double iou_thr, float* out,
+                             int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream);
+/* kernels launched by one sgb_sliding_window_merge call with these dimensions */
+int32_t sgb_sliding_window_merge_launches(int32_t B, const int32_t* image_tiles_host, int32_t T, int32_t P);
+
 /* ---- DetectionMetrics matching (SURVEY section 8(f) N4: training/utils/detection_utils.py:1120-1290, IoUMatching :880-1005) ---- */
 #define SGB_MATCH_MAX_THRESHOLDS 32
 typedef struct SgbMatchDesc {

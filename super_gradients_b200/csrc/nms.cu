@@ -12,6 +12,7 @@
 //   * batched_nms uses the coordinate trick when 4*n <= 4000 on CPU, otherwise per-class NMS on the raw boxes;
 //   * IoU arithmetic is fp32 with no fused multiply-add, and `ovr > iou_threshold` is evaluated in double.
 #include "common.cuh"
+#include "nms_math.cuh"
 
 #include <math.h>
 
@@ -36,10 +37,7 @@ struct NmsSmem {
   float fmisc[4];
 };
 
-__device__ __forceinline__ unsigned okey(float f) {
-  unsigned b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
+__device__ __forceinline__ unsigned okey(float f) { return sgb_nms::score_key(f); }
 
 __device__ __forceinline__ bool passes(float s, float thr, int incl) { return incl ? (s >= thr) : (s > thr); }
 
@@ -376,12 +374,7 @@ __global__ void __launch_bounds__(NT, 1) nms_mask_kernel(SgbNmsDesc d, const Nms
       const int jend = min(j0 + 64, nsel);
       for (int j = max(j0, i + 1); j < jend; ++j) {
         if (same_class_only && label[j] != li) continue;
-        float xx1 = fmaxf(ix1, bx[0][j]), yy1 = fmaxf(iy1, bx[1][j]);
-        float xx2 = fminf(ix2, bx[2][j]), yy2 = fminf(iy2, bx[3][j]);
-        float ww = fmaxf(0.f, __fsub_rn(xx2, xx1)), hh = fmaxf(0.f, __fsub_rn(yy2, yy1));
-        float inter = __fmul_rn(ww, hh);
-        float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(ia, area[j]), inter));
-        if ((double)ovr > d.iou_thr) bits |= 1ull << (j - j0);
+        if (sgb_nms::suppresses(ix1, iy1, ix2, iy2, ia, bx[0][j], bx[1][j], bx[2][j], bx[3][j], area[j], d.iou_thr)) bits |= 1ull << (j - j0);
       }
     }
     mrow[i * (KMAX / 64) + w] = bits;
@@ -485,12 +478,12 @@ __global__ void __launch_bounds__(NT, 1) nms_kernel(SgbNmsDesc d, const float* _
     if (t == 0) {
       float m = -INFINITY;
       for (int w = 0; w < 32; ++w) m = fmaxf(m, wmax[w]);
-      S.fmisc[1] = __fadd_rn(m, 1.0f);  // max_coordinate + 1
+      S.fmisc[1] = sgb_nms::offset_step(m);  // max_coordinate + 1
     }
     __syncthreads();
     const float step = S.fmisc[1];
     for (int i = t; i < nsel; i += NT) {
-      float off = __fmul_rn((float)S.label[i], step);
+      float off = sgb_nms::label_offset(S.label[i], step);
       S.bx[0][i] = __fadd_rn(S.bx[0][i], off);
       S.bx[1][i] = __fadd_rn(S.bx[1][i], off);
       S.bx[2][i] = __fadd_rn(S.bx[2][i], off);
@@ -499,7 +492,7 @@ __global__ void __launch_bounds__(NT, 1) nms_kernel(SgbNmsDesc d, const float* _
   }
   __syncthreads();
   for (int i = t; i < nsel; i += NT)
-    S.area[i] = __fmul_rn(__fsub_rn(S.bx[2][i], S.bx[0][i]), __fsub_rn(S.bx[3][i], S.bx[1][i]));
+    S.area[i] = sgb_nms::area(S.bx[0][i], S.bx[1][i], S.bx[2][i], S.bx[3][i]);
   __syncthreads();
 
   }
@@ -534,12 +527,7 @@ __global__ void __launch_bounds__(NT, 1) nms_kernel(SgbNmsDesc d, const float* _
       int jend = min(j0 + 64, nsel);
       for (int j = max(j0, i + 1); j < jend; ++j) {
         if (same_class_only && S.label[j] != li) continue;
-        float xx1 = fmaxf(ix1, S.bx[0][j]), yy1 = fmaxf(iy1, S.bx[1][j]);
-        float xx2 = fminf(ix2, S.bx[2][j]), yy2 = fminf(iy2, S.bx[3][j]);
-        float ww = fmaxf(0.f, __fsub_rn(xx2, xx1)), hh = fmaxf(0.f, __fsub_rn(yy2, yy1));
-        float inter = __fmul_rn(ww, hh);
-        float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(ia, S.area[j]), inter));
-        if ((double)ovr > d.iou_thr) bits |= 1ull << (j - j0);
+        if (sgb_nms::suppresses(ix1, iy1, ix2, iy2, ia, S.bx[0][j], S.bx[1][j], S.bx[2][j], S.bx[3][j], S.area[j], d.iou_thr)) bits |= 1ull << (j - j0);
       }
     }
     S.mask[i * (KMAX / 64) + w] = bits;

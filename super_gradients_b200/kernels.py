@@ -942,8 +942,9 @@ def pose_loss(d, cls_logits, reg_distri, pose_coords, pose_logits, anchor_points
     return out, gc, gr, gp, gl
 
 
-def batched_nms(boxes, scores, score_thr, iou_thr, top_k, max_out, multi_label=True, class_agnostic=False, thr_inclusive=None):
-    """boxes [B,L,4] f32, scores [B,L,C] f32 -> (out [B,max_out,6], out_idx [B,max_out] int32, count [B] int32)."""
+def batched_nms(boxes, scores, score_thr, iou_thr, top_k, max_out, multi_label=True, class_agnostic=False, thr_inclusive=None, out=None, out_idx=None, out_count=None):
+    """boxes [B,L,4] f32, scores [B,L,C] f32 -> (out [B,max_out,6], out_idx [B,max_out] int32, count [B] int32).  out / out_idx /
+    out_count (optional): contiguous tensors of those shapes to write into (e.g. a slice of a larger buffer)."""
     require_cuda(boxes, "boxes")
     B, Lc, C = scores.shape
     d = L.NmsDesc()
@@ -954,13 +955,60 @@ def batched_nms(boxes, scores, score_thr, iou_thr, top_k, max_out, multi_label=T
     d.thr_inclusive = int(not multi_label) if thr_inclusive is None else int(bool(thr_inclusive))
     boxes = boxes.contiguous().float()
     scores = scores.contiguous().float()
-    out = torch.empty((B, max_out, 6), dtype=torch.float32, device=boxes.device)
-    oidx = torch.empty((B, max_out), dtype=torch.int32, device=boxes.device)
-    cnt = torch.empty((B,), dtype=torch.int32, device=boxes.device)
+    for t, shape, dt, name in ((out, (B, max_out, 6), torch.float32, "out"), (out_idx, (B, max_out), torch.int32, "out_idx"), (out_count, (B,), torch.int32, "out_count")):
+        if t is not None and (tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous() or t.device != boxes.device):
+            raise L.SgbError(f"{name} must be a contiguous {dt} tensor of shape {shape} on {boxes.device}")
+    out = torch.empty((B, max_out, 6), dtype=torch.float32, device=boxes.device) if out is None else out
+    oidx = torch.empty((B, max_out), dtype=torch.int32, device=boxes.device) if out_idx is None else out_idx
+    cnt = torch.empty((B,), dtype=torch.int32, device=boxes.device) if out_count is None else out_count
     nbytes = L.load().sgb_nms_workspace_bytes(ctypes.byref(d))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=boxes.device)
     _timed("sgb_batched_nms", ctypes.byref(d), _ptr(boxes), _ptr(scores), _ptr(out), _ptr(oidx), _ptr(cnt), _ptr(ws), nbytes, _stream())
     return out, oidx, cnt
+
+
+def sliding_window_gather(canvas, tiles_host, tiles, tile, out=None):
+    """canvas: bf16 NHWC [B, pitch, H, W]; tiles_host / tiles: int32 [T, 3] rows (image, y0, x0) on the host / the device ->
+    bf16 NHWC [T, pitch, tile, tile] = canvas[image, :, y0:y0+tile, x0:x0+tile], zero outside the canvas (one launch)."""
+    require_cuda(canvas, "canvas")
+    B, C, H, W = canvas.shape
+    pitch = nhwc_pitch(canvas)
+    if canvas.dtype != torch.bfloat16 or C != pitch:
+        raise L.SgbError("canvas must be a dense bf16 NHWC tensor (all its channels)")
+    T = tiles_host.shape[0]
+    for t, dev in ((tiles_host, False), (tiles, True)):
+        if t.dtype != torch.int32 or t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous() or t.is_cuda != dev or t.shape[0] != T:
+            raise L.SgbError("tiles_host / tiles must be contiguous int32 [T, 3] tensors on the host / the device")
+    if out is None:
+        out = empty_nhwc(T, C, tile, tile, canvas.device)
+    elif tuple(out.shape) != (T, C, tile, tile) or out.dtype != torch.bfloat16 or nhwc_pitch(out) != pitch:
+        raise L.SgbError(f"out must be a dense bf16 NHWC [{T}, {C}, {tile}, {tile}] tensor")
+    _timed("sgb_sliding_window_gather", _ptr(canvas), B, H, W, pitch, ctypes.c_void_p(tiles_host.data_ptr()), _ptr(tiles), T, int(tile), _ptr(out), _stream())
+    return out
+
+
+def sliding_window_merge(rows, counts, tiles, image_tiles_host, image_tiles, ncls, iou_thr):
+    """rows [T, P, 6] f32 / counts [T] int32: the per-tile NMS result in tile pixels; tiles int32 [T, 3] (image, y0, x0) and
+    image_tiles int32 [B + 1] (image b owns tiles [image_tiles[b], image_tiles[b + 1])) on the device, image_tiles_host its host
+    copy.  -> (out [B, cap, 6] f32 rows in canvas pixels, count [B] int32): the reference's per-image merge (shift by the tile
+    origin, concatenate, torchvision CPU batched_nms); a negative count marks a malformed input row of that image."""
+    require_cuda(rows, "rows")
+    T, P, six = rows.shape
+    B = image_tiles_host.shape[0] - 1
+    if six != 6 or rows.dtype != torch.float32 or not rows.is_contiguous() or counts.dtype != torch.int32 or tuple(counts.shape) != (T,):
+        raise L.SgbError("rows must be a contiguous f32 [T, P, 6] tensor and counts an int32 [T] tensor")
+    if image_tiles_host.dtype != torch.int32 or image_tiles_host.is_cuda or image_tiles.dtype != torch.int32 or tuple(image_tiles.shape) != (B + 1,) or B < 1:
+        raise L.SgbError("image_tiles_host / image_tiles must be int32 [B + 1] tensors on the host / the device")
+    it = ctypes.c_void_p(image_tiles_host.data_ptr())
+    lib = L.load()
+    nbytes = lib.sgb_sliding_window_merge_workspace_bytes(B, it, T, P, int(ncls))
+    cap = P * int((image_tiles_host[1:] - image_tiles_host[:-1]).max())
+    out = torch.empty((B, cap, 6), dtype=torch.float32, device=rows.device)
+    cnt = torch.empty((B,), dtype=torch.int32, device=rows.device)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=rows.device)
+    _timed("sgb_sliding_window_merge", _ptr(rows), _ptr(counts), _ptr(tiles), it, _ptr(image_tiles), B, T, P, int(ncls), float(iou_thr), _ptr(out), _ptr(cnt), _ptr(ws), nbytes, _stream())
+    L.LAUNCHES[0] += lib.sgb_sliding_window_merge_launches(B, it, T, P) - 1
+    return out, cnt
 
 
 # ------------------------------------------------------------------------------------------------ optimizer

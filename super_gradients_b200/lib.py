@@ -215,6 +215,10 @@ _SIGNATURES = {
     "sgb_pose_loss_fwd_bwd": (c_int, [POINTER(PoseLossDesc)] + [P] * 12 + [_F] + [P] * 5),
     "sgb_pose_loss_finalize": (c_int, [POINTER(PoseLossDesc), P, P, P]),
     "sgb_head_grad_scatter": (c_int, [P, _I, _I, _I, _I, _I, P, _I, P]),
+    "sgb_sliding_window_gather": (c_int, [P, _I, _I, _I, _I, P, P, _I, _I, P, P]),
+    "sgb_sliding_window_merge_workspace_bytes": (c_int64, [_I, P, _I, _I, _I]),
+    "sgb_sliding_window_merge": (c_int, [P, P, P, P, P, _I, _I, _I, _I, c_double, P, P, P, _L, P]),
+    "sgb_sliding_window_merge_launches": (c_int32, [_I, P, _I, _I]),
     "sgb_nms_workspace_bytes": (c_int64, [POINTER(NmsDesc)]),
     "sgb_batched_nms": (c_int, [POINTER(NmsDesc), P, P, P, P, P, P, _L, P]),
     "sgb_sgd_step": (c_int, [P, P, P, _L, P, P]),
@@ -225,7 +229,7 @@ _SIGNATURES = {
 _lib = None
 
 # kernels launched by one call of each entry point (default 1); LAUNCHES[0] accumulates them (bench.py: gpu_launches)
-LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
+LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
 LAUNCHES = [0]
 
 

@@ -94,16 +94,34 @@ class CustomizableDetector(SgModule):
         if class_agnostic_nms is not None:
             self._default_class_agnostic_nms = bool(class_agnostic_nms)
 
+    def get_dataset_processing_params(self):
+        """customizable_detector.py:197-207, including its `conf=self._default_nms_iou` (DESIGN.md section 4)."""
+        return dict(class_names=self._class_names, image_processor=self._image_processor, iou=self._default_nms_iou, conf=self._default_nms_iou,
+                    nms_top_k=self._default_nms_top_k, max_predictions=self._default_max_predictions, multi_label_per_box=self._default_multi_label_per_box,
+                    class_agnostic_nms=self._default_class_agnostic_nms)  # fmt: skip
+
+    def get_processing_params(self):
+        return self._image_processor
+
+    def image_processor_for_predict(self, skip_image_resizing: bool = False):
+        """The chain predict() runs on raw images: the model's image processor -- the YOLO-NAS COCO chain when none was set, where the
+        reference's pipeline raises (DESIGN.md section 4.9) -- or with skip_image_resizing its equivalent without resizing."""
+        from ...processing import default_yolo_nas_coco_processing_params
+
+        return (self._image_processor or default_yolo_nas_coco_processing_params()["image_processor"]).for_predict(skip_image_resizing)
+
     @torch.no_grad()
-    def predict(self, images, iou=None, conf=None, batch_size: int = 32, fuse_model: bool = True, nms_top_k=None, max_predictions=None, multi_label_per_box=None, class_agnostic_nms=None):
+    def predict(self, images, iou=None, conf=None, batch_size: int = 32, fuse_model: bool = True, skip_image_resizing: bool = False, nms_top_k=None, max_predictions=None,
+                multi_label_per_box=None, class_agnostic_nms=None, fp16: bool = True):  # fmt: skip
         """images: either a pre-processed tensor [B, C, H, W], or raw images -- one uint8 H x W x C array or a list of them (any
         sizes) -- which go through the model's image processor (set_dataset_processing_params; default: the YOLO-NAS COCO chain)
         as ONE fused GPU launch per image (training/processing/processing.py) and whose boxes come back in original-image pixels,
-        like the reference's Pipeline (training/pipelines/pipelines.py:192-216).
-        Returns a list (one per image) of [Ni, 6] tensors (x1, y1, x2, y2, confidence, class)."""
+        like the reference's Pipeline (training/pipelines/pipelines.py:192-216).  skip_image_resizing: the chain without its resizing
+        steps, padded bottom / right to a multiple of 32.  fp16 is accepted for the reference's signature: the model always runs its
+        bf16 kernels.  Returns a list (one per image) of [Ni, 6] tensors (x1, y1, x2, y2, confidence, class)."""
         if not torch.is_tensor(images):
             return self._predict_raw_images(images, dict(iou=iou, conf=conf, nms_top_k=nms_top_k, max_predictions=max_predictions, multi_label_per_box=multi_label_per_box,
-                                                         class_agnostic_nms=class_agnostic_nms), batch_size)  # fmt: skip
+                                                         class_agnostic_nms=class_agnostic_nms), batch_size, skip_image_resizing)  # fmt: skip
         cb = self.get_post_prediction_callback(
             conf=self._default_nms_conf if conf is None else conf,
             iou=self._default_nms_iou if iou is None else iou,
@@ -120,13 +138,11 @@ class CustomizableDetector(SgModule):
         self.train(was_training)
         return out
 
-    def _predict_raw_images(self, images, kw, batch_size):
-        from ...processing import default_yolo_nas_coco_processing_params
-
+    def _predict_raw_images(self, images, kw, batch_size, skip_image_resizing=False):
         import numpy as np
 
         images = [images] if isinstance(images, np.ndarray) else list(images)
-        processor = self._image_processor or default_yolo_nas_coco_processing_params()["image_processor"]
+        processor = self.image_processor_for_predict(skip_image_resizing)
         device = next(self.parameters()).device
         dflt = dict(conf=self._default_nms_conf, iou=self._default_nms_iou, nms_top_k=self._default_nms_top_k, max_predictions=self._default_max_predictions,
                     multi_label_per_box=self._default_multi_label_per_box, class_agnostic_nms=self._default_class_agnostic_nms)  # fmt: skip

@@ -25,14 +25,19 @@ class PPYoloEPostPredictionCallback(DetectionPostPredictionCallback):
         self.class_agnostic_nms = class_agnostic_nms
 
     @torch.no_grad()
-    def forward_batched(self, outputs: Any) -> Tuple[Tensor, Tensor, Tensor]:
-        """Device-resident result: rows [B, max_predictions, 6], flat candidate index [B, max_predictions], count [B]."""
+    def forward_batched(self, outputs: Any, out=None, out_idx=None, out_count=None) -> Tuple[Tensor, Tensor, Tensor]:
+        """Device-resident result: rows [B, max_predictions, 6], flat candidate index [B, max_predictions], count [B] (written into
+        out / out_idx / out_count when given, see kernels.batched_nms)."""
         pred_bboxes, pred_scores = self._get_decoded_predictions_from_model_output(outputs)
-        max_out = min(int(self.max_predictions), 1024)
+        dest = {k: v for k, v in dict(out=out, out_idx=out_idx, out_count=out_count).items() if v is not None}
         return K.batched_nms(
-            pred_bboxes, pred_scores, self.score_threshold, self.nms_threshold, self.nms_top_k, max_out,
-            multi_label=self.multi_label_per_box, class_agnostic=self.class_agnostic_nms,
+            pred_bboxes, pred_scores, self.score_threshold, self.nms_threshold, self.nms_top_k, self.max_rows(),
+            multi_label=self.multi_label_per_box, class_agnostic=self.class_agnostic_nms, **dest,
         )  # fmt: skip
+
+    def max_rows(self) -> int:
+        """Row pitch of forward_batched's result."""
+        return min(int(self.max_predictions), 1024)
 
     @torch.no_grad()
     def forward(self, outputs: Any, device: str = None) -> List[Tensor]:

@@ -6,7 +6,8 @@ padding and rescaling on the prediction tensors with the reference's float32 ari
 
 Supported chains, each step optional, in this order:
   detection (the YOLO-NAS / YOLO-NAS-POSE defaults, processing.py:960-980, 1060-1075): ReverseImageChannels, one *Rescale, one
-  *Padding, StandardizeImage, NormalizeImage, ImagePermute((2, 0, 1)) -- one launch per image (csrc/preprocess.cu);
+  *Padding, StandardizeImage, NormalizeImage, ImagePermute((2, 0, 1)) -- one launch per image (csrc/preprocess.cu); for
+  predict(skip_image_resizing=True) a DetectionAutoPadding first instead of the rescale and padding steps;
   classification (the ImageNet default, processing.py:1142-1151): ReverseImageChannels, Resize, CenterCrop, StandardizeImage,
   NormalizeImage, ImagePermute((2, 0, 1)) -- Pillow's antialiased bilinear resize evaluated inside the crop window, ONE launch per
   batch (csrc/resample.cu).
@@ -114,6 +115,22 @@ class KeypointsBottomRightPadding(DetectionBottomRightPadding):
     pass
 
 
+class DetectionAutoPadding(Processing):
+    """processing.py:443-470: pads bottom / right with `pad_value` up to the next multiple of `shape_multiple` (H, W); the image
+    stays at the top-left corner.  In a chain it comes first (get_equivalent_compose_without_resizing).  Like the reference's
+    AutoPadding (processing.py:128-130) it does not count as resizing."""
+
+    resizes_image = False
+
+    def __init__(self, shape_multiple: Tuple[int, int], pad_value: int):
+        self.shape_multiple = tuple(shape_multiple)
+        self.pad_value = pad_value
+
+    def padded_shape(self, height: int, width: int) -> Tuple[int, int]:
+        mh, mw = self.shape_multiple
+        return ((height + mh - 1) // mh) * mh, ((width + mw - 1) // mw) * mw
+
+
 class Resize(Processing):
     """processing.py:614-644: scales the shorter side to `size` with PIL's bilinear filter (no-op when the scale is exactly 1)."""
 
@@ -148,17 +165,19 @@ class CenterCrop(Processing):
 class ComposeProcessing(Processing):
     def __init__(self, processings: Sequence[Processing]):
         self.processings = list(processings)
-        order = [ReverseImageChannels, _Rescale, _Padding, Resize, CenterCrop, StandardizeImage, NormalizeImage, ImagePermute]
+        order = [DetectionAutoPadding, ReverseImageChannels, _Rescale, _Padding, Resize, CenterCrop, StandardizeImage, NormalizeImage, ImagePermute]
         pos = -1
-        self.reverse = self.rescale = self.padding = self.resize = self.crop = self.standardize = self.normalize = None
+        self.auto_padding = self.reverse = self.rescale = self.padding = self.resize = self.crop = self.standardize = self.normalize = None
         for p in self.processings:
             idx = next((i for i, t in enumerate(order) if isinstance(p, t)), None)
             if idx is None or idx <= pos:
-                raise NotImplementedError(f"unsupported processing chain at {type(p).__name__}: supported order is [ReverseImageChannels] "
+                raise NotImplementedError(f"unsupported processing chain at {type(p).__name__}: supported order is [DetectionAutoPadding] [ReverseImageChannels] "
                                           "([Rescale] [Padding] | [Resize] [CenterCrop]) [StandardizeImage] [NormalizeImage] [ImagePermute]")  # fmt: skip
             pos = idx
-            name = ("reverse", "rescale", "padding", "resize", "crop", "standardize", "normalize", "permute")[idx]
+            name = ("auto_padding", "reverse", "rescale", "padding", "resize", "crop", "standardize", "normalize", "permute")[idx]
             setattr(self, name, p)
+        if self.auto_padding is not None and any(p is not None for p in (self.rescale, self.padding, self.resize, self.crop)):
+            raise NotImplementedError("DetectionAutoPadding cannot be combined with a resizing or padding step")
         if (self.resize is not None or self.crop is not None) and (self.rescale is not None or self.padding is not None):
             raise NotImplementedError("Resize / CenterCrop (classification) cannot be combined with a detection Rescale / Padding step")
         if self.padding is None and self.rescale is not None and self.rescale.keep_aspect:
@@ -168,7 +187,18 @@ class ComposeProcessing(Processing):
 
     @property
     def resizes_image(self) -> bool:
-        return self.rescale is not None or self.padding is not None or self.resize is not None or self.crop is not None
+        return any(p is not None for p in (self.rescale, self.padding, self.resize, self.crop))
+
+    def get_equivalent_compose_without_resizing(self, auto_padding: DetectionAutoPadding) -> "ComposeProcessing":
+        """processing.py:185-201: `auto_padding` first, then every step of this chain that does not resize the image."""
+        return ComposeProcessing([auto_padding] + [p for p in self.processings if not p.resizes_image])
+
+    def for_predict(self, skip_image_resizing: bool) -> "ComposeProcessing":
+        """The chain a detector's predict() runs: this one, or with skip_image_resizing its equivalent without resizing behind
+        DetectionAutoPadding((32, 32), 0) (the reference's _get_pipeline)."""
+        if not skip_image_resizing:
+            return self
+        return self.get_equivalent_compose_without_resizing(auto_padding=DetectionAutoPadding(shape_multiple=(32, 32), pad_value=0))
 
     @property
     def classification(self) -> bool:
@@ -228,6 +258,8 @@ class ComposeProcessing(Processing):
         if self.padding is not None:
             top, left = self.padding.top_left(nh, nw)
             canvas = self.padding.output_shape
+        elif self.auto_padding is not None:
+            top, left, canvas = 0, 0, self.auto_padding.padded_shape(nh, nw)
         else:
             top, left, canvas = 0, 0, (nh, nw)
         return ImageGeometry((height, width), sh, sw, (nh, nw), top, left), canvas
@@ -240,11 +272,12 @@ class ComposeProcessing(Processing):
             raise ValueError(f"the images of a batch must map to one input shape, got {sorted(set(canvases))}")
         oh, ow = canvases[0]
         batch = K.empty_nhwc(len(images), 16, oh, ow, device)
+        pad = self.padding or self.auto_padding
         for b, (im, g) in enumerate(zip(images, geos)):
             if im.dtype != np.uint8 or im.ndim != 3:
                 raise ValueError("predict() images must be uint8 H x W x C arrays")
             src = torch.from_numpy(np.ascontiguousarray(im)).to(device, non_blocking=True)
-            K.preprocess_u8(src, batch[b : b + 1], g.resized_shape, (g.pad_top, g.pad_left), pad_value=self.padding.pad_value if self.padding is not None else 0.0,
+            K.preprocess_u8(src, batch[b : b + 1], g.resized_shape, (g.pad_top, g.pad_left), pad_value=pad.pad_value if pad is not None else 0.0,
                             max_value=self.standardize.max_value if self.standardize is not None else 0.0, reverse_channels=self.reverse is not None,
                             mean=self.normalize.mean if self.normalize is not None else None, std=self.normalize.std if self.normalize is not None else None)  # fmt: skip
         return batch, list(geos)

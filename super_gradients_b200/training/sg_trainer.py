@@ -654,6 +654,8 @@ class Trainer:
                 swapped = True
             if loss is not None:
                 self.criterion = LossesFactory().get(loss) if isinstance(loss, (str, Mapping)) else loss
+            elif keep_criterion is None:
+                self.criterion = None  # a model that was never trained here: metrics only
             handler = CallbackHandler(list(test_phase_callbacks or []))
             context = PhaseContext(net=self.net, criterion=self.criterion, device=self.device, experiment_name=self.experiment_name)
             handler.fire("on_test_loader_start", context)
