@@ -500,6 +500,63 @@ int sgb_resample_crop_u8(const int64_t* table_host, const int64_t* table, const 
                          int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t reverse_channels,
                          double max_value, const float* mean_host, const float* std_host, sgb_bf16* out, void* stream);
 
+/* ---- detection train augmentation (training/transforms/transforms.py:603-690 DetectionRandomAffine, :693-809 DetectionMixup,
+ *      :945-977 DetectionPaddedRescale, :980-1009 DetectionHorizontalFlip, :1150-1229 DetectionRGB2BGR / DetectionHSV,
+ *      :490-511 DetectionStandardize; random_affine :1464-1534, augment_hsv :1623-1634, utils.py:203-226) ---- */
+/* Per-image table: int64 [batch][SGB_AUG_FIELDS]; the six affine coefficients are float64 values stored bit for bit in their slots.
+ *   source image: byte offset in src, h, w (dense rows of w * 3 bytes)
+ *   affine: flag, output size (the image size after the affine; == h, w when the flag is 0), forward 2 x 3 matrix M (row major),
+ *           border value
+ *   channel swap flag (DetectionRGB2BGR), HSV flag and int gains dh / ds / dv, bgr_channels packed as c0 | c1 << 2 | c2 << 4,
+ *   horizontal flip flag
+ *   mixup: flag, partner byte offset / h / w, partner flip flag, first resize size, canvas size (target_dim), border value,
+ *          second resize size (jit_factor), crop offsets x / y
+ *   padded rescale: resized size (int(h * r), int(w * r)) of the affine-size image inside the out_h x out_w canvas */
+#define SGB_AUG_OFFSET 0
+#define SGB_AUG_H 1
+#define SGB_AUG_W 2
+#define SGB_AUG_AFFINE 3
+#define SGB_AUG_AFF_H 4
+#define SGB_AUG_AFF_W 5
+#define SGB_AUG_M 6 /* 6 slots */
+#define SGB_AUG_AFF_BORDER 12
+#define SGB_AUG_SWAP 13
+#define SGB_AUG_HSV 14
+#define SGB_AUG_DH 15
+#define SGB_AUG_DS 16
+#define SGB_AUG_DV 17
+#define SGB_AUG_BGR 18
+#define SGB_AUG_FLIP 19
+#define SGB_AUG_MIX 20
+#define SGB_AUG_MIX_OFFSET 21
+#define SGB_AUG_MIX_H 22
+#define SGB_AUG_MIX_W 23
+#define SGB_AUG_MIX_FLIP 24
+#define SGB_AUG_MIX_R1_H 25
+#define SGB_AUG_MIX_R1_W 26
+#define SGB_AUG_MIX_CANVAS_H 27
+#define SGB_AUG_MIX_CANVAS_W 28
+#define SGB_AUG_MIX_BORDER 29
+#define SGB_AUG_MIX_R2_H 30
+#define SGB_AUG_MIX_R2_W 31
+#define SGB_AUG_MIX_X 32
+#define SGB_AUG_MIX_Y 33
+#define SGB_AUG_RS_H 34
+#define SGB_AUG_RS_W 35
+#define SGB_AUG_FIELDS 36
+/* table_host: the table in host memory (validated here); table: the same table in device memory.  src: device uint8 buffer of
+ * src_bytes holding every source and mixup-partner image (channels == 3).  out: device bf16 [batch, out_h, out_w, out_pitch]
+ * (out_pitch >= 3, a multiple of 8; channels >= 3 written as 0).  ONE launch for the batch.  Per output pixel: cv2.warpAffine
+ * (INTER_LINEAR, BORDER_CONSTANT, fixed point) -> channel swap -> augment_hsv (cv2 BGR2HSV / HSV2BGR; hsv_simd_block: the pixel
+ * count of one vector block of cv2's HSV2BGR, whose columns below w - w % block truncate and whose tail rounds) -> horizontal flip
+ * -> mixup with the partner's canvas, each cv2.resize on the way recomputed -> bottom-right placement, resized (INTER_LINEAR)
+ * when the rescale size differs from the affine size, onto pad_value -> v / max_value -> round-to-nearest bf16.  Bit-exact with
+ * the reference's cv2 / numpy chain.  A table naming bytes outside src, a degenerate or non-finite matrix, a matrix mapping
+ * the output outside +-2^20 source pixels, or a bad size or flag is refused with SGB_E_INVALID.  batch == 0 is a no-op. */
+int sgb_detection_augment(const int64_t* table_host, const int64_t* table, const uint8_t* src, int64_t src_bytes, int32_t batch,
+                          int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t pad_value, double max_value,
+                          int32_t hsv_simd_block, sgb_bf16* out, void* stream);
+
 /* ---- row-wise classification decode (training/metrics/classification_metrics.py:40-78 Accuracy / Top5, utils.py accuracy(),
  *      pipelines.py:516-531 torch.max(softmax(logits), 1)) ---- */
 /* logits [N, C] (row stride row_stride >= C elements; bf16 when logits_bf16, else f32).  One warp per row, one pass over the row.

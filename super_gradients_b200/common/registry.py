@@ -29,5 +29,7 @@ CALLBACKS: Dict[str, Callable] = {}
 register_callback = create_register_decorator(CALLBACKS)
 METRICS: Dict[str, Callable] = {}
 register_metric = create_register_decorator(METRICS)
+TRANSFORMS: Dict[str, Callable] = {}
+register_transform = create_register_decorator(TRANSFORMS)
 COLLATE_FUNCTIONS: Dict[str, Callable] = {}
 register_collate_function = create_register_decorator(COLLATE_FUNCTIONS)

@@ -55,18 +55,37 @@ SGB_HD Coef resize_coef(int d, int dst, int src, bool clamp) {
   return c;
 }
 
+// the four source pixels (rows y0 / y1, columns x0 / x1) and weights of pixel (y, x) of the dst_h x dst_w resize of an H x W image
+struct Taps {
+  int x0, x1, y0, y1;
+  Coef cx, cy;
+};
+
+SGB_HD Taps resize_taps(int H, int W, int dst_h, int dst_w, int y, int x) {
+  Taps t;
+  t.cx = resize_coef(x, dst_w, W, true);
+  t.cy = resize_coef(y, dst_h, H, false);
+  t.x0 = t.cx.s;
+  t.x1 = t.cx.s + 1 < W ? t.cx.s + 1 : W - 1;  // c1 == 0 whenever s + 1 would leave the row
+  t.y0 = t.cy.s < 0 ? 0 : (t.cy.s > H - 1 ? H - 1 : t.cy.s);
+  t.y1 = t.cy.s + 1 < 0 ? 0 : (t.cy.s + 1 > H - 1 ? H - 1 : t.cy.s + 1);
+  return t;
+}
+
+// the resized value from the source values at (y0, x0), (y0, x1), (y1, x0), (y1, x1)
+SGB_HD int resize_combine(const Taps& t, int p00, int p01, int p10, int p11) {
+  const int d0 = p00 * t.cx.c0 + p01 * t.cx.c1;
+  const int d1 = p10 * t.cx.c0 + p11 * t.cx.c1;
+  return (((t.cy.c0 * (d0 >> 4)) >> 16) + ((t.cy.c1 * (d1 >> 4)) >> 16) + 2) >> 2;
+}
+
 // channel c of pixel (y, x) of the dst_h x dst_w INTER_LINEAR resize of an H x W x C uint8 image (row pitch in bytes)
 SGB_HD int resized_u8(const uint8_t* img, int H, int W, int C, int pitch, int dst_h, int dst_w, int y, int x, int c) {
   if (dst_h == H && dst_w == W) return img[(int64_t)y * pitch + x * C + c];
-  const Coef cx = resize_coef(x, dst_w, W, true), cy = resize_coef(y, dst_h, H, false);
-  const int x0 = cx.s, x1 = cx.s + 1 < W ? cx.s + 1 : W - 1;  // c1 == 0 whenever s + 1 would leave the row
-  int y0 = cy.s < 0 ? 0 : (cy.s > H - 1 ? H - 1 : cy.s);
-  int y1 = cy.s + 1 < 0 ? 0 : (cy.s + 1 > H - 1 ? H - 1 : cy.s + 1);
-  const uint8_t* r0 = img + (int64_t)y0 * pitch;
-  const uint8_t* r1 = img + (int64_t)y1 * pitch;
-  const int d0 = (int)r0[x0 * C + c] * cx.c0 + (int)r0[x1 * C + c] * cx.c1;
-  const int d1 = (int)r1[x0 * C + c] * cx.c0 + (int)r1[x1 * C + c] * cx.c1;
-  return (((cy.c0 * (d0 >> 4)) >> 16) + ((cy.c1 * (d1 >> 4)) >> 16) + 2) >> 2;
+  const Taps t = resize_taps(H, W, dst_h, dst_w, y, x);
+  const uint8_t* r0 = img + (int64_t)t.y0 * pitch;
+  const uint8_t* r1 = img + (int64_t)t.y1 * pitch;
+  return resize_combine(t, r0[t.x0 * C + c], r0[t.x1 * C + c], r1[t.x0 * C + c], r1[t.x1 * C + c]);
 }
 
 // StandardizeImage (max_value > 0) then NormalizeImage (normalize != 0) of one value of output channel c, in fp32

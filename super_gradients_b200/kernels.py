@@ -430,6 +430,31 @@ def resample_crop_u8(table_host, table, src, out, max_value=255.0, reverse_chann
     return out
 
 
+AUG_FIELDS = 36  # SGB_AUG_FIELDS: per-image draws of the detection train augmentation (include/sgb200.h)
+HSV_SIMD_BLOCK = 32  # pixels per vector block of cv2's 8-bit HSV2BGR in its x86 builds (the row tail is rounded, the blocks truncated)
+
+
+def detection_augment(table_host, table, src, out, pad_value=114, max_value=255.0):
+    """Detection train augmentation of a whole batch in one launch.  table_host: int64 [B, AUG_FIELDS] CPU tensor (sgb200.h
+    SGB_AUG_*), table: the same on the device; src: device uint8 buffer holding the HWC source and mixup-partner images;
+    out: bf16 NHWC [B, c_pad, out_h, out_w] (channels >= 3 are zeroed)."""
+    require_cuda(src, "src")
+    require_cuda(table, "table")
+    require_cuda(out, "out")
+    if out.data_ptr() % 16:
+        raise L.SgbError("out must be 16-byte aligned (the kernel stores 8 channels at a time)")
+    if table_host.dtype != torch.int64 or table_host.dim() != 2 or table_host.shape[1] != AUG_FIELDS or not table_host.is_contiguous() or table_host.is_cuda:
+        raise L.SgbError(f"table_host must be a contiguous int64 [B, {AUG_FIELDS}] host tensor")
+    if table.dtype != torch.int64 or tuple(table.shape) != tuple(table_host.shape) or not table.is_contiguous() or src.dtype != torch.uint8:
+        raise L.SgbError("table must be the device copy of table_host and src a uint8 buffer")
+    B, pitch = table_host.shape[0], nhwc_pitch(out)
+    if out.dtype != torch.bfloat16 or out.shape[0] != B or out.shape[1] != pitch:
+        raise L.SgbError("out must be a dense bf16 NHWC batch [B, c_pad, out_h, out_w]")
+    _timed("sgb_detection_augment", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel(), B, 3, out.shape[2], out.shape[3], pitch,
+           int(pad_value), float(max_value), HSV_SIMD_BLOCK, _ptr(out), _stream())  # fmt: skip
+    return out
+
+
 def classify_rows(logits, target=None, k=1, counters=None, label=None, confidence=None):
     """Row-wise classification decode of fp32 / bf16 logits [N, C] (unit column stride).  target: int64 [N] class indices or a
     float [N, C] soft-label tensor (argmax per row); counters: int64 [4] device accumulators (top-1 correct, top-k correct, rows,

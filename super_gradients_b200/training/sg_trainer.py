@@ -23,6 +23,7 @@ from torch import nn
 from .. import functional as SF
 from .. import kernels as K
 from ..common.factories import LossesFactory, MetricsFactory, _fuzzy
+from .datasets.detection_augment_dataset import PackedDetectionBatch
 from .flat_state import FlatState
 from .utils.callbacks import CallbackHandler, PhaseContext
 
@@ -519,7 +520,10 @@ class Trainer:
             for batch_idx, batch in enumerate(train_loader):
                 if batch_idx >= steps_per_epoch:
                     break
-                inputs, targets = batch[0], batch[1]
+                if isinstance(batch, PackedDetectionBatch):  # GPU detection augmentation: one copy + one launch make the input
+                    inputs, targets = batch.to_model_input(self.device)
+                else:
+                    inputs, targets = batch[0], batch[1]
                 inputs = inputs.to(self.device, non_blocking=True)
                 if torch.is_tensor(targets) and not (hasattr(criterion, "forward") and type(criterion).__name__ == "PPYoloELoss"):
                     targets = targets.to(self.device, non_blocking=True)
