@@ -557,6 +557,68 @@ int sgb_detection_augment(const int64_t* table_host, const int64_t* table, const
                           int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t pad_value, double max_value,
                           int32_t hsv_simd_block, sgb_bf16* out, void* stream);
 
+/* ---- pose train augmentation (training/transforms/keypoints/*.py of the YOLO-NAS-POSE recipes: KeypointsRandomHorizontalFlip,
+ *      KeypointsBrightnessContrast, KeypointsReverseImageChannels, KeypointsHSV, KeypointsRandomRotate90,
+ *      KeypointsRandomAffineTransform, KeypointsMosaic, KeypointsLongestMaxSize, KeypointsPadIfNeeded, KeypointsImageStandardize) ---- */
+/* Per-sample table: int64 [batch][SGB_POSE_FIELDS].  Three uint8 values (pad colours) are packed as v0 | v1 << 8 | v2 << 16.
+ *   NSUB: 1, or 4 for a mosaic; CANVAS_H / W: the mosaic canvas (or the single tile's size); MOSAIC_PAD: the mosaic pad colour
+ *   RS_H / W: the LongestMaxSize size of the canvas (== the canvas size when it is not resized)
+ *   PAD_TOP / PAD_LEFT: the resized canvas' position in the out_size x out_size output; PAD_VALUE: the pad colour
+ *   then NSUB sub-sample records of SGB_POSE_SUB_FIELDS from SGB_POSE_SUB (top-left, top-right, bottom-left, bottom-right):
+ *     source byte offset in src, h, w (dense rows of w * 3 bytes); flip flag; brightness-contrast flag, the three float32 channel
+ *     means, the float32 contrast and brightness gains (float32 bits); channel reversal flag; HSV flag and gains dh / ds / dv;
+ *     np.rot90 count k in [0, 3]; affine flag, forward 2 x 3 matrix (float64 bits), cv2 interpolation flag in [0, 4], border
+ *     colour; the byte offset of the tile's rotated image in the workspace; the tile's position y / x in the canvas; its size
+ *     rh / rw after rot90 (the affine keeps the size) */
+#define SGB_POSE_NSUB 0
+#define SGB_POSE_CANVAS_H 1
+#define SGB_POSE_CANVAS_W 2
+#define SGB_POSE_MOSAIC_PAD 3
+#define SGB_POSE_RS_H 4
+#define SGB_POSE_RS_W 5
+#define SGB_POSE_PAD_TOP 6
+#define SGB_POSE_PAD_LEFT 7
+#define SGB_POSE_PAD_VALUE 8
+#define SGB_POSE_SUB 16
+#define SGB_POSE_SUB_FIELDS 32
+#define SGB_POSE_FIELDS 144
+#define SGB_POSE_S_OFFSET 0
+#define SGB_POSE_S_H 1
+#define SGB_POSE_S_W 2
+#define SGB_POSE_S_FLIP 3
+#define SGB_POSE_S_BC 4
+#define SGB_POSE_S_MEAN 5 /* 3 slots */
+#define SGB_POSE_S_CONTRAST 8
+#define SGB_POSE_S_BRIGHTNESS 9
+#define SGB_POSE_S_REVERSE 10
+#define SGB_POSE_S_HSV 11
+#define SGB_POSE_S_DH 12
+#define SGB_POSE_S_DS 13
+#define SGB_POSE_S_DV 14
+#define SGB_POSE_S_ROT 15
+#define SGB_POSE_S_AFFINE 16
+#define SGB_POSE_S_M 17 /* 6 slots */
+#define SGB_POSE_S_MODE 23
+#define SGB_POSE_S_BORDER 24
+#define SGB_POSE_S_WS_OFFSET 25
+#define SGB_POSE_S_Y 26
+#define SGB_POSE_S_X 27
+#define SGB_POSE_S_RH 28
+#define SGB_POSE_S_RW 29
+/* table_host: the table in host memory (validated here); table: the same table in device memory.  src: device uint8 buffer of
+ * src_bytes holding every sub-sample's source image (H x W x 3).  workspace: caller-owned device uint8 buffer of workspace_bytes
+ * receiving every tile's rotated image at its WS_OFFSET.  out: device bf16 [batch, out_size, out_size, out_pitch] (out_pitch >= 3,
+ * a multiple of 8; channels >= 3 written as 0).  TWO launches for the batch, whatever its size: (1) per tile pixel, flip ->
+ * brightness-contrast -> channel reversal -> augment_hsv (hsv_simd_block as in sgb_detection_augment) -> np.rot90 into the
+ * workspace; (2) per output pixel, pad -> cv2.resize INTER_LINEAR of the canvas -> mosaic placement -> cv2.warpAffine
+ * (BORDER_CONSTANT, fixed point, INTER_NEAREST / LINEAR / CUBIC / AREA / LANCZOS4) -> v / max_value -> round-to-nearest bf16.
+ * Bit-exact with the reference's cv2 / numpy chain.  Bytes outside src or the workspace, a degenerate or non-finite matrix, a
+ * matrix mapping the tile outside +-2^20 pixels, a tile outside the canvas, or a bad size, count, mode or flag is refused with
+ * SGB_E_INVALID.  batch == 0 is a no-op. */
+int sgb_pose_augment(const int64_t* table_host, const int64_t* table, const uint8_t* src, int64_t src_bytes, uint8_t* workspace,
+                     int64_t workspace_bytes, int32_t batch, int32_t out_size, int32_t out_pitch, double max_value, int32_t hsv_simd_block,
+                     sgb_bf16* out, void* stream);
+
 /* ---- row-wise classification decode (training/metrics/classification_metrics.py:40-78 Accuracy / Top5, utils.py accuracy(),
  *      pipelines.py:516-531 torch.max(softmax(logits), 1)) ---- */
 /* logits [N, C] (row stride row_stride >= C elements; bf16 when logits_bf16, else f32).  One warp per row, one pass over the row.

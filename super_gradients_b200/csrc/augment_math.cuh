@@ -58,23 +58,68 @@ SGB_HD void warp_coord(const Inverse& a, int y, int x, int& X, int& Y) {
   Y = (Y0 + (int)rint(dmul(dmul(a.a21, (double)x), 1024.0))) >> 5;
 }
 
-// cv2.warpAffine pixel (y, x) of an H x W x 3 image (dense rows) into p[3]
-SGB_HD void warp_pixel(const uint8_t* img, int H, int W, const Inverse& a, int border, int y, int x, int p[3]) {
+// cv2's INTER_REMAP_COEF_BITS = 15 coefficient tables of INTER_CUBIC (4 x 4 taps) and INTER_LANCZOS4 (8 x 8 taps) per sub-pixel
+// phase (fy * 32 + fx), row-major taps: the fixed-point `itab` of initInterTab2D (imgwarp.cpp).  Filled once on the host.
+struct RemapTabs {
+  const int16_t* cubic;    // [1024][16]
+  const int16_t* lanczos;  // [1024][64]
+};
+
+// cv2.warpAffine pixel (y, x) of an H x W x 3 image (dense rows) into p[3], BORDER_CONSTANT with border[3].  mode: cv2's
+// interpolation flag, 0 INTER_NEAREST, 1 INTER_LINEAR, 2 INTER_CUBIC, 3 INTER_AREA (warpAffine runs it as INTER_LINEAR),
+// 4 INTER_LANCZOS4.  Nearest rounds the coordinate (+ 2^9, >> 10) and reads one pixel or the border; the others take the 1/32
+// sub-pixel phase and sum ksize x ksize taps from (X >> 5) - (ksize / 2 - 1), reading the border outside the image, as
+// (sum + 2^14) >> 15 saturated to uint8.  tabs is only read by modes 2 and 4.
+SGB_HD void warp_pixel_mode(const uint8_t* img, int H, int W, const Inverse& a, int mode, const int border[3], const RemapTabs& tabs, int y, int x,
+                            int p[3]) {
+  if (mode == 0) {
+    const int X0 = (int)rint(dmul(dadd(dmul(a.a12, (double)y), a.b1), 1024.0)) + 512;
+    const int Y0 = (int)rint(dmul(dadd(dmul(a.a22, (double)y), a.b2), 1024.0)) + 512;
+    const int sx = (X0 + (int)rint(dmul(dmul(a.a11, (double)x), 1024.0))) >> 10;
+    const int sy = (Y0 + (int)rint(dmul(dmul(a.a21, (double)x), 1024.0))) >> 10;
+    const bool in = sy >= 0 && sy < H && sx >= 0 && sx < W;
+    for (int c = 0; c < 3; ++c) p[c] = in ? (int)img[((int64_t)sy * W + sx) * 3 + c] : border[c];
+    return;
+  }
   int X, Y;
   warp_coord(a, y, x, X, Y);
-  const int sx = X >> 5, sy = Y >> 5, fx = X & 31, fy = Y & 31;
-  const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+  const int fx = X & 31, fy = Y & 31;
   int acc[3] = {0, 0, 0};
-  for (int k = 0; k < 4; ++k) {
-    const int ty = sy + (k >> 1), tx = sx + (k & 1);
-    const bool in = ty >= 0 && ty < H && tx >= 0 && tx < W;
-    const uint8_t* s = img + ((int64_t)(in ? ty : 0) * W + (in ? tx : 0)) * 3;
-    for (int c = 0; c < 3; ++c) acc[c] += (in ? (int)s[c] : border) * w[k];
+  if (mode == 2 || mode == 4) {
+    const int k = mode == 2 ? 4 : 8;
+    const int sx = (X >> 5) - (k / 2 - 1), sy = (Y >> 5) - (k / 2 - 1);
+    const int16_t* w = (mode == 2 ? tabs.cubic + (fy * 32 + fx) * 16 : tabs.lanczos + (fy * 32 + fx) * 64);
+    for (int i = 0; i < k; ++i) {
+      const int ty = sy + i;
+      const bool row_in = ty >= 0 && ty < H;
+      const uint8_t* row = img + (int64_t)(row_in ? ty : 0) * W * 3;
+      for (int j = 0; j < k; ++j) {
+        const int tx = sx + j, wk = w[i * k + j];
+        const bool in = row_in && tx >= 0 && tx < W;
+        const uint8_t* s = row + (in ? tx : 0) * 3;
+        for (int c = 0; c < 3; ++c) acc[c] += (in ? (int)s[c] : border[c]) * wk;
+      }
+    }
+  } else {
+    const int sx = X >> 5, sy = Y >> 5;
+    const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+    for (int k = 0; k < 4; ++k) {
+      const int ty = sy + (k >> 1), tx = sx + (k & 1);
+      const bool in = ty >= 0 && ty < H && tx >= 0 && tx < W;
+      const uint8_t* s = img + ((int64_t)(in ? ty : 0) * W + (in ? tx : 0)) * 3;
+      for (int c = 0; c < 3; ++c) acc[c] += (in ? (int)s[c] : border[c]) * w[k];
+    }
   }
   for (int c = 0; c < 3; ++c) {
     const int v = (acc[c] + (1 << 14)) >> 15;
     p[c] = v < 0 ? 0 : (v > 255 ? 255 : v);
   }
+}
+
+// cv2.warpAffine INTER_LINEAR pixel (y, x) of an H x W x 3 image (dense rows) into p[3], one border value for every channel
+SGB_HD void warp_pixel(const uint8_t* img, int H, int W, const Inverse& a, int border, int y, int x, int p[3]) {
+  const int b[3] = {border, border, border};
+  warp_pixel_mode(img, H, W, a, 1, b, RemapTabs{nullptr, nullptr}, y, x, p);
 }
 
 SGB_HD int sdiv(int i) { return i == 0 ? 0 : (int)rint((double)(255 << 12) / (double)i); }

@@ -455,6 +455,31 @@ def detection_augment(table_host, table, src, out, pad_value=114, max_value=255.
     return out
 
 
+POSE_FIELDS = 144  # SGB_POSE_FIELDS: per-sample draws of the pose train augmentation (include/sgb200.h)
+
+
+def pose_augment(table_host, table, src, workspace, out, max_value=255.0):
+    """Pose train augmentation of a whole batch in two launches.  table_host: int64 [B, POSE_FIELDS] CPU tensor (sgb200.h
+    SGB_POSE_*), table: the same on the device; src: device uint8 buffer of every tile's HWC source image; workspace: device uint8
+    buffer receiving the rotated tiles; out: bf16 NHWC [B, c_pad, S, S] (channels >= 3 are zeroed)."""
+    for t, n in ((src, "src"), (table, "table"), (workspace, "workspace"), (out, "out")):
+        require_cuda(t, n)
+    if out.data_ptr() % 16:
+        raise L.SgbError("out must be 16-byte aligned (the kernel stores 8 channels at a time)")
+    if table_host.dtype != torch.int64 or table_host.dim() != 2 or table_host.shape[1] != POSE_FIELDS or not table_host.is_contiguous() or table_host.is_cuda:
+        raise L.SgbError(f"table_host must be a contiguous int64 [B, {POSE_FIELDS}] host tensor")
+    if table.dtype != torch.int64 or tuple(table.shape) != tuple(table_host.shape) or not table.is_contiguous():
+        raise L.SgbError("table must be the device copy of table_host")
+    if src.dtype != torch.uint8 or workspace.dtype != torch.uint8 or not src.is_contiguous() or not workspace.is_contiguous():
+        raise L.SgbError("src and workspace must be contiguous uint8 buffers")
+    B, pitch = table_host.shape[0], nhwc_pitch(out)
+    if out.dtype != torch.bfloat16 or out.shape[0] != B or out.shape[1] != pitch or out.shape[2] != out.shape[3]:
+        raise L.SgbError("out must be a dense square bf16 NHWC batch [B, c_pad, S, S]")
+    _timed("sgb_pose_augment", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel(), _ptr(workspace), workspace.numel(), B, out.shape[2],
+           pitch, float(max_value), HSV_SIMD_BLOCK, _ptr(out), _stream())  # fmt: skip
+    return out
+
+
 def classify_rows(logits, target=None, k=1, counters=None, label=None, confidence=None):
     """Row-wise classification decode of fp32 / bf16 logits [N, C] (unit column stride).  target: int64 [N] class indices or a
     float [N, C] soft-label tensor (argmax per row); counters: int64 [4] device accumulators (top-1 correct, top-k correct, rows,

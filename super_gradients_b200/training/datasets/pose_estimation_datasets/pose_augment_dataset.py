@@ -1,0 +1,88 @@
+"""Train-time loading for the GPU pose augmentation.
+
+`PoseAugmentDataset` wraps any map-style dataset with `__len__` and `load_sample(index)` returning a PoseEstimationSample-like
+object (image uint8 H x W x 3, joints [N, J, 3], areas, bboxes_xywh, is_crowd): the contract of the reference's
+AbstractPoseEstimationDataset.  In DataLoader workers it runs the host half of the keypoint transforms the way the reference's
+KeypointsCompose.apply_to_sample does: sanitize, then the transforms, loading a mosaic's three extra samples with
+random.randrange and passing each through the transforms applied so far.  `PoseAugmentCollateFN` packs a batch into one uint8
+buffer (table + images) plus YoloNASPoseCollateFN's targets, touching no CUDA state; `PackedPoseBatch.to_model_input(device)`
+then makes the model input with one copy and one kernel call."""
+import random
+from typing import List, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from ....common.registry import register_collate_function
+from ...transforms.keypoints import KeypointsImageStandardize, PoseHostSample, check_pose_pipeline
+from ...transforms.keypoints_augment import PosePlan, pack_into, packed_size, run_packed
+from .yolo_nas_pose_collate_fn import flat_collate_tensors_with_batch_index
+
+
+class PoseAugmentDataset(torch.utils.data.Dataset):
+    def __init__(self, dataset, transforms: Sequence):
+        self.output_size = check_pose_pipeline(transforms)
+        self.dataset, self.transforms = dataset, list(transforms)
+        self.max_value = float([t for t in self.transforms if isinstance(t, KeypointsImageStandardize)][0].max_value)
+
+    def __len__(self) -> int:
+        return len(self.dataset)
+
+    def _load(self, index: int) -> PoseHostSample:
+        return PoseHostSample.from_sample(self.dataset.load_sample(index))
+
+    def _apply(self, sample: PoseHostSample, transforms) -> PoseHostSample:
+        applied = []
+        for t in transforms:
+            if not t.may_require_additional_samples:
+                sample = t.apply_to_sample(sample)
+                applied.append(t)
+            else:
+                extra = [self._load(random.randrange(0, len(self.dataset))) for _ in range(t.get_number_of_additional_samples())]
+                sample.additional_samples = [self._apply(s, applied) for s in extra]
+                sample = t.apply_to_sample(sample)
+        return sample
+
+    def __getitem__(self, index: int) -> Tuple[PosePlan, Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+        """(plan of the pixel work, (boxes [n, 4] xyxy, joints [n, J, 3], is_crowd [n, 1])) of sample `index` after the transforms:
+        the targets YoloNASPoseCollateFN takes from the reference's sample."""
+        s = self._apply(self._load(index).sanitize_sample(), self.transforms)
+        xywh = np.asarray(s.bboxes_xywh)
+        xyxy = np.concatenate([xywh[..., :2], xywh[..., :2] + xywh[..., 2:4]], axis=-1)
+        is_crowd = np.zeros(len(xyxy)) if s.is_crowd is None else s.is_crowd
+        return s.plan, (xyxy, s.joints, is_crowd.astype(int).reshape((-1, 1)))
+
+
+class PackedPoseBatch:
+    """A collated batch: `buffer` (uint8: the int64 per-sample table, then the images) and YoloNASPoseCollateFN's targets
+    (boxes [N, 5], joints [N, J, 4], is_crowd [N, 2], each with the sample index first)."""
+
+    def __init__(self, buffer: torch.Tensor, batch: int, targets, output_size: int, max_value: float):
+        self.buffer, self.batch, self.targets, self.output_size, self.max_value = buffer, batch, targets, output_size, max_value
+
+    def pin_memory(self) -> "PackedPoseBatch":
+        """Called by DataLoader(pin_memory=True) in the main process, so the copy to the device is asynchronous."""
+        return PackedPoseBatch(self.buffer.pin_memory(), self.batch, self.targets, self.output_size, self.max_value)
+
+    def to_model_input(self, device):
+        """(images bf16 NHWC [B, 16, S, S], (boxes, joints, is_crowd)): one copy and one augmentation call, no host synchronisation."""
+        return run_packed(self.buffer, self.batch, device, self.output_size, self.max_value), self.targets
+
+
+@register_collate_function()
+class PoseAugmentCollateFN:
+    """Collates PoseAugmentDataset items into a PackedPoseBatch."""
+
+    def __init__(self, output_size: int = 640, max_value: float = 255.0):
+        self.output_size, self.max_value = int(output_size), float(max_value)
+
+    @classmethod
+    def for_dataset(cls, dataset: PoseAugmentDataset) -> "PoseAugmentCollateFN":
+        return cls(dataset.output_size, dataset.max_value)
+
+    def __call__(self, data: List[Tuple[PosePlan, tuple]]) -> PackedPoseBatch:
+        plans = [d[0] for d in data]
+        buf = torch.empty(packed_size(plans), dtype=torch.uint8)
+        pack_into(plans, buf.numpy())
+        targets = tuple(flat_collate_tensors_with_batch_index([torch.from_numpy(d[1][k]) for d in data]) for k in range(3))
+        return PackedPoseBatch(buf, len(plans), targets, self.output_size, self.max_value)

@@ -23,7 +23,6 @@ from torch import nn
 from .. import functional as SF
 from .. import kernels as K
 from ..common.factories import LossesFactory, MetricsFactory, _fuzzy
-from .datasets.detection_augment_dataset import PackedDetectionBatch
 from .flat_state import FlatState
 from .utils.callbacks import CallbackHandler, PhaseContext
 
@@ -520,7 +519,7 @@ class Trainer:
             for batch_idx, batch in enumerate(train_loader):
                 if batch_idx >= steps_per_epoch:
                     break
-                if isinstance(batch, PackedDetectionBatch):  # GPU detection augmentation: one copy + one launch make the input
+                if hasattr(batch, "to_model_input"):  # PackedDetectionBatch / PackedPoseBatch: the GPU augmentation makes the input
                     inputs, targets = batch.to_model_input(self.device)
                 else:
                     inputs, targets = batch[0], batch[1]

@@ -1,4 +1,17 @@
 from .detection_augment import AugmentPlan, BatchAugmenter, MixupPlan
+from .keypoints import (
+    KeypointsBrightnessContrast,
+    KeypointsHSV,
+    KeypointsImageStandardize,
+    KeypointsLongestMaxSize,
+    KeypointsMosaic,
+    KeypointsPadIfNeeded,
+    KeypointsRandomAffineTransform,
+    KeypointsRandomHorizontalFlip,
+    KeypointsRandomRotate90,
+    KeypointsRemoveSmallObjects,
+    KeypointsReverseImageChannels,
+)
 from .transforms import (
     DetectionHorizontalFlip,
     DetectionHSV,
@@ -11,4 +24,6 @@ from .transforms import (
 )
 
 __all__ = ["AugmentPlan", "BatchAugmenter", "MixupPlan", "DetectionRandomAffine", "DetectionRGB2BGR", "DetectionHSV", "DetectionHorizontalFlip",
-           "DetectionMixup", "DetectionPaddedRescale", "DetectionStandardize", "DetectionTargetsFormatTransform"]  # fmt: skip
+           "DetectionMixup", "DetectionPaddedRescale", "DetectionStandardize", "DetectionTargetsFormatTransform", "KeypointsRandomHorizontalFlip",
+           "KeypointsBrightnessContrast", "KeypointsReverseImageChannels", "KeypointsHSV", "KeypointsRandomRotate90", "KeypointsRandomAffineTransform",
+           "KeypointsMosaic", "KeypointsLongestMaxSize", "KeypointsPadIfNeeded", "KeypointsImageStandardize", "KeypointsRemoveSmallObjects"]  # fmt: skip
