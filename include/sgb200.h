@@ -65,6 +65,11 @@ int sgb_check_device(void);
 /* Number of wgmma/TMA convolution launches issued by this process so far (evidence that the Hopper-native path,
  * not the generic mma.sync kernel, served a call). */
 int64_t sgb_sm100_launches(void);
+/* Number of those launches served by the halo-tile kernel of 3x3 / stride-1 convolutions (conv3x3_halo_kernel). */
+int64_t sgb_conv_halo_launches(void);
+/* Test-only: on != 0 sends every later 3x3 / stride-1 convolution to the im2col wgmma kernel instead of the halo-tile kernel,
+ * so tests and timing tools can compare the two engines on one shape.  Not a user option. */
+void sgb_conv_force_im2col(int on);
 
 /* ---- convolution family (rows C1-C5, C8, C10 of SURVEY.md section 8a) --------------------------------------
  * replaces nn.Conv2d forward in modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,

@@ -47,6 +47,7 @@ struct Params {
   // output row m -> address.  out_mode 0: rows are consecutive NHWC pixels.  out_mode 1: row m = (n, j, i) over a
   // (P x Q) grid is written to pixel (n, j*o_mul + oh_add, i*o_mul + ow_add) of an (outH x outW) image.
   int out_mode, o_mul, oh_add, ow_add, outH, outW;
+  int halo_tw, halo_thw;  // conv3x3_halo_kernel: 8 x 8 output tiles per image row band / per image
   long long y_pitch;  // elements
   int y_off;
   bf16* y;
@@ -68,10 +69,117 @@ __device__ __forceinline__ long long out_row(const Params& p, long long m) {
 }
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory"); }
+// Both consumer warpgroups (WARPS = 8), or consumer warpgroup wg alone (WARPS = 4, named barrier 2 + wg).
+template <int WARPS>
+__device__ __forceinline__ void group_sync(int wg) {
+  if (WARPS == 8)
+    consumer_sync();
+  else
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+}
 
 // Shared-memory layout after the stages: full / empty barriers, then (statistics only) the per-warp column partials of the
 // current tile [8 warps][2][BN] and the CTA's per-channel totals [2][N].
 constexpr uint32_t CTRL_BAR_BYTES = 16u * MAX_STAGES;
+
+// Epilogue of one tile straight from the accumulator registers of a consumer warp (warpgroup wg, 16-row slice wq): the thread
+// holds two rows, at output pixels orow[0] / orow[1] (row_ok false: the row lies past the output), and the column pairs
+// 8 j + 2 (lane % 4) of N tile nt.  (scale, shift, residual, activation) -> bf16 -> global, plus the per-channel sum /
+// sum-of-squares of the stored values, combined in a fixed order across the WARPS warps that share the tile (8: both consumer
+// warpgroups; 4: warpgroup wg alone, with its own s_part / s_stats) into s_stats.
+template <int BN, int WARPS = 8>
+__device__ __forceinline__ void tile_epilogue(const Params& p, const float (&acc)[BN / 2], const long long (&orow)[2],
+                                              const bool (&row_ok)[2], int nt, int wg, int wq, int lane, float* s_part,
+                                              float* s_stats) {
+  const int n0 = nt * BN;
+  const int ncols = min(BN, p.N - n0);
+  bf16* yrow[2];
+  const bf16* rrow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    yrow[h] = p.y + orow[h] * p.y_pitch + p.y_off + n0;
+    rrow[h] = p.residual ? p.residual + orow[h] * p.y_pitch + p.y_off + n0 : nullptr;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = 8 * j + 2 * (lane & 3);
+    const bool col_ok = col < ncols;  // N % 8 == 0: both columns of the pair are valid or neither
+    float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      const bool ok = row_ok[h] && col_ok;
+      if (p.scale && col_ok) {
+        v0 *= p.scale[n0 + col];
+        v1 *= p.scale[n0 + col + 1];
+      }
+      if (p.shift && col_ok) {
+        v0 += p.shift[n0 + col];
+        v1 += p.shift[n0 + col + 1];
+      }
+      if (rrow[h] && ok) {
+        const uint32_t rr = *reinterpret_cast<const uint32_t*>(rrow[h] + col);
+        v0 += __uint_as_float(rr << 16);
+        v1 += __uint_as_float(rr & 0xffff0000u);
+      }
+      if (p.act != SGB_ACT_NONE) {
+        v0 = apply_act(v0, p.act);
+        v1 = apply_act(v1, p.act);
+      }
+      __nv_bfloat162 hh = __floats2bfloat162_rn(v0, v1);
+      const uint32_t pk = *reinterpret_cast<uint32_t*>(&hh);
+      if (ok) {
+        *reinterpret_cast<uint32_t*>(yrow[h] + col) = pk;
+        const float lo = __uint_as_float(pk << 16), hi = __uint_as_float(pk & 0xffff0000u);
+        sum0 += lo;
+        sum1 += hi;
+        sq0 = fmaf(lo, lo, sq0);
+        sq1 = fmaf(hi, hi, sq1);
+      }
+    }
+    if (p.stats) {
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+        sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+        sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
+        sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
+      }
+      if (lane < 4) {
+        float* part = s_part + (WARPS == 8 ? wg * 4 + wq : wq) * 2 * BN;
+        part[col] = sum0;
+        part[col + 1] = sum1;
+        part[BN + col] = sq0;
+        part[BN + col + 1] = sq1;
+      }
+    }
+  }
+  if (p.stats) {
+    // the eight warps' partials of this tile, summed in a fixed order (bit-reproducible statistics)
+    group_sync<WARPS>(wg);
+    for (int i = threadIdx.x - 128 - (WARPS == 8 ? 0 : 128 * wg); i < 2 * BN; i += WARPS * 32) {
+      const int which = i / BN, c = i - which * BN;
+      if (c < ncols) {
+        float v = 0.f;
+#pragma unroll
+        for (int w = 0; w < WARPS; ++w) v += s_part[w * 2 * BN + i];
+        s_stats[which * p.N + n0 + c] += v;
+      }
+    }
+    group_sync<WARPS>(wg);
+  }
+}
+
+// The CTA's per-channel totals -> the fp64 statistics buffer (after a __syncthreads).
+__device__ __forceinline__ void flush_stats(const Params& p, const float* s_stats) {
+  if (p.stats) {
+    double* st = p.stats + (long long)(blockIdx.x & (p.stats_repl - 1)) * 2 * p.N;
+    for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) {
+      const float v = s_stats[i];
+      if (v != 0.f) atomicAdd(&st[i], (double)v);
+    }
+  }
+}
 
 // ------------------------------------------------------------------------------------------------ the kernel
 template <int BN>
@@ -177,100 +285,156 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       __syncwarp();
       if (lane == 0 && prev >= 0) mbar_arrive(empty_bar(prev));
 
-      // ---- epilogue: thread holds rows r_lo, r_lo + 8 and column pairs 8 j + 2 (lane % 4)
-      const int r_lo = wg * 64 + wq * 16 + (lane >> 2);
-      const int n0 = nt * BN;
-      const int ncols = min(BN, p.N - n0);
-      const long long m_lo = (long long)mt * BLOCK_M + r_lo;
-      bf16* yrow[2];
-      const bf16* rrow[2];
+      // ---- epilogue: thread holds rows r_lo, r_lo + 8 of the tile
+      const long long m_lo = (long long)mt * BLOCK_M + wg * 64 + wq * 16 + (lane >> 2);
+      long long orow[2];
       bool row_ok[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long m = m_lo + 8 * h;
         row_ok[h] = m < p.M;
-        const long long orow = out_row(p, row_ok[h] ? m : 0);
-        yrow[h] = p.y + orow * p.y_pitch + p.y_off + n0;
-        rrow[h] = p.residual ? p.residual + orow * p.y_pitch + p.y_off + n0 : nullptr;
+        orow[h] = out_row(p, row_ok[h] ? m : 0);
       }
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = 8 * j + 2 * (lane & 3);
-        const bool col_ok = col < ncols;  // N % 8 == 0: both columns of the pair are valid or neither
-        float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          const bool ok = row_ok[h] && col_ok;
-          if (p.scale && col_ok) {
-            v0 *= p.scale[n0 + col];
-            v1 *= p.scale[n0 + col + 1];
-          }
-          if (p.shift && col_ok) {
-            v0 += p.shift[n0 + col];
-            v1 += p.shift[n0 + col + 1];
-          }
-          if (rrow[h] && ok) {
-            const uint32_t rr = *reinterpret_cast<const uint32_t*>(rrow[h] + col);
-            v0 += __uint_as_float(rr << 16);
-            v1 += __uint_as_float(rr & 0xffff0000u);
-          }
-          if (p.act != SGB_ACT_NONE) {
-            v0 = apply_act(v0, p.act);
-            v1 = apply_act(v1, p.act);
-          }
-          __nv_bfloat162 hh = __floats2bfloat162_rn(v0, v1);
-          const uint32_t pk = *reinterpret_cast<uint32_t*>(&hh);
-          if (ok) {
-            *reinterpret_cast<uint32_t*>(yrow[h] + col) = pk;
-            const float lo = __uint_as_float(pk << 16), hi = __uint_as_float(pk & 0xffff0000u);
-            sum0 += lo;
-            sum1 += hi;
-            sq0 = fmaf(lo, lo, sq0);
-            sq1 = fmaf(hi, hi, sq1);
-          }
-        }
-        if (p.stats) {
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
-            sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
-            sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
-            sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
-          }
-          if (lane < 4) {
-            float* part = s_part + (wg * 4 + wq) * 2 * BN;
-            part[col] = sum0;
-            part[col + 1] = sum1;
-            part[BN + col] = sq0;
-            part[BN + col + 1] = sq1;
-          }
-        }
-      }
-      if (p.stats) {
-        // the eight warps' partials of this tile, summed in a fixed order (bit-reproducible statistics)
-        consumer_sync();
-        for (int i = threadIdx.x - 128; i < 2 * BN; i += CONSUMER_THREADS) {
-          const int which = i / BN, c = i - which * BN;
-          if (c < ncols) {
-            float v = 0.f;
-#pragma unroll
-            for (int w = 0; w < 8; ++w) v += s_part[w * 2 * BN + i];
-            s_stats[which * p.N + n0 + c] += v;
-          }
-        }
-        consumer_sync();
-      }
+      tile_epilogue<BN>(p, acc, orow, row_ok, nt, wg, wq, lane, s_part, s_stats);
     }
   }
   __syncthreads();
-  if (p.stats) {
-    double* st = p.stats + (long long)(blockIdx.x & (p.stats_repl - 1)) * 2 * p.N;
-    for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) {
-      const float v = s_stats[i];
-      if (v != 0.f) atomicAdd(&st[i], (double)v);
+  flush_stats(p, s_stats);
+}
+
+// ------------------------------------------------------------------------------------------------ halo-tile kernel
+// 3x3 / stride 1 / pad 1 convolutions, out_mode 0, no tap table: fprop and the stride-1 dgrad over the flipped CRSK filter.
+// A tile is 8 x 8 output pixels of one image (M = 64, one 8-pixel output row per wgmma 8-row core-matrix group), and the two
+// consumer warpgroups take alternate tiles of the CTA's sequence, each with its own accumulators, so one warpgroup's epilogue
+// overlaps the other's MMAs.  The producer loads a tile's 10 x 10-pixel input halo once, as one tiled TMA box {8 channels, 10, 10}
+// per 8-channel group, into the no-swizzle K-major layout [channel group][10 x 10 pixels][8 channels]: the A operand of tap
+// (dh, dw) is the same buffer with its start moved by (dh * 10 + dw) * 16 bytes (SBO = one 10-pixel row, LBO = one channel
+// group).  Image borders and the padding are TMA's out-of-bounds zero fill; pixels past the image are computed and masked in
+// the epilogue.  Each CTA serves one N tile and keeps its 9 x C x BN filter slice resident in shared memory (16 channels per
+// box, 32-byte swizzle), loaded once before its first tile; the halo buffers form the mbarrier ring.
+// The k16 steps run tap-major, channels ascending, and the epilogue is conv_wgmma_kernel's, so every output equals that kernel's
+// bit for bit, except that its zero-filled steps past C (C = 48 / 96) can turn a -0 into +0.
+constexpr int HALO_W = 10, HALO_H = 10, HALO_TILE = 8;
+constexpr uint32_t HALO_CG_BYTES = 1664;  // one channel group of the halo: 10 x 10 x 16 bytes, padded to the TMA's 128-byte alignment
+constexpr uint32_t HALO_CTRL_BYTES = CTRL_BAR_BYTES + 16;  // + the filter barrier
+constexpr int HALO_MAX_STAGES = 6;
+
+// N tiles up to 48 wide are held to 80 registers so that two CTAs can share an SM.
+template <int BN>
+__global__ void __launch_bounds__(NUM_THREADS, BN <= 48 ? 2 : 1)
+conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
+  SGB_GRID_DEP_LAUNCH();
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const int ksteps = p.C / 16;
+  constexpr uint32_t b_box = BN * 32;  // 16 channels of BN filter rows
+  const uint32_t b_bytes = 9u * ksteps * b_box;
+  const uint32_t a_stage = ((uint32_t)(p.C / 8) * HALO_CG_BYTES + 1023u) & ~1023u;
+  const uint32_t sb = smem_base, sa0 = smem_base + ((b_bytes + 1023u) & ~1023u);
+  const uint32_t ctrl = sa0 + p.stages * a_stage;
+  auto full_bar = [&](int s) { return ctrl + 8u * s; };
+  auto empty_bar = [&](int s) { return ctrl + 8u * (MAX_STAGES + s); };
+  const uint32_t b_bar = ctrl + CTRL_BAR_BYTES;
+  float* s_part = reinterpret_cast<float*>(smem_raw + (ctrl + HALO_CTRL_BYTES - smem_u32(smem_raw)));  // [2 wg][4 warps][2][BN]
+  float* s_stats = s_part + 8 * 2 * BN;                                                                  // [2 wg][2][N]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tiles = p.M;  // here: the number of 8 x 8 tiles
+  const int nt = blockIdx.x % p.n_tiles;
+  const int mt_step = gridDim.x / p.n_tiles;
+  const int mt0 = blockIdx.x / p.n_tiles;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 4);  // one arrival per warp of the consuming warpgroup
+    }
+    mbar_init(b_bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  if (p.stats)
+    for (int i = threadIdx.x; i < 4 * p.N; i += NUM_THREADS) s_stats[i] = 0.f;
+  __syncthreads();
+  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
+
+  if (warp == 0) {
+    // ===================================================================================== TMA producer
+    if (elect_one()) {
+      mbar_expect_tx(b_bar, b_bytes);
+      for (int bt = 0; bt < 9; ++bt)
+        for (int ks = 0; ks < ksteps; ++ks)
+          tma_load_2d(sb + (uint32_t)(bt * ksteps + ks) * b_box, &map_b, b_bar, bt * p.b_cols_per_tap + 16 * ks, nt * BN);
+      const uint32_t a_tx = (uint32_t)(p.C / 8) * (HALO_H * HALO_W * 16);
+      int stg = 0;
+      uint32_t par = 1;  // the first pass through the ring is free
+      for (int mt = mt0; mt < m_tiles; mt += mt_step) {
+        const int n_img = mt / p.halo_thw;
+        const int rem = mt - n_img * p.halo_thw;
+        const int th = rem / p.halo_tw, tw = rem - th * p.halo_tw;
+        mbar_wait(empty_bar(stg), par);
+        const uint32_t sa = sa0 + stg * a_stage;
+        mbar_expect_tx(full_bar(stg), a_tx);
+        for (int cg = 0; cg < p.C / 8; ++cg)
+          tma_load_tiled_4d(sa + (uint32_t)cg * HALO_CG_BYTES, &map_a, full_bar(stg), 8 * cg, tw * HALO_TILE - 1, th * HALO_TILE - 1,
+                            n_img);
+        if (++stg == p.stages) {
+          stg = 0;
+          par ^= 1;
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================================================================================== MMA + epilogue
+    const int wg = (warp >> 2) - 1;  // takes tiles wg, wg + 2, wg + 4, ... of the CTA's sequence
+    const int wq = warp & 3;
+    float acc[BN / 2];
+    mbar_wait(b_bar, 0);
+    for (int j = wg, mt = mt0 + wg * mt_step; mt < m_tiles; j += 2, mt += 2 * mt_step) {
+      const int stg = j % p.stages;
+      mbar_wait(full_bar(stg), (uint32_t)(j / p.stages) & 1u);
+      const uint32_t sa = sa0 + stg * a_stage;
+      wgmma_fence();
+      // one flat loop over (tap, 16-channel step): a nested loop makes ptxas fence the accumulators at every tap
+      uint32_t sa_t = sa, sb_t = sb + (uint32_t)(p.tap_b[0] * ksteps) * b_box;
+      for (int k = 0, t = 0, ks = 0; k < 9 * ksteps; ++k) {
+        const uint64_t da = smem_desc_noswizzle(sa_t + (uint32_t)(2 * ks) * HALO_CG_BYTES, HALO_CG_BYTES, HALO_W * 16);
+        const uint64_t db = smem_desc(sb_t + (uint32_t)ks * b_box, 32, 16u, 256u);
+        mma_kk<BN>(acc, da, db, k != 0);
+        if (++ks == ksteps && ++t < 9) {
+          ks = 0;
+          sa_t = sa + (uint32_t)((t / 3) * HALO_W + t % 3) * 16u;
+          sb_t = sb + (uint32_t)(p.tap_b[t] * ksteps) * b_box;
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(stg));
+
+      // ---- epilogue: thread holds output rows 2 wq and 2 wq + 1 of the tile, column lane / 4
+      const int n_img = mt / p.halo_thw;
+      const int rem = mt - n_img * p.halo_thw;
+      const int th = rem / p.halo_tw, tw = rem - th * p.halo_tw;
+      const int ow = tw * HALO_TILE + (lane >> 2);
+      long long orow[2];
+      bool row_ok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int oh = th * HALO_TILE + 2 * wq + h;
+        row_ok[h] = oh < p.P && ow < p.Q;
+        orow[h] = row_ok[h] ? ((long long)n_img * p.P + oh) * p.Q + ow : 0;
+      }
+      tile_epilogue<BN, 4>(p, acc, orow, row_ok, nt, wg, wq, lane, s_part + wg * 4 * 2 * BN, s_stats + wg * 2 * p.N);
     }
   }
+  __syncthreads();
+  if (p.stats) {  // the two warpgroups' totals, in a fixed order
+    for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) s_stats[i] += s_stats[2 * p.N + i];
+    __syncthreads();
+  }
+  flush_stats(p, s_stats);
 }
 
 // ------------------------------------------------------------------------------------------------ wgrad kernel
@@ -407,7 +571,11 @@ EncodeTiledFn g_tiled = nullptr;
 EncodeIm2colFn g_im2col = nullptr;
 int g_num_sms = 0;
 long long g_launches = 0;
+long long g_halo_launches = 0;
+bool g_force_im2col = false;
 long long launch_count() { return g_launches; }
+long long halo_launch_count() { return g_halo_launches; }
+void force_im2col(bool on) { g_force_im2col = on; }
 
 int init_driver() {
   if (g_tiled && g_im2col) return SGB_OK;
@@ -470,6 +638,9 @@ typedef void (*WgradFn)(const CUtensorMap, const CUtensorMap, const WParams);
 Variant<ConvFn> g_conv[] = {{16, conv_wgmma_kernel<16>, 0, false},   {32, conv_wgmma_kernel<32>, 0, false},
                             {48, conv_wgmma_kernel<48>, 0, false},   {64, conv_wgmma_kernel<64>, 0, false},
                             {96, conv_wgmma_kernel<96>, 0, false},   {128, conv_wgmma_kernel<128>, 0, false}};
+Variant<ConvFn> g_halo[] = {{16, conv3x3_halo_kernel<16>, 0, false},   {32, conv3x3_halo_kernel<32>, 0, false},
+                            {48, conv3x3_halo_kernel<48>, 0, false},   {64, conv3x3_halo_kernel<64>, 0, false},
+                            {96, conv3x3_halo_kernel<96>, 0, false},   {128, conv3x3_halo_kernel<128>, 0, false}};
 Variant<WgradFn> g_wgrad[] = {{16, wgrad_wgmma_kernel<16>, 0, false}, {32, wgrad_wgmma_kernel<32>, 0, false},
                               {48, wgrad_wgmma_kernel<48>, 0, false}, {64, wgrad_wgmma_kernel<64>, 0, false},
                               {96, wgrad_wgmma_kernel<96>, 0, false}, {128, wgrad_wgmma_kernel<128>, 0, false}};
@@ -495,6 +666,95 @@ int pick_bn(int n) {
     if (waste < best_waste) { best_waste = waste; best = bn; }
   }
   return best;
+}
+
+// Shared memory of conv3x3_halo_kernel: the resident filter slice, `stages` halo buffers, barriers and statistics partials.
+size_t halo_smem(int C, int bn, int n, bool stats, int stages) {
+  const size_t b_bytes = ((size_t)9 * C * bn * 2 + 1023) & ~(size_t)1023;
+  const size_t a_stage = ((size_t)(C / 8) * HALO_CG_BYTES + 1023) & ~(size_t)1023;
+  return 1024 + b_bytes + (size_t)stages * a_stage + HALO_CTRL_BYTES + (stats ? (size_t)(8 * 2 * bn + 4 * n) * 4 : 0);
+}
+
+// Shape rule of the halo kernel, from the per-shape timings of tools/time_conv_halo.py: a 3x3 / stride-1 / pad-1 "same"
+// convolution with plain NHWC rows whose 8 x 8 tiles put at least 85 % of the MMA rows inside the image (160², 80², 56², 40²
+// maps; not 28², 20², 14², 7²), with the filter slice and two halo buffers in one CTA's shared memory.  Returns its N tile:
+// pick_bn's, else -- for at most 96 gathered channels -- a narrower one of at least 64 columns that pads N no more (each N tile
+// reloads the halo; narrowed tiles over 128 channels lost to conv_wgmma_kernel); 0: the shape stays on conv_wgmma_kernel.
+// The N tile does not change any output: each column is its own dot product.
+int halo_bn(const Problem& q) {
+  if (q.R != 3 || q.S != 3 || q.stride != 1 || q.pad != 1 || q.ntaps > 0 || q.out_mode != 0) return 0;
+  if (q.P != q.H || q.Q != q.W) return 0;
+  const long long covered = (long long)((q.P + 7) / 8) * 8 * ((q.Q + 7) / 8) * 8;
+  if (20ll * q.P * q.Q < 17 * covered) return 0;
+  const int n = q.b_rows, full = pick_bn(n);
+  auto waste = [&](int bn) { return (n + bn - 1) / bn * bn - n; };
+  for (int bn : {full, 96, 64})
+    if (bn <= full && (bn == full || (q.C <= 96 && bn >= 64 && waste(bn) <= waste(full))) &&
+        halo_smem(q.C, bn, n, q.stats != nullptr, 2) <= 227 * 1024)
+      return bn;
+  return 0;
+}
+
+int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
+  Params p = p0;
+  p.n_tiles = (p.N + bn - 1) / bn;
+  p.halo_tw = (q.Q + HALO_TILE - 1) / HALO_TILE;
+  p.halo_thw = p.halo_tw * ((q.P + HALO_TILE - 1) / HALO_TILE);
+  p.M = q.N * p.halo_thw;  // tiles
+  Variant<ConvFn>* var = nullptr;
+  for (auto& v : g_halo)
+    if (v.bn == bn) var = &v;
+  if (int rc = prepare(*var, "conv3x3_halo_kernel")) return rc;
+  const int regs_alloc = ((var->regs + 7) / 8) * 8 * NUM_THREADS;
+  int ctas_per_sm = 65536 / regs_alloc;
+  if (ctas_per_sm > 2) ctas_per_sm = 2;
+  if (ctas_per_sm < 1) ctas_per_sm = 1;
+  int stages = 0;
+  for (;; --ctas_per_sm) {
+    const size_t budget = (ctas_per_sm == 1 ? 227u : 227u / ctas_per_sm - 1u) * 1024u;
+    for (stages = HALO_MAX_STAGES; stages >= 2 && halo_smem(q.C, bn, p.N, p.stats != nullptr, stages) > budget; --stages) {
+    }
+    if (stages >= 2 || ctas_per_sm == 1) break;
+  }
+  if (stages < 2) { sgb_set_error("conv3x3_halo: tile does not fit shared memory"); return SGB_E_UNSUPPORTED; }
+  p.stages = stages;
+  const size_t smem = halo_smem(q.C, bn, p.N, p.stats != nullptr, stages);
+
+  alignas(64) CUtensorMap map_a, map_b;
+  {
+    cuuint64_t dims[4] = {(cuuint64_t)q.C, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
+    cuuint64_t strides[3] = {(cuuint64_t)q.a_pitch * 2, (cuuint64_t)q.W * q.a_pitch * 2, (cuuint64_t)q.H * q.W * q.a_pitch * 2};
+    cuuint32_t box[4] = {8, HALO_W, HALO_H, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = g_tiled(&map_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.a), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      sgb_set_error("cuTensorMapEncodeTiled(halo) failed with %d (C=%d W=%d H=%d N=%d pitch=%d)", (int)r, q.C, q.W, q.H, q.N, q.a_pitch);
+      return SGB_E_CUDA;
+    }
+  }
+  {
+    cuuint64_t dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows};
+    cuuint64_t strides[1] = {(cuuint64_t)q.b_cols * 2};
+    cuuint32_t box[2] = {16, (cuuint32_t)bn};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = g_tiled(&map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(q.b), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      sgb_set_error("cuTensorMapEncodeTiled(halo B) failed with %d (cols=%d rows=%d BN=%d)", (int)r, q.b_cols, q.b_rows, bn);
+      return SGB_E_CUDA;
+    }
+  }
+  // every CTA serves one N tile: the grid is a multiple of n_tiles
+  int per_nt = g_num_sms * ctas_per_sm / p.n_tiles;
+  if (per_nt > p.M) per_nt = p.M;
+  if (per_nt < 1) per_nt = 1;
+  SGB_LAUNCH(var->fn, per_nt * p.n_tiles, NUM_THREADS, smem, st, map_a, map_b, p);
+  ++g_launches;
+  ++g_halo_launches;
+  return sgb_cuda_check(cudaGetLastError(), "conv3x3_halo_kernel");
 }
 
 }  // namespace
@@ -531,6 +791,8 @@ int launch(const Problem& q, cudaStream_t st) {
   p.y = (bf16*)q.y; p.y_pitch = q.y_pitch; p.y_off = q.y_off;
   p.scale = q.scale; p.shift = q.shift; p.residual = (const bf16*)q.residual;
   p.stats = q.stats; p.stats_repl = q.stats_repl > 0 ? q.stats_repl : 1; p.act = q.act;
+  if (!g_force_im2col)
+    if (const int hbn = halo_bn(q)) return launch_halo(q, p, hbn, st);
   Variant<ConvFn>* var = nullptr;
   for (auto& v : g_conv)
     if (v.bn == bn) var = &v;

@@ -182,6 +182,12 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, int row_bytes,
   return (uint64_t)((smem_addr >> 4) & 0x3fff) | ((uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16) |
          ((uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32) | (layout << 62);
 }
+// No-swizzle K-major descriptor: core matrices of 8 rows x 16 contiguous bytes; LBO = bytes between the two core matrices
+// along K (the next 8 channels), SBO = bytes between consecutive 8-row groups along M / N.  Any 16-byte-aligned start is legal.
+__device__ __forceinline__ uint64_t smem_desc_noswizzle(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((smem_addr >> 4) & 0x3fff) | ((uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32);
+}
 
 __device__ __forceinline__ void tma_load_tiled_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
   asm volatile(
