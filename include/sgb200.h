@@ -45,6 +45,11 @@ typedef struct SgbConvDesc {
   int32_t x_pitch, x_off; /* channel pitch / offset of the buffer holding the input  (elements) */
   int32_t y_pitch, y_off; /* channel pitch / offset of the buffer holding the output (elements) */
   int32_t up2;            /* 1: ConvTranspose2d(k=2,s=2) mode -- see sgb_convt2x2_* */
+  /* 0, or the first of the K channels (fprop: output channels; dgrad: dy channels; wgrad: dy rows) whose eight off-centre
+   * filter taps are known to be zero (fprop, dgrad) or not wanted (wgrad: those dw entries are left as they are) -- the folded
+   * QARepVGG filter [K3 ; centre(alpha*K1 + I)].  The kernels skip that work; the results are the same.  Needs R = S = 3,
+   * stride 1, pad 1, 0 < centre_from < K and centre_from % 16 == 0, else SGB_E_INVALID. */
+  int32_t centre_from;
 } SgbConvDesc;
 
 /* Fused epilogue of the forward implicit GEMM.  All pointers may be NULL. */

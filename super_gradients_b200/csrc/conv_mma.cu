@@ -479,6 +479,9 @@ int check_desc(const SgbConvDesc* d) {
   SGB_REQUIRE(d->x_pitch % 8 == 0 && d->x_off % 8 == 0, "x pitch/offset must be multiples of 8");
   SGB_REQUIRE(d->x_pitch >= d->x_off + d->C, "x slice exceeds pitch");
   SGB_REQUIRE(d->y_pitch >= d->y_off + d->K, "y slice exceeds pitch");
+  SGB_REQUIRE(d->centre_from == 0 || (d->R == 3 && d->S == 3 && d->stride == 1 && d->pad == 1 && d->centre_from > 0 &&
+                                      d->centre_from < d->K && d->centre_from % 16 == 0),
+              "centre_from needs a 3x3 / stride-1 / pad-1 convolution and 0 < centre_from < K, a multiple of 16");
   return SGB_OK;
 }
 
@@ -494,6 +497,7 @@ extern "C" int sgb_conv_fprop(const SgbConvDesc* d, const sgb_bf16* x, const sgb
     q.b = w; q.b_rows = d->K; q.b_cols = d->R * d->S * d->C; q.b_cols_per_tap = d->C;
     q.R = d->R; q.S = d->S; q.stride = d->stride; q.pad = d->pad; q.P = d->P; q.Q = d->Q; q.flip = 0;
     q.y = y; q.y_pitch = d->y_pitch; q.y_off = d->y_off;
+    q.centre_from = d->centre_from;
     if (ep) {
       q.scale = ep->scale; q.shift = ep->shift; q.residual = ep->residual; q.stats = ep->stats;
       q.stats_repl = ep->stats_repl > 0 ? ep->stats_repl : 1; q.act = ep->act;
@@ -510,6 +514,7 @@ extern "C" int sgb_conv_fprop(const SgbConvDesc* d, const sgb_bf16* x, const sgb
         (long long)d->N * (d->H / 2) < (1ll << 31)) {
       q.N = d->N * (d->H / 2); q.H = 2; q.W = d->W / 2; q.C = 2 * d->C; q.a_pitch = 2 * d->C;
       q.b_cols_per_tap = 2 * d->C;
+      q.centre_from = 0;  // a 2 x 2 filter: check_desc refused a non-zero field
       q.R = 1; q.S = 1; q.stride = 1; q.pad = 0; q.P = 1; q.Q = d->W / 2;
       q.ntaps = 2;
       q.tap_dh[0] = 0; q.tap_dw[0] = 0; q.tap_b[0] = 0;
@@ -640,6 +645,7 @@ extern "C" int sgb_conv_dgrad(const SgbConvDesc* d, const sgb_bf16* dy, const sg
     q.y = dx; q.y_pitch = d->x_pitch; q.y_off = d->x_off;
     q.residual = accumulate ? dx : nullptr;
     q.stats_repl = 1;
+    q.centre_from = d->centre_from;
     if (sm100::supported(q)) return sm100::launch(q, (cudaStream_t)stream);
   }
   if (s == 2 && d->K % 16 == 0 && d->R == 3 && d->S == 3 && d->pad == 1 && d->C % 8 == 0 && d->H % 2 == 0 &&
@@ -754,6 +760,7 @@ extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb
     q.K = d->K; q.y_pitch = d->y_pitch;
     q.R = d->R; q.S = d->S; q.stride = d->stride; q.pad = d->pad; q.P = d->P; q.Q = d->Q;
     q.dw = dw;
+    q.centre_from = d->centre_from;
     if (sm100::wgrad_supported(q)) return sm100::wgrad_launch(q, (cudaStream_t)stream);
     // 2 x 2 / stride 2 / no padding over a dense x: the same re-description as in sgb_conv_fprop -- a (2 x 1)-tap stride-1 valid
     // convolution over the image [N * H/2][2][W/2][2C]; dW rows [K][dh][(dw, c)] are the KRSC rows of the 2 x 2 filter.

@@ -57,7 +57,22 @@ struct Params {
   double* stats;
   int stats_repl;
   int act;
+  // folded QARepVGG filters (Problem::centre_from): output columns >= centre_n (fprop) / gathered channels >= centre_c (dgrad)
+  // meet only zeros on the eight off-centre taps (tap 4 of 9 is the centre); 0: off
+  int centre_n, centre_c;
 };
+
+// The k-steps per off-centre tap on N tile nt when a folded filter's zero taps are skipped (of `steps` per tap, each over
+// step_ch gathered channels; the centre tap runs all of them): none for a tile wholly at or past centre_n, those below centre_c.
+// A tile that straddles centre_n runs every tap: issuing its off-centre taps as wgmmas of half the tile's width measured slower
+// than the full width in the halo kernel.  Each product skipped is one by an exact zero, so skipping changes no sum.
+template <int BN>
+__device__ __forceinline__ int off_centre_steps(const Params& p, int nt, int steps, int step_ch) {
+  if (p.centre_n > 0 && nt * BN >= p.centre_n) return 0;
+  if (p.centre_c > 0) return (p.centre_c + step_ch - 1) / step_ch;
+  return steps;
+}
+constexpr int CENTRE_TAP = 4;
 
 __device__ __forceinline__ long long out_row(const Params& p, long long m) {
   if (p.out_mode == 0) return m;
@@ -182,7 +197,8 @@ __device__ __forceinline__ void flush_stats(const Params& p, const float* s_stat
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-template <int BN>
+// SKIP: a folded QARepVGG filter (Params::centre_n / centre_c): the off-centre taps run off_centre_steps chunks.
+template <int BN, bool SKIP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
   SGB_GRID_DEP_LAUNCH();
@@ -200,7 +216,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   const int total_tiles = m_tiles * p.n_tiles;
   const int chunks = (p.C + p.KC - 1) / p.KC;  // a last chunk reaching past C is zero-filled by TMA (out-of-bounds channels)
-  const int k_iters = p.ntaps * chunks;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
@@ -228,10 +243,12 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         const int rem = m0 - n_img * pq;
         const int p0 = rem / p.Q, q0 = rem - p0 * p.Q;
         const int w0 = q0 * p.stride - p.pad, h0 = p0 * p.stride - p.pad;
+        const int off = SKIP ? off_centre_steps<BN>(p, nt, chunks, p.KC) : chunks;
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const int r = p.tap_dh[tap], s = p.tap_dw[tap];
           const int btap = p.tap_b[tap];
-          for (int ck = 0; ck < chunks; ++ck) {
+          const int n_ck = tap == CENTRE_TAP ? chunks : off;
+          for (int ck = 0; ck < n_ck; ++ck) {
             mbar_wait(empty_bar(stg), par);
             const uint32_t sa = smem_base + stg * stage_bytes, sb = sa + a_bytes;
             mbar_expect_tx(full_bar(stg), a_bytes + b_bytes);
@@ -257,6 +274,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     uint32_t par = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+      // the producer's k-sequence: taps in order, `chunks` k-iterations on the centre tap, fewer on the others when skipping
+      const int k_iters = SKIP ? 8 * off_centre_steps<BN>(p, nt, chunks, p.KC) + chunks : p.ntaps * chunks;
       int prev = -1;
       for (int k = 0; k < k_iters; ++k) {
         mbar_wait(full_bar(stg), par);
@@ -319,8 +338,9 @@ constexpr uint32_t HALO_CG_BYTES = 1664;  // one channel group of the halo: 10 x
 constexpr uint32_t HALO_CTRL_BYTES = CTRL_BAR_BYTES + 16;  // + the filter barrier
 constexpr int HALO_MAX_STAGES = 6;
 
-// N tiles up to 48 wide are held to 80 registers so that two CTAs can share an SM.
-template <int BN>
+// N tiles up to 48 wide are held to 80 registers so that two CTAs can share an SM.  SKIP: a folded QARepVGG filter
+// (Params::centre_n / centre_c): the off-centre taps run off_centre_steps k16 steps.
+template <int BN, bool SKIP>
 __global__ void __launch_bounds__(NUM_THREADS, BN <= 48 ? 2 : 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
   SGB_GRID_DEP_LAUNCH();
@@ -343,6 +363,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   const int nt = blockIdx.x % p.n_tiles;
   const int mt_step = gridDim.x / p.n_tiles;
   const int mt0 = blockIdx.x / p.n_tiles;
+  // k16 steps of each off-centre tap (the centre tap runs ksteps)
+  const int off = SKIP ? off_centre_steps<BN>(p, nt, ksteps, 16) : ksteps;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
@@ -361,9 +383,10 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   if (warp == 0) {
     // ===================================================================================== TMA producer
     if (elect_one()) {
-      mbar_expect_tx(b_bar, b_bytes);
+      // the filter boxes the MMAs read (B tap 4 is the centre, flipped or not); the others stay unloaded
+      mbar_expect_tx(b_bar, (uint32_t)(8 * off + ksteps) * b_box);
       for (int bt = 0; bt < 9; ++bt)
-        for (int ks = 0; ks < ksteps; ++ks)
+        for (int ks = 0; ks < (bt == CENTRE_TAP ? ksteps : off); ++ks)
           tma_load_2d(sb + (uint32_t)(bt * ksteps + ks) * b_box, &map_b, b_bar, bt * p.b_cols_per_tap + 16 * ks, nt * BN);
       const uint32_t a_tx = (uint32_t)(p.C / 8) * (HALO_H * HALO_W * 16);
       int stg = 0;
@@ -395,13 +418,15 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
       mbar_wait(full_bar(stg), (uint32_t)(j / p.stages) & 1u);
       const uint32_t sa = sa0 + stg * a_stage;
       wgmma_fence();
-      // one flat loop over (tap, 16-channel step): a nested loop makes ptxas fence the accumulators at every tap
-      uint32_t sa_t = sa, sb_t = sb + (uint32_t)(p.tap_b[0] * ksteps) * b_box;
-      for (int k = 0, t = 0, ks = 0; k < 9 * ksteps; ++k) {
+      // one flat loop over (tap, 16-channel step): a nested loop makes ptxas fence the accumulators at every tap.  Taps in order,
+      // ksteps steps on the centre tap and `off` on the others (none: the loop starts at the centre).
+      int t = off > 0 ? 0 : CENTRE_TAP;
+      uint32_t sa_t = sa + (uint32_t)((t / 3) * HALO_W + t % 3) * 16u, sb_t = sb + (uint32_t)(p.tap_b[t] * ksteps) * b_box;
+      for (int k = 0, ks = 0, nk = 8 * off + ksteps; k < nk; ++k) {
         const uint64_t da = smem_desc_noswizzle(sa_t + (uint32_t)(2 * ks) * HALO_CG_BYTES, HALO_CG_BYTES, HALO_W * 16);
         const uint64_t db = smem_desc(sb_t + (uint32_t)ks * b_box, 32, 16u, 256u);
         mma_kk<BN>(acc, da, db, k != 0);
-        if (++ks == ksteps && ++t < 9) {
+        if (++ks == (t == CENTRE_TAP ? ksteps : off) && ++t < 9) {
           ks = 0;
           sa_t = sa + (uint32_t)((t / 3) * HALO_W + t % 3) * 16u;
           sb_t = sb + (uint32_t)(p.tap_b[t] * ksteps) * b_box;
@@ -442,19 +467,28 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
 // GEMM view: M = out-channels (64 per consumer warpgroup), N = NB in-channels of one tap, K = pixels.  Both operands are
 // "MN-major": a TMA box of [WPIX pixels][channels] IS the canonical MN-major swizzled layout (each K index is one swizzled
 // row), so dy and the im2col'd x stream straight from NHWC memory with no transpose.
-// One CTA = (128 out-channels) x (one tap) x (NB in-channels) x (pixel range).
+// One CTA = (one or two 64-row blocks of out-channels) x (one tap) x (NB in-channels) x (pixel range).  A tap takes the 64-row
+// blocks that cover K, or -- off the centre of a folded QARepVGG filter (centre_from) -- those that cover centre_from.  They are
+// paired into CTAs of 128 rows, one block per consumer warpgroup; an odd last block is a CTA of its own whose two warpgroups take
+// the even / odd pipeline stages and both add their partial sums into dW, so a layer of K <= 64 no longer pays for 128 rows.
 struct WParams {
   int K, C;            // out / in channels
   int R, S, stride, pad, P, Q;
   int npix;            // N*P*Q
   int CB;              // in-channels per im2col box (16 / 32 / 64)
-  int n_ctiles, n_ktiles;
+  int n_ctiles;
+  int rb_all, rb_off;  // 64-row blocks of the centre tap / of each other tap (== rb_all without centre_from)
+  int items;           // row items (CTAs per in-channel tile and pixel range) summed over the taps
   int pix_per_cta;     // multiple of WPIX
   int stages;
   int cpad;            // channel count of the KRSC output rows (x channels incl. padding)
   float* dw;
 };
 constexpr int WPIX = 64;  // pixels (GEMM K) per pipeline stage
+
+__host__ __device__ __forceinline__ int wgrad_row_blocks(const WParams& p, int tap) {
+  return p.R * p.S == 9 && tap != CENTRE_TAP ? p.rb_off : p.rb_all;
+}
 
 template <int NB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -471,12 +505,18 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
   auto empty_bar = [&](int s) { return ctrl + 8u * (MAX_STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // decode the CTA's work item
+  // decode the CTA's work item: pixel range, then tap, in-channel tile and row item (fastest)
   int w = blockIdx.x;
-  const int ktile = w % p.n_ktiles; w /= p.n_ktiles;
-  const int ctile = w % p.n_ctiles; w /= p.n_ctiles;
-  const int tap = w % (p.R * p.S); w /= p.R * p.S;
-  const int split = w;
+  const int split = w / (p.items * p.n_ctiles);
+  w -= split * p.items * p.n_ctiles;
+  int tap = 0, tap_items = (wgrad_row_blocks(p, 0) + 1) / 2;
+  while (w >= tap_items * p.n_ctiles) {
+    w -= tap_items * p.n_ctiles;
+    tap_items = (wgrad_row_blocks(p, ++tap) + 1) / 2;
+  }
+  const int ctile = w / tap_items, item = w - ctile * tap_items;
+  const bool shared_rows = 2 * item + 1 == wgrad_row_blocks(p, tap);  // one row block for both warpgroups
+  const int row0 = 128 * item;
   const int pix0 = split * p.pix_per_cta;
   const int pix1 = min(pix0 + p.pix_per_cta, p.npix);
   const int n_iters = (pix1 - pix0 + WPIX - 1) / WPIX;
@@ -484,7 +524,7 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);
+      mbar_init(empty_bar(s), shared_rows ? 4 : 8);  // one arrival per warp that reads the stage
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -502,10 +542,10 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
         for (int it = 0; it < n_iters; ++it) {
           mbar_wait(empty_bar(stg), par);
           const uint32_t sa = smem_base + stg * stage_bytes, sb = sa + a_bytes;
-          mbar_expect_tx(full_bar(stg), a_bytes + (uint32_t)boxes * b_box);
+          mbar_expect_tx(full_bar(stg), (shared_rows ? a_bytes / 2 : a_bytes) + (uint32_t)boxes * b_box);
           const int pix = pix0 + it * WPIX;
-          tma_load_2d(sa, &map_dy, full_bar(stg), ktile * 128, pix);
-          tma_load_2d(sa + WPIX * 128, &map_dy, full_bar(stg), ktile * 128 + 64, pix);
+          tma_load_2d(sa, &map_dy, full_bar(stg), row0, pix);
+          if (!shared_rows) tma_load_2d(sa + WPIX * 128, &map_dy, full_bar(stg), row0 + 64, pix);
           const int n_img = pix / pq;
           const int rem = pix - n_img * pq;
           const int p0 = rem / p.Q, q0 = rem - p0 * p.Q;
@@ -523,18 +563,21 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
       const int wg = (warp >> 2) - 1, wq = warp & 3;
       const int b_row_bytes = p.CB * 2;
       float acc[NB / 2];
-      int stg = 0, prev = -1;
+      // own row block: every stage; shared row block: stages wg, wg + 2, ...
+      const int it0 = shared_rows ? wg : 0, it_step = shared_rows ? 2 : 1;
+      const uint32_t a_off = shared_rows ? 0u : (uint32_t)wg * (WPIX * 128);
+      int stg = it0, prev = -1;
       uint32_t par = 0;
-      for (int it = 0; it < n_iters; ++it) {
+      for (int it = it0; it < n_iters; it += it_step) {
         mbar_wait(full_bar(stg), par);
-        const uint32_t sa = smem_base + stg * stage_bytes + (uint32_t)wg * (WPIX * 128), sb = smem_base + stg * stage_bytes + a_bytes;
+        const uint32_t sa = smem_base + stg * stage_bytes + a_off, sb = smem_base + stg * stage_bytes + a_bytes;
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < WPIX / 16; ++j) {
           // A: one 64-channel atom of 128-byte pixel rows; B: the boxes are consecutive MN atoms (LBO = box size)
           const uint64_t da = smem_desc(sa + (uint32_t)j * 16u * 128u, 128, WPIX * 128, 8 * 128);
           const uint64_t db = smem_desc(sb + (uint32_t)j * 16u * (uint32_t)b_row_bytes, b_row_bytes, b_box, 8u * (uint32_t)b_row_bytes);
-          mma_mn<NB>(acc, da, db, (it | j) != 0);
+          mma_mn<NB>(acc, da, db, (it != it0 || j != 0) ? 1u : 0u);
         }
         wgmma_commit();
         if (prev >= 0) {
@@ -543,17 +586,18 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
           if (lane == 0) mbar_arrive(empty_bar(prev));
         }
         prev = stg;
-        if (++stg == p.stages) {
-          stg = 0;
+        if ((stg += it_step) >= p.stages) {  // it_step <= 2 <= stages
+          stg -= p.stages;
           par ^= 1;
         }
       }
+      if (prev < 0) return;  // a shared row block with a single stage: nothing for warpgroup 1
       wgmma_wait<0>();
       fence_regs(acc);
       const int row_len = p.R * p.S * p.cpad;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int ko = ktile * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int ko = row0 + (shared_rows ? 0 : wg * 64) + wq * 16 + (lane >> 2) + 8 * h;
         if (ko < p.K) {
           float* drow = p.dw + (long long)ko * row_len + tap * p.cpad + ctile * NB + 2 * (lane & 3);
 #pragma unroll
@@ -635,12 +679,18 @@ struct Variant {
 };
 typedef void (*ConvFn)(const CUtensorMap, const CUtensorMap, const Params);
 typedef void (*WgradFn)(const CUtensorMap, const CUtensorMap, const WParams);
-Variant<ConvFn> g_conv[] = {{16, conv_wgmma_kernel<16>, 0, false},   {32, conv_wgmma_kernel<32>, 0, false},
-                            {48, conv_wgmma_kernel<48>, 0, false},   {64, conv_wgmma_kernel<64>, 0, false},
-                            {96, conv_wgmma_kernel<96>, 0, false},   {128, conv_wgmma_kernel<128>, 0, false}};
-Variant<ConvFn> g_halo[] = {{16, conv3x3_halo_kernel<16>, 0, false},   {32, conv3x3_halo_kernel<32>, 0, false},
-                            {48, conv3x3_halo_kernel<48>, 0, false},   {64, conv3x3_halo_kernel<64>, 0, false},
-                            {96, conv3x3_halo_kernel<96>, 0, false},   {128, conv3x3_halo_kernel<128>, 0, false}};
+Variant<ConvFn> g_conv[] = {{16, conv_wgmma_kernel<16, false>, 0, false},   {32, conv_wgmma_kernel<32, false>, 0, false},
+                            {48, conv_wgmma_kernel<48, false>, 0, false},   {64, conv_wgmma_kernel<64, false>, 0, false},
+                            {96, conv_wgmma_kernel<96, false>, 0, false},   {128, conv_wgmma_kernel<128, false>, 0, false}};
+Variant<ConvFn> g_conv_skip[] = {{16, conv_wgmma_kernel<16, true>, 0, false},   {32, conv_wgmma_kernel<32, true>, 0, false},
+                                 {48, conv_wgmma_kernel<48, true>, 0, false},   {64, conv_wgmma_kernel<64, true>, 0, false},
+                                 {96, conv_wgmma_kernel<96, true>, 0, false},   {128, conv_wgmma_kernel<128, true>, 0, false}};
+Variant<ConvFn> g_halo[] = {{16, conv3x3_halo_kernel<16, false>, 0, false},   {32, conv3x3_halo_kernel<32, false>, 0, false},
+                            {48, conv3x3_halo_kernel<48, false>, 0, false},   {64, conv3x3_halo_kernel<64, false>, 0, false},
+                            {96, conv3x3_halo_kernel<96, false>, 0, false},   {128, conv3x3_halo_kernel<128, false>, 0, false}};
+Variant<ConvFn> g_halo_skip[] = {{16, conv3x3_halo_kernel<16, true>, 0, false},   {32, conv3x3_halo_kernel<32, true>, 0, false},
+                                 {48, conv3x3_halo_kernel<48, true>, 0, false},   {64, conv3x3_halo_kernel<64, true>, 0, false},
+                                 {96, conv3x3_halo_kernel<96, true>, 0, false},   {128, conv3x3_halo_kernel<128, true>, 0, false}};
 Variant<WgradFn> g_wgrad[] = {{16, wgrad_wgmma_kernel<16>, 0, false}, {32, wgrad_wgmma_kernel<32>, 0, false},
                               {48, wgrad_wgmma_kernel<48>, 0, false}, {64, wgrad_wgmma_kernel<64>, 0, false},
                               {96, wgrad_wgmma_kernel<96>, 0, false}, {128, wgrad_wgmma_kernel<128>, 0, false}};
@@ -701,8 +751,12 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   p.halo_tw = (q.Q + HALO_TILE - 1) / HALO_TILE;
   p.halo_thw = p.halo_tw * ((q.P + HALO_TILE - 1) / HALO_TILE);
   p.M = q.N * p.halo_thw;  // tiles
+  // Of a folded filter the halo kernel skips only dgrad's zero taps (centre_c).  fprop runs every tap: a straddling N tile has
+  // nothing to skip, and the grid gives every N tile the same number of CTAs, so those of a centre-only tile finish early and
+  // idle -- skipping measured 1-4 % slower there (tools/time_zero_taps.py).
+  p.centre_n = 0;
   Variant<ConvFn>* var = nullptr;
-  for (auto& v : g_halo)
+  for (auto& v : p.centre_c > 0 ? g_halo_skip : g_halo)
     if (v.bn == bn) var = &v;
   if (int rc = prepare(*var, "conv3x3_halo_kernel")) return rc;
   const int regs_alloc = ((var->regs + 7) / 8) * 8 * NUM_THREADS;
@@ -791,10 +845,16 @@ int launch(const Problem& q, cudaStream_t st) {
   p.y = (bf16*)q.y; p.y_pitch = q.y_pitch; p.y_off = q.y_off;
   p.scale = q.scale; p.shift = q.shift; p.residual = (const bf16*)q.residual;
   p.stats = q.stats; p.stats_repl = q.stats_repl > 0 ? q.stats_repl : 1; p.act = q.act;
+  if (q.centre_from > 0) {
+    if (q.R != 3 || q.S != 3 || q.stride != 1 || q.pad != 1 || q.ntaps > 0 || q.centre_from % 16 != 0 ||
+        q.centre_from >= (q.flip ? q.C : q.b_rows))
+      return SGB_E_INVALID;
+    (q.flip ? p.centre_c : p.centre_n) = q.centre_from;
+  }
   if (!g_force_im2col)
     if (const int hbn = halo_bn(q)) return launch_halo(q, p, hbn, st);
   Variant<ConvFn>* var = nullptr;
-  for (auto& v : g_conv)
+  for (auto& v : p.centre_n > 0 || p.centre_c > 0 ? g_conv_skip : g_conv)
     if (v.bn == bn) var = &v;
   if (int rc = prepare(*var, "conv_wgmma_kernel")) return rc;
   // Small tiles leave the pipeline latency-bound: co-resident CTAs overlap each other's loads, MMAs and epilogues.
@@ -881,7 +941,14 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
     if (q.C % cand == 0) { nb = cand; break; }
   p.CB = nb % 64 == 0 ? 64 : (nb % 32 == 0 ? 32 : 16);
   p.n_ctiles = q.C / nb;
-  p.n_ktiles = (q.K + 127) / 128;
+  if (q.centre_from != 0 && (q.R != 3 || q.S != 3 || q.stride != 1 || q.pad != 1 || q.centre_from < 0 || q.centre_from >= q.K ||
+                             q.centre_from % 16 != 0))
+    return SGB_E_INVALID;
+  // the 64-row blocks that cover K (off the centre of a folded filter: centre_from), paired, with a shared odd last one
+  p.rb_all = (q.K + 63) / 64;
+  p.rb_off = q.centre_from > 0 ? (q.centre_from + 63) / 64 : p.rb_all;
+  p.items = 0;
+  for (int t = 0; t < q.R * q.S; ++t) p.items += (wgrad_row_blocks(p, t) + 1) / 2;
   p.cpad = q.C;
   p.dw = q.dw;
   Variant<WgradFn>* var = nullptr;
@@ -891,11 +958,15 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   const uint32_t stage_bytes = 2 * WPIX * 128 + (uint32_t)(nb / p.CB) * WPIX * p.CB * 2;
   int stages = (int)((200 * 1024 - CTRL_BAR_BYTES - 1024) / stage_bytes);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
+  // A CTA that shares one row block gives stage s to warpgroup s % 2 only when the ring has an even length.  With an odd one a
+  // warpgroup would wait for phase n of a stage whose phase n - 1 (the other warpgroup's) may not have completed, and a parity wait
+  // cannot tell the two apart.
+  if (p.rb_all % 2 || p.rb_off % 2) stages &= ~1;
   if (stages < 2) return SGB_E_UNSUPPORTED;
   p.stages = stages;
   const size_t smem = 1024 + (size_t)stages * stage_bytes + CTRL_BAR_BYTES;
   // pixel splits: fill ~2 waves of SMs, keep at least 8 pipeline iterations per CTA
-  const int base_ctas = p.n_ktiles * p.n_ctiles * q.R * q.S;
+  const int base_ctas = p.items * p.n_ctiles;
   const int total_iters = (p.npix + WPIX - 1) / WPIX;
   int splits = (2 * g_num_sms + base_ctas - 1) / base_ctas;
   if (splits > total_iters / 8) splits = total_iters / 8;

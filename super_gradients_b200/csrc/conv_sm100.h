@@ -24,6 +24,9 @@ struct Problem {
   const void* residual;
   double* stats;
   int stats_repl, act;
+  // 0, or SgbConvDesc::centre_from: fprop (flip 0) -- output channels from here on have zero off-centre taps; dgrad (flip 1) --
+  // gathered channels from here on meet zero off-centre taps.  Only with R = S = 3, stride 1, pad 1 and no tap table.
+  int centre_from;
 };
 
 struct WgradProblem {
@@ -33,6 +36,7 @@ struct WgradProblem {
   int K, y_pitch;
   int R, S, stride, pad, P, Q;
   float* dw;       // fp32 [K][R][S][C], accumulated into
+  int centre_from; // 0, or (3x3 only) rows from here on need only their centre tap: their off-centre dw entries are not written
 };
 
 bool enabled();

@@ -4,6 +4,8 @@ libsgb200 kernels (kernels.py).  torch only owns memory, streams and the autogra
 Activations are channels_last bf16 (NHWC); parameters stay fp32 (state-dict compatible with the reference) and are
 re-laid-out to bf16 KRSC / CRSK once per optimizer step (cached on the parameter's version counter).
 """
+import functools
+import inspect
 import weakref
 from types import SimpleNamespace
 from typing import Optional
@@ -403,7 +405,7 @@ def _has_slots(dest) -> bool:
     return slot is not None
 
 
-def _wgrad(x, dy, r, s, stride, pad, cin, *dests):
+def _wgrad(x, dy, r, s, stride, pad, cin, *dests, centre_from=0):
     """The weight gradient of one convolution, dw = fp32 KRSC conv_wgrad(x, dy), delivered to `dests`:
       ("oihw", rows, slot)                 dw[rows] -> that filter's OIHW gradient
       ("alpha", rows, slot, chain)         dw[rows] is the gradient of a QARepVGG block's alpha * K1 + I; chain = (w1, alpha, dab, bias1,
@@ -413,8 +415,10 @@ def _wgrad(x, dy, r, s, stride, pad, cin, *dests):
     A slot is the parameter's flat gradient slot, or None: the gradient goes to autograd.  Inside a train step, when every
     destination has its slots, nothing reads the result before flush_wgrads(): the launch goes to the step's side stream (when it
     has one) and the deliveries wait for the batched passes there.  Otherwise the gradient is computed and delivered now.
-    Returns per destination what autograd receives: a tensor or None ("oihw"), (dK1, dbias, dalpha) ("alpha"), a list ("stem")."""
+    Returns per destination what autograd receives: a tensor or None ("oihw"), (dK1, dbias, dalpha) ("alpha"), a list ("stem").
+    centre_from (a folded QARepVGG filter): rows from there on get only their centre tap, the only one the destinations read."""
     ctx = _CTX[0]
+    ckw = _centre_kw(K.conv_wgrad, centre_from) if centre_from else {}
     if ctx is not None and all(_has_slots(d) for d in dests):
         if ctx.side_stream is not None:
             dw = K.zeros((dy.shape[1], r, s, x.shape[1]), torch.float32, x.device)  # arena (host-side) or a fill on the current stream
@@ -422,11 +426,11 @@ def _wgrad(x, dy, r, s, stride, pad, cin, *dests):
             ev.record(torch.cuda.current_stream())
             with torch.cuda.stream(ctx.side_stream):
                 ctx.side_stream.wait_event(ev)
-                K.conv_wgrad(x, dy, r, s, stride, pad, dw_krsc=dw)
+                K.conv_wgrad(x, dy, r, s, stride, pad, dw_krsc=dw, **ckw)
             ctx.keep.append((x, dy, dw))
             ctx.side_used = True
         else:
-            dw = K.conv_wgrad(x, dy, r, s, stride, pad)
+            dw = K.conv_wgrad(x, dy, r, s, stride, pad, **ckw)
         out = []
         for kind, rows, slot, *chain in dests:  # the queued tensors (step arena or plain) stay referenced until flush_wgrads()
             if kind == "oihw":
@@ -440,7 +444,7 @@ def _wgrad(x, dy, r, s, stride, pad, cin, *dests):
                 ctx.stem_pending.append((dw, cin, *rows, slot))
                 out.append([None] * len(slot))
         return out
-    dw = K.conv_wgrad(x, dy, r, s, stride, pad)
+    dw = K.conv_wgrad(x, dy, r, s, stride, pad, **ckw)
     out = []
     for kind, rows, slot, *chain in dests:
         if kind == "stem":
@@ -786,9 +790,10 @@ def conv_bias(x, w, b, *, stride, pad, cache: WeightCache, act=None):
 # Folded QARepVGG (default; SGB_QAREP_FOLD=0 restores the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
 # of ONE 3x3 convolution with 2K output channels (rows [0, K) = the 3x3 filters, rows [K, 2K) = alpha * K1 + I embedded at the centre),
 # so y3 and u come out of one convolution launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
-# epilogue) and wgrad produces both gradients in one launch (for K <= 64 inside the M = 128 padding the 3x3 weight gradient pays
-# for anyway).  The folded filters are written in place by the step's batched re-layout launch (WeightCache.get_blocks) and the weight
-# gradient goes to the side stream.
+# epilogue) and wgrad produces both gradients in one launch.  The eight off-centre taps of rows [K, 2K) are zeros: the three calls
+# pass centre_from=K, and the kernels skip the products with those zeros (and, in wgrad, the off-centre gradients of those rows,
+# which nobody reads).  The folded filters are written in place by the step's batched re-layout launch (WeightCache.get_blocks) and
+# the weight gradient goes to the side stream.
 QAREP_FOLD = [__import__("os").environ.get("SGB_QAREP_FOLD", "1") != "0"]
 QAREP_FOLD_MAXPIX = [int(__import__("os").environ.get("SGB_QAREP_FOLD_MAXPIX", "0"))]  # > 0: fold only maps of at most this many pixels (N*H*W)
 _FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS stride-1 blocks that fold
@@ -796,6 +801,18 @@ _FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS st
 
 def qarep_fold_supported(cin: int, x_channels: int, kout: int, stride: int) -> bool:
     return stride == 1 and cin == x_channels and cin in _FOLD_CHANNELS and 2 * kout in _FOLD_CHANNELS
+
+
+@functools.lru_cache(maxsize=None)
+def _takes_centre_from(fn) -> bool:
+    return "centre_from" in inspect.signature(fn).parameters
+
+
+def _centre_kw(fn, kout: int) -> dict:
+    """centre_from=kout for a folded filter's convolution `fn` (kernels.conv_fprop / conv_dgrad / conv_wgrad) when the kernels
+    accept it (a multiple of 16).  Skipping the zero taps changes no result, so a substitute of `fn` without the keyword is called
+    without it."""
+    return {"centre_from": kout} if kout % 16 == 0 and _takes_centre_from(fn) else {}
 
 
 class _QARepVGG(torch.autograd.Function):
@@ -816,7 +833,7 @@ class _QARepVGG(torch.autograd.Function):
             # one filter [2K, 3, 3, C]: rows [0, K) = K3, rows [K, 2K) = alpha * K1 + I at the centre tap (tap 4 of 9)
             srcs = [(w3, None, False, slice(None, kout), (0, 0)), (w1, alpha, cfg.residual, slice(kout, None), (9, 4))]
             kf, cf = cfg.cache_fold.get_blocks(srcs, 3, 3, x.shape[1])
-            ycat = K.conv_fprop(x, kf, 2 * kout, 3, 3, 1, 1)
+            ycat = K.conv_fprop(x, kf, 2 * kout, 3, 3, 1, 1, **_centre_kw(K.conv_fprop, kout))
             y3, u, c3, c1 = ycat[:, :kout], ycat[:, kout:], cf, None
         else:
             k3, c3 = cfg.cache3.get(w3, c_pad=x.shape[1])
@@ -864,10 +881,11 @@ class _QARepVGG(torch.autograd.Function):
         dx = None
         if ctx.fold:
             if ctx.needs_input_grad[0]:
-                dx = K.conv_dgrad(dcat, ctx.c3, x.shape, 3, 3, 1, 1)
+                dx = K.conv_dgrad(dcat, ctx.c3, x.shape, 3, 3, 1, 1, **_centre_kw(K.conv_dgrad, kout))
             dx = _defer_finish(ctx.defer, dx)
-            # fp32 [2K, 3, 3, C]: rows [0, K) = dW3, the centre tap of rows [K, 2K) = d(alpha * K1 + I)
-            dw3, d1 = _wgrad(x, dcat, 3, 3, 1, 1, cin, ("oihw", slice(None, kout), sw3), dest1((slice(kout, None), slice(1, 2), slice(1, 2))))
+            # fp32 [2K, 3, 3, C]: rows [0, K) = dW3, the centre tap of rows [K, 2K) = d(alpha * K1 + I) (their other taps are not computed)
+            dw3, d1 = _wgrad(x, dcat, 3, 3, 1, 1, cin, ("oihw", slice(None, kout), sw3), dest1((slice(kout, None), slice(1, 2), slice(1, 2))),
+                             centre_from=kout)
         else:
             if ctx.needs_input_grad[0]:
                 dx = K.conv_dgrad(dy3, ctx.c3, x.shape, 3, 3, cfg.stride, 1)

@@ -195,8 +195,10 @@ def _with_count(sums: torch.Tensor) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------ conv family
-def conv_fprop(x, w_krsc, K, R, S, stride, pad, *, scale=None, shift=None, residual=None, stats=None, act=ACT_NONE, out=None, out_f32=False):
-    """y = act(conv(x, w) * scale + shift + residual); optionally accumulates per-channel sum / sum-of-squares."""
+def conv_fprop(x, w_krsc, K, R, S, stride, pad, *, scale=None, shift=None, residual=None, stats=None, act=ACT_NONE, out=None, out_f32=False,
+               centre_from=0):
+    """y = act(conv(x, w) * scale + shift + residual); optionally accumulates per-channel sum / sum-of-squares.
+    centre_from > 0: output channels from there on have zero off-centre taps (a folded QARepVGG filter), which are skipped."""
     require_cuda(x, "x")
     n, c, h, w = x.shape
     P = (h + 2 * pad - R) // stride + 1
@@ -215,13 +217,15 @@ def conv_fprop(x, w_krsc, K, R, S, stride, pad, *, scale=None, shift=None, resid
     ep.stats_repl = stats.shape[0] if stats is not None else 1
     ep.act = act_code(act)
     ep.out_f32 = 1 if out_f32 else 0
+    d.centre_from = centre_from
     if residual is not None and nhwc_pitch(residual) != d.y_pitch:
         raise L.SgbError("residual must share the output's channel pitch")
     _timed("sgb_conv_fprop", ctypes.byref(d), _ptr(x), _ptr(w_krsc), _ptr(out), ctypes.byref(ep), _stream())
     return out
 
 
-def conv_dgrad(dy, w_crsk, x_shape, R, S, stride, pad, out=None, accumulate=False):
+def conv_dgrad(dy, w_crsk, x_shape, R, S, stride, pad, out=None, accumulate=False, centre_from=0):
+    """centre_from > 0: dy channels from there on meet zero off-centre taps (a folded QARepVGG filter), which are skipped."""
     n, c, h, w = x_shape
     K = dy.shape[1]
     if out is None:
@@ -232,17 +236,20 @@ def conv_dgrad(dy, w_crsk, x_shape, R, S, stride, pad, out=None, accumulate=Fals
     d.stride, d.pad = stride, pad
     d.x_pitch, d.x_off = nhwc_pitch(out), 0
     d.y_pitch, d.y_off = nhwc_pitch(dy), 0
+    d.centre_from = centre_from
     _timed("sgb_conv_dgrad", ctypes.byref(d), _ptr(dy), _ptr(w_crsk), _ptr(out), 1 if accumulate else 0, _stream())
     return out
 
 
-def conv_wgrad(x, dy, R, S, stride, pad, dw_krsc=None):
-    """Returns fp32 [K, R, S, C] (C = x.shape[1], i.e. including any channel padding of x)."""
+def conv_wgrad(x, dy, R, S, stride, pad, dw_krsc=None, centre_from=0):
+    """Returns fp32 [K, R, S, C] (C = x.shape[1], i.e. including any channel padding of x).  centre_from > 0: rows from there on
+    get only their centre tap; their off-centre entries of dw_krsc are left as they are (zero when it is allocated here)."""
     n, c, h, w = x.shape
     K = dy.shape[1]
     if dw_krsc is None:
         dw_krsc = zeros((K, R, S, c), torch.float32, x.device)
     d = conv_desc(x, K, R, S, stride, pad, dy, dy.shape[2], dy.shape[3])
+    d.centre_from = centre_from
     _timed("sgb_conv_wgrad", ctypes.byref(d), _ptr(x), _ptr(dy), _ptr(dw_krsc), _stream())
     return dw_krsc
 

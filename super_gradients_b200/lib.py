@@ -18,7 +18,7 @@ class SgbError(RuntimeError):
 
 
 class ConvDesc(Structure):
-    _fields_ = [(n, c_int32) for n in ("N", "H", "W", "C", "K", "R", "S", "P", "Q", "stride", "pad", "x_pitch", "x_off", "y_pitch", "y_off", "up2")]
+    _fields_ = [(n, c_int32) for n in ("N", "H", "W", "C", "K", "R", "S", "P", "Q", "stride", "pad", "x_pitch", "x_off", "y_pitch", "y_off", "up2", "centre_from")]
 
 
 class Epilogue(Structure):
