@@ -75,6 +75,12 @@ int64_t sgb_conv_halo_launches(void);
 /* Test-only: on != 0 sends every later 3x3 / stride-1 convolution to the im2col wgmma kernel instead of the halo-tile kernel,
  * so tests and timing tools can compare the two engines on one shape.  Not a user option. */
 void sgb_conv_force_im2col(int on);
+/* Number of wgmma/TMA launches served by the halo-tile weight-gradient kernel of 3x3 / stride-1 convolutions
+ * (wgrad3x3_halo_kernel). */
+int64_t sgb_conv_wgrad_halo_launches(void);
+/* Test-only: on != 0 sends every later 3x3 / stride-1 weight gradient to the per-tap wgmma kernel (wgrad_wgmma_kernel) instead
+ * of the halo-tile kernel, so tests and timing tools can compare the two engines on one shape.  Not a user option. */
+void sgb_conv_wgrad_force_im2col(int on);
 
 /* ---- convolution family (rows C1-C5, C8, C10 of SURVEY.md section 8a) --------------------------------------
  * replaces nn.Conv2d forward in modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,

@@ -38,3 +38,5 @@ extern "C" int sgb_check_device(void) {
 extern "C" int64_t sgb_sm100_launches(void) { return (int64_t)sm100::launch_count(); }
 extern "C" int64_t sgb_conv_halo_launches(void) { return (int64_t)sm100::halo_launch_count(); }
 extern "C" void sgb_conv_force_im2col(int on) { sm100::force_im2col(on != 0); }
+extern "C" int64_t sgb_conv_wgrad_halo_launches(void) { return (int64_t)sm100::wgrad_halo_launch_count(); }
+extern "C" void sgb_conv_wgrad_force_im2col(int on) { sm100::wgrad_force_im2col(on != 0); }

@@ -9,8 +9,8 @@
 //
 // Serves every 1x1 and 3x3 convolution with C % 16 == 0 (fprop; stride-1 dgrad over the flipped CRSK filter; stride-2 dgrad as
 // s^2 output-parity classes through the explicit tap table) and their weight gradients (wgrad_wgmma_kernel, MN-major
-// operands).  3-channel stems that are not padded to 16 channels, 7x7, ragged channel counts and fp32 outputs stay on the
-// mma.sync kernels of conv_mma.cu.
+// operands; wgrad3x3_halo_kernel for the 3x3 stride-1 ones).  3-channel stems that are not padded to 16 channels, 7x7, ragged
+// channel counts and fp32 outputs stay on the mma.sync kernels of conv_mma.cu.
 //
 // Reference arithmetic replaced: nn.Conv2d forward / input-gradient / weight-gradient as used by
 // modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,
@@ -483,6 +483,7 @@ struct WParams {
   int stages;
   int cpad;            // channel count of the KRSC output rows (x channels incl. padding)
   float* dw;
+  int halo_tw, halo_thw, tiles, tiles_per_cta;  // wgrad3x3_halo_kernel: 8 x 8 tiles per image row band / per image / in all
 };
 constexpr int WPIX = 64;  // pixels (GEMM K) per pipeline stage
 
@@ -610,16 +611,174 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
   }
 }
 
+// ------------------------------------------------------------------------------------------------ halo-tile wgrad kernel
+// Weight gradient of a 3x3 / stride 1 / pad 1 convolution over 8 x 8 output tiles, loading each tile's dy block and input halo
+// once for all nine taps (wgrad_wgmma_kernel streams dy and an im2col view of x once per tap).  One CTA = one 64-row block rb of
+// out-channels x NB in-channels (in-channel tile ctile) x a range of tiles; GEMM M = the 64 rows, N = NB, K = the tile's 64 pixels.
+// Per stage the producer loads
+//   A: dy of the tile, one tiled TMA box {64 channels, 8, 8, 1} with 128-byte swizzle: 64 pixel rows of 128 bytes, the MN-major
+//      layout wgrad_wgmma_kernel reads; pixels past the image are zero-filled and add nothing;
+//   B: the 10 x 10 input halo of the NB channels, as conv3x3_halo_kernel loads it ([channel group][10 x 10 pixels][8 channels],
+//      image borders and padding from TMA's zero fill).  Read MN-major, 8 consecutive pixels of a halo row are one 128-byte core
+//      matrix: tap (dh, dw) starts (dh * 10 + dw) * 16 bytes in, the second 8 pixels of a k16 step (the next output row) lie one
+//      halo row (LBO = 160 bytes) on, the next 8 channels one channel group (SBO = HALO_CG_BYTES) on.
+// Warpgroup 0 accumulates taps 0-4 and warpgroup 1 taps 5-8 (9 x NB / 2 fp32 per thread would not fit one warpgroup), so both
+// read every stage and its empty barrier counts all eight consumer warps.  A row block past the off-centre rows of a folded
+// filter (rb >= rb_off) runs the centre tap alone, on warpgroup 0.  Each CTA adds its partial sums into dW once, at the end.
+constexpr uint32_t WH_A_BYTES = WPIX * 128;  // the dy tile of a stage
+
+__host__ __device__ constexpr uint32_t wgrad_halo_stage_bytes(int nb) {
+  return (WH_A_BYTES + (uint32_t)(nb / 8) * HALO_CG_BYTES + 1023u) & ~1023u;
+}
+
+// One consumer warpgroup of wgrad3x3_halo_kernel: taps tap0 .. tap0 + NT - 1 of every stage (NT = 0: none, the warpgroup only
+// frees the stages), then their partial sums into dW.  The tap count is a template parameter and the waits are unconditional so
+// that no branch separates the wgmmas of the loop: ptxas serialises wgmmas on a divergent path.
+template <int NB, int NT>
+__device__ __forceinline__ void wgrad_halo_consume(const WParams& p, uint32_t ring, uint32_t bars, int t0, int t1, int tap0, int rb,
+                                                   int ctile) {
+  constexpr uint32_t stage_bytes = wgrad_halo_stage_bytes(NB);
+  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  auto full_bar = [&](int s) { return bars + 8u * s; };
+  auto empty_bar = [&](int s) { return bars + 8u * (MAX_STAGES + s); };
+  float acc[NT > 0 ? NT : 1][NB / 2];
+  int stg = 0, prev = 0;
+  uint32_t par = 0;
+  for (int mt = t0; mt < t1; ++mt) {
+    mbar_wait(full_bar(stg), par);
+    if constexpr (NT > 0) {
+      const uint32_t sa = ring + stg * stage_bytes, sx = sa + WH_A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < NT; ++t) {
+        const int tap = tap0 + t;
+        const uint32_t sx_t = sx + (uint32_t)((tap / 3) * HALO_W + tap % 3) * 16u;
+#pragma unroll
+        for (int j = 0; j < WPIX / 16; ++j) {
+          const uint64_t da = smem_desc(sa + (uint32_t)j * 16u * 128u, 128, WPIX * 128, 8 * 128);
+          const uint64_t db = smem_desc_noswizzle(sx_t + (uint32_t)j * 2u * HALO_W * 16u, HALO_W * 16, HALO_CG_BYTES);
+          mma_mn<NB>(acc[t], da, db, (mt != t0 || j != 0) ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's MMAs are complete: its shared memory may be refilled
+    }
+    __syncwarp();
+    if (lane == 0 && mt != t0) mbar_arrive(empty_bar(prev));
+    prev = stg;
+    if (++stg == p.stages) {
+      stg = 0;
+      par ^= 1;
+    }
+  }
+  if constexpr (NT > 0) {
+    wgmma_wait<0>();
+#pragma unroll
+    for (int t = 0; t < NT; ++t) fence_regs(acc[t]);
+  }
+  __syncwarp();
+  if (lane == 0) mbar_arrive(empty_bar(prev));
+  if constexpr (NT > 0) {
+    const int row_len = 9 * p.cpad;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int ko = 64 * rb + wq * 16 + (lane >> 2) + 8 * h;
+      if (ko < p.K) {
+        float* drow = p.dw + (long long)ko * row_len + tap0 * p.cpad + ctile * NB + 2 * (lane & 3);
+#pragma unroll
+        for (int t = 0; t < NT; ++t)
+#pragma unroll
+          for (int j = 0; j < NB / 8; ++j)
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(drow + t * p.cpad + 8 * j), "f"(acc[t][4 * j + 2 * h]),
+                         "f"(acc[t][4 * j + 2 * h + 1])
+                         : "memory");
+      }
+    }
+  }
+}
+
+template <int NB>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+wgrad3x3_halo_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WParams p) {
+  SGB_GRID_DEP_LAUNCH();
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  constexpr uint32_t a_bytes = WH_A_BYTES, stage_bytes = wgrad_halo_stage_bytes(NB);
+  const uint32_t ctrl = smem_base + p.stages * stage_bytes;
+  auto full_bar = [&](int s) { return ctrl + 8u * s; };
+  auto empty_bar = [&](int s) { return ctrl + 8u * (MAX_STAGES + s); };
+
+  const int warp = threadIdx.x >> 5;
+  // work item: tile range (slowest), then in-channel tile, then row block
+  const int items = p.rb_all * p.n_ctiles;
+  const int split = blockIdx.x / items, item = blockIdx.x - split * items;
+  const int ctile = item / p.rb_all, rb = item - ctile * p.rb_all;
+  const bool all_taps = rb < p.rb_off;
+  const int t0 = split * p.tiles_per_cta, t1 = min(t0 + p.tiles_per_cta, p.tiles);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
+
+  if (warp == 0) {
+    // ===================================================================================== TMA producer
+    if (elect_one()) {
+      const uint32_t tx = a_bytes + (NB / 8) * (HALO_H * HALO_W * 16);
+      int stg = 0;
+      uint32_t par = 1;  // the first pass through the ring is free
+      for (int mt = t0; mt < t1; ++mt) {
+        const int n_img = mt / p.halo_thw;
+        const int rem = mt - n_img * p.halo_thw;
+        const int th = rem / p.halo_tw, tw = rem - th * p.halo_tw;
+        mbar_wait(empty_bar(stg), par);
+        const uint32_t sa = smem_base + stg * stage_bytes;
+        mbar_expect_tx(full_bar(stg), tx);
+        tma_load_tiled_4d(sa, &map_dy, full_bar(stg), 64 * rb, tw * HALO_TILE, th * HALO_TILE, n_img);
+        for (int cg = 0; cg < NB / 8; ++cg)
+          tma_load_tiled_4d(sa + a_bytes + (uint32_t)cg * HALO_CG_BYTES, &map_x, full_bar(stg), ctile * NB + 8 * cg,
+                            tw * HALO_TILE - 1, th * HALO_TILE - 1, n_img);
+        if (++stg == p.stages) {
+          stg = 0;
+          par ^= 1;
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================================================================================== MMA + epilogue
+    const int wg = (warp >> 2) - 1;
+    const uint32_t ring = smem_base, bars = ctrl;  // full barriers, then the empty ones at + 8 MAX_STAGES
+    if (!all_taps && wg == 0)
+      wgrad_halo_consume<NB, 1>(p, ring, bars, t0, t1, CENTRE_TAP, rb, ctile);
+    else if (!all_taps)
+      wgrad_halo_consume<NB, 0>(p, ring, bars, t0, t1, 0, rb, ctile);
+    else if (wg == 0)
+      wgrad_halo_consume<NB, 5>(p, ring, bars, t0, t1, 0, rb, ctile);
+    else
+      wgrad_halo_consume<NB, 4>(p, ring, bars, t0, t1, 5, rb, ctile);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 EncodeTiledFn g_tiled = nullptr;
 EncodeIm2colFn g_im2col = nullptr;
 int g_num_sms = 0;
 long long g_launches = 0;
 long long g_halo_launches = 0;
+long long g_wgrad_halo_launches = 0;
 bool g_force_im2col = false;
+bool g_wgrad_force_im2col = false;
 long long launch_count() { return g_launches; }
 long long halo_launch_count() { return g_halo_launches; }
+long long wgrad_halo_launch_count() { return g_wgrad_halo_launches; }
 void force_im2col(bool on) { g_force_im2col = on; }
+void wgrad_force_im2col(bool on) { g_wgrad_force_im2col = on; }
 
 int init_driver() {
   if (g_tiled && g_im2col) return SGB_OK;
@@ -694,6 +853,8 @@ Variant<ConvFn> g_halo_skip[] = {{16, conv3x3_halo_kernel<16, true>, 0, false}, 
 Variant<WgradFn> g_wgrad[] = {{16, wgrad_wgmma_kernel<16>, 0, false}, {32, wgrad_wgmma_kernel<32>, 0, false},
                               {48, wgrad_wgmma_kernel<48>, 0, false}, {64, wgrad_wgmma_kernel<64>, 0, false},
                               {96, wgrad_wgmma_kernel<96>, 0, false}, {128, wgrad_wgmma_kernel<128>, 0, false}};
+Variant<WgradFn> g_wgrad_halo[] = {{16, wgrad3x3_halo_kernel<16>, 0, false}, {32, wgrad3x3_halo_kernel<32>, 0, false},
+                                   {48, wgrad3x3_halo_kernel<48>, 0, false}};
 
 template <class Fn>
 int prepare(Variant<Fn>& v, const char* what) {
@@ -725,6 +886,12 @@ size_t halo_smem(int C, int bn, int n, bool stats, int stages) {
   return 1024 + b_bytes + (size_t)stages * a_stage + HALO_CTRL_BYTES + (stats ? (size_t)(8 * 2 * bn + 4 * n) * 4 : 0);
 }
 
+// The 8 x 8 tiles of a P x Q map put at least 85 % of the MMA rows inside the image (160², 80², 56², 40²; not 28², 20², 14², 7²).
+bool halo_tiles_fit(int P, int Q) {
+  const long long covered = (long long)((P + 7) / 8) * 8 * ((Q + 7) / 8) * 8;
+  return 20ll * P * Q >= 17 * covered;
+}
+
 // Shape rule of the halo kernel, from the per-shape timings of tools/time_conv_halo.py: a 3x3 / stride-1 / pad-1 "same"
 // convolution with plain NHWC rows whose 8 x 8 tiles put at least 85 % of the MMA rows inside the image (160², 80², 56², 40²
 // maps; not 28², 20², 14², 7²), with the filter slice and two halo buffers in one CTA's shared memory.  Returns its N tile:
@@ -734,8 +901,7 @@ size_t halo_smem(int C, int bn, int n, bool stats, int stages) {
 int halo_bn(const Problem& q) {
   if (q.R != 3 || q.S != 3 || q.stride != 1 || q.pad != 1 || q.ntaps > 0 || q.out_mode != 0) return 0;
   if (q.P != q.H || q.Q != q.W) return 0;
-  const long long covered = (long long)((q.P + 7) / 8) * 8 * ((q.Q + 7) / 8) * 8;
-  if (20ll * q.P * q.Q < 17 * covered) return 0;
+  if (!halo_tiles_fit(q.P, q.Q)) return 0;
   const int n = q.b_rows, full = pick_bn(n);
   auto waste = [&](int bn) { return (n + bn - 1) / bn * bn - n; };
   for (int bn : {full, 96, 64})
@@ -743,6 +909,22 @@ int halo_bn(const Problem& q) {
         halo_smem(q.C, bn, n, q.stats != nullptr, 2) <= 227 * 1024)
       return bn;
   return 0;
+}
+
+// The input-halo map of the halo kernels: an NHWC bf16 tensor of `pitch` elements per pixel, read as {8 channels, 10, 10, 1}
+// boxes, no swizzle; boxes reaching past the image or past C are zero-filled.
+int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, int pitch) {
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
+  cuuint32_t box[4] = {8, HALO_W, HALO_H, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    sgb_set_error("cuTensorMapEncodeTiled(halo) failed with %d (C=%d W=%d H=%d N=%d pitch=%d)", (int)r, C, W, H, N, pitch);
+    return SGB_E_CUDA;
+  }
+  return SGB_OK;
 }
 
 int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
@@ -775,19 +957,7 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   const size_t smem = halo_smem(q.C, bn, p.N, p.stats != nullptr, stages);
 
   alignas(64) CUtensorMap map_a, map_b;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)q.C, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
-    cuuint64_t strides[3] = {(cuuint64_t)q.a_pitch * 2, (cuuint64_t)q.W * q.a_pitch * 2, (cuuint64_t)q.H * q.W * q.a_pitch * 2};
-    cuuint32_t box[4] = {8, HALO_W, HALO_H, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = g_tiled(&map_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.a), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeTiled(halo) failed with %d (C=%d W=%d H=%d N=%d pitch=%d)", (int)r, q.C, q.W, q.H, q.N, q.a_pitch);
-      return SGB_E_CUDA;
-    }
-  }
+  if (int rc = encode_halo_map(&map_a, q.a, q.N, q.H, q.W, q.C, q.a_pitch)) return rc;
   {
     cuuint64_t dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows};
     cuuint64_t strides[1] = {(cuuint64_t)q.b_cols * 2};
@@ -930,6 +1100,65 @@ bool wgrad_supported(const WgradProblem& q) {
   return true;
 }
 
+namespace {
+
+// Shape rule of wgrad3x3_halo_kernel, from the per-shape timings of tools/time_conv_halo.py: the 3x3 / stride-1 / pad-1 "same"
+// convolutions whose 8 x 8 tiles cover the map with little waste (halo_tiles_fit), where it measured 1.13-5.5x faster than
+// wgrad_wgmma_kernel on every such shape of bench configurations 2-4; the smaller maps were not timed on it.  Returns its
+// in-channel tile (32 channels, else 48, else 16: each tile reads dy once more, and 5 taps x NB / 2 accumulators per thread must
+// fit the registers); 0: wgrad_wgmma_kernel serves the shape.
+int wgrad_halo_nb(const WgradProblem& q) {
+  if (q.R != 3 || q.S != 3 || q.stride != 1 || q.pad != 1 || q.P != q.H || q.Q != q.W) return 0;
+  if (!halo_tiles_fit(q.P, q.Q)) return 0;
+  return q.C % 32 == 0 ? 32 : (q.C % 48 == 0 ? 48 : 16);
+}
+
+int launch_wgrad_halo(const WgradProblem& q, const WParams& p0, int nb, cudaStream_t st) {
+  WParams p = p0;
+  p.n_ctiles = q.C / nb;
+  p.halo_tw = (q.Q + HALO_TILE - 1) / HALO_TILE;
+  p.halo_thw = p.halo_tw * ((q.P + HALO_TILE - 1) / HALO_TILE);
+  p.tiles = q.N * p.halo_thw;
+  Variant<WgradFn>* var = nullptr;
+  for (auto& v : g_wgrad_halo)
+    if (v.bn == nb) var = &v;
+  if (int rc = prepare(*var, "wgrad3x3_halo_kernel")) return rc;
+  const int ctas_per_sm = ((var->regs + 7) / 8) * 8 * NUM_THREADS * 2 <= 65536 ? 2 : 1;
+  const uint32_t stage_bytes = wgrad_halo_stage_bytes(nb);
+  const uint32_t budget = (ctas_per_sm == 1 ? 227u : 113u) * 1024u - 1024u - CTRL_BAR_BYTES;
+  p.stages = (int)(budget / stage_bytes);
+  if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
+  const size_t smem = 1024 + (size_t)p.stages * stage_bytes + CTRL_BAR_BYTES;
+  // tile ranges: one wave of CTAs over the (row block, in-channel tile) items
+  const int items = p.rb_all * p.n_ctiles;
+  int splits = g_num_sms * ctas_per_sm / items;
+  if (splits < 1) splits = 1;
+  p.tiles_per_cta = (p.tiles + splits - 1) / splits;
+  splits = (p.tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
+
+  alignas(64) CUtensorMap map_dy, map_x;
+  {
+    cuuint64_t dims[4] = {(cuuint64_t)q.K, (cuuint64_t)q.Q, (cuuint64_t)q.P, (cuuint64_t)q.N};
+    cuuint64_t strides[3] = {(cuuint64_t)q.y_pitch * 2, (cuuint64_t)q.Q * q.y_pitch * 2, (cuuint64_t)q.P * q.Q * q.y_pitch * 2};
+    cuuint32_t box[4] = {64, HALO_TILE, HALO_TILE, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = g_tiled(&map_dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.dy), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      sgb_set_error("cuTensorMapEncodeTiled(dy tile) failed with %d (K=%d Q=%d P=%d N=%d pitch=%d)", (int)r, q.K, q.Q, q.P, q.N, q.y_pitch);
+      return SGB_E_CUDA;
+    }
+  }
+  if (int rc = encode_halo_map(&map_x, q.x, q.N, q.H, q.W, q.C, q.x_pitch)) return rc;
+  SGB_LAUNCH(var->fn, splits * items, NUM_THREADS, smem, st, map_dy, map_x, p);
+  ++g_launches;
+  ++g_wgrad_halo_launches;
+  return sgb_cuda_check(cudaGetLastError(), "wgrad3x3_halo_kernel");
+}
+
+}  // namespace
+
 int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   if (int rc = init_driver()) return rc;
   WParams p{};
@@ -951,6 +1180,8 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   for (int t = 0; t < q.R * q.S; ++t) p.items += (wgrad_row_blocks(p, t) + 1) / 2;
   p.cpad = q.C;
   p.dw = q.dw;
+  if (!g_wgrad_force_im2col)
+    if (const int nb = wgrad_halo_nb(q)) return launch_wgrad_halo(q, p, nb, st);
   Variant<WgradFn>* var = nullptr;
   for (auto& v : g_wgrad)
     if (v.bn == nb) var = &v;

@@ -47,5 +47,7 @@ int launch(const Problem& q, cudaStream_t st);
 long long launch_count();       // every launch of the kernels of conv_sm100.cu
 long long halo_launch_count();  // the conv3x3_halo_kernel launches among them
 void force_im2col(bool on);     // test-only: 3x3 stride-1 convolutions skip the halo kernel
+long long wgrad_halo_launch_count();  // the wgrad3x3_halo_kernel launches among them
+void wgrad_force_im2col(bool on);     // test-only: 3x3 stride-1 weight gradients skip the halo kernel
 
 }  // namespace sm100

@@ -163,6 +163,8 @@ _SIGNATURES = {
     "sgb_sm100_launches": (c_int64, []),
     "sgb_conv_halo_launches": (c_int64, []),
     "sgb_conv_force_im2col": (None, [_I]),
+    "sgb_conv_wgrad_halo_launches": (c_int64, []),
+    "sgb_conv_wgrad_force_im2col": (None, [_I]),
     "sgb_conv_fprop": (c_int, [POINTER(ConvDesc), P, P, P, POINTER(Epilogue), P]),
     "sgb_conv_dgrad": (c_int, [POINTER(ConvDesc), P, P, P, _I, P]),
     "sgb_conv_wgrad": (c_int, [POINTER(ConvDesc), P, P, P, P]),
@@ -233,7 +235,7 @@ _SIGNATURES = {
 _lib = None
 
 # kernels launched by one call of each entry point (default 1); LAUNCHES[0] accumulates them (bench.py: gpu_launches)
-LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
+LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_conv_wgrad_halo_launches": 0, "sgb_conv_wgrad_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
 LAUNCHES = [0]
 
 
