@@ -144,8 +144,6 @@ __device__ __forceinline__ void chan_body(const Op& op, const int64_t M, const i
 // dynamic shared memory: [ring][coefficients + reduction scratch]
 template <class Op>
 __global__ void __launch_bounds__(TPB) chan_kernel(const Op op, const int64_t M, const int C) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   extern __shared__ __align__(16) unsigned char smem_raw[];
   chan_body(op, M, C, reinterpret_cast<float*>(smem_raw + chan_ring_bytes<Op>()), smem_u32(smem_raw));
 }
@@ -217,7 +215,7 @@ int launch_chan(const Op& op, int64_t M, int C, cudaStream_t st, const char* wha
   int64_t cap = (int64_t)sgb_sm_count() * per_sm;
   if (cap > sgb_chan_grid_cap()) cap = sgb_chan_grid_cap();
   const int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
-  SGB_LAUNCH(chan_kernel<Op>, grid, TPB, smem, st, op, M, C);
+  chan_kernel<Op><<<grid, TPB, smem, st>>>(op, M, C);
   return sgb_cuda_check(cudaGetLastError(), what);
 }
 

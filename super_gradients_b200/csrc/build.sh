@@ -4,14 +4,9 @@ set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 ROOT="$(cd "$HERE/../.." && pwd)"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-OUT="${SGB_OUT:-$HERE/../libsgb200.so}"   # SGB_OUT / SGB_OBJ: build a variant (e.g. without -DSGB_DETERMINISTIC_STATS) next to the default library
-OBJ="${SGB_OBJ:-$HERE/obj}"
-# Default feature set:
-#   SGB_DETERMINISTIC_STATS  per-warp BatchNorm-statistics slots of the mma.sync kernels summed in a fixed order: removes the
-#                            run-to-run last-bit differences of interleaved models (DESIGN.md section 8.1)
-# -DSGB_PDL (programmatic dependent launch) is an experiment and stays off.
-DEFS=(${SGB_DEFS:--DSGB_DETERMINISTIC_STATS})
-FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I"$ROOT/include" -I"$HERE" --expt-relaxed-constexpr "${DEFS[@]}")
+OUT="$HERE/../libsgb200.so"
+OBJ="$HERE/obj"
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I"$ROOT/include" -I"$HERE" --expt-relaxed-constexpr)
 mkdir -p "$OBJ"
 pids=()
 for f in "$HERE"/*.cu; do

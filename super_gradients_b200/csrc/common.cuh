@@ -78,47 +78,5 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-// CTA cap of the streaming per-channel kernels: 132 SMs x SGB_CHAN_CTAS_PER_SM (default 6; the environment variable is a tuning hook)
-static inline int sgb_chan_grid_cap() {
-  static int cap = 0;
-  if (cap == 0) {
-    const char* e = getenv("SGB_CHAN_CTAS_PER_SM");
-    const int per_sm = (e && atoi(e) > 0) ? atoi(e) : 6;
-    cap = 132 * per_sm;
-  }
-  return cap;
-}
-
-// Programmatic dependent launch (experiment, -DSGB_PDL; the default build compiles these to nothing and launches with <<<>>>).
-// A kernel first tells the runtime that its dependents may be scheduled (SGB_GRID_DEP_LAUNCH), does whatever does not touch
-// global memory (barrier init, TMEM allocation, shared-memory clears), then SGB_GRID_DEP_WAIT blocks until every prerequisite
-// grid has completed and its writes are visible.  The launch side marks the kernel as programmatically serialised, so its CTAs
-// may become resident while the previous kernel drains; stream capture turns that into programmatic graph edges.
-#ifdef SGB_PDL
-#define SGB_GRID_DEP_LAUNCH() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
-#define SGB_GRID_DEP_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
-template <class... KArgs, class... Args>
-static inline void sgb_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  static int enabled = -1;  // SGB_PDL=0 in the environment launches the same build with plain stream serialisation (A/B in one library)
-  if (enabled < 0) {
-    const char* e = getenv("SGB_PDL");
-    enabled = (e && e[0] == '0') ? 0 : 1;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = enabled ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);  // a failure surfaces through cudaGetLastError() at the call site
-}
-#define SGB_LAUNCH(kernel, grid, block, smem, st, ...) sgb_launch_pdl(kernel, dim3(grid), dim3(block), smem, st, __VA_ARGS__)
-#else
-#define SGB_GRID_DEP_LAUNCH() ((void)0)
-#define SGB_GRID_DEP_WAIT() ((void)0)
-#define SGB_LAUNCH(kernel, grid, block, smem, st, ...) kernel<<<grid, block, smem, st>>>(__VA_ARGS__)
-#endif
+// CTA cap of the streaming per-channel kernels: 132 SMs x 6 CTAs
+static inline int sgb_chan_grid_cap() { return 132 * 6; }

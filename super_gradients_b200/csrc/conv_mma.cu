@@ -179,14 +179,10 @@ __global__ void __launch_bounds__(THREADS) igemm_conv_kernel(const __grid_consta
   __syncthreads();
 
   // ---- epilogue
-  float* sstat = reinterpret_cast<float*>(smem_raw);  // [2][BN]
+  float* sstat = reinterpret_cast<float*>(smem_raw);  // [WARPS_M][2][BN]
   const bool do_stats = p.stats != nullptr;
   if (do_stats) {
-#ifdef SGB_DETERMINISTIC_STATS  // one slot per warp row (sm100_host.h explains the experiment)
-    for (int i = tid; i < WARPS_M * 2 * BN; i += THREADS) sstat[i] = 0.f;
-#else
-    for (int i = tid; i < 2 * BN; i += THREADS) sstat[i] = 0.f;
-#endif
+    for (int i = tid; i < WARPS_M * 2 * BN; i += THREADS) sstat[i] = 0.f;  // one slot per warp row
     __syncthreads();
   }
   float cs1[NT][2], cs2[NT][2];
@@ -260,13 +256,8 @@ __global__ void __launch_bounds__(THREADS) igemm_conv_kernel(const __grid_consta
         }
         if (lane < 4) {
           int c = wn * WTN + nt * 8 + 2 * lane + e;
-#ifdef SGB_DETERMINISTIC_STATS
           sstat[wm * 2 * BN + c] = a;  // (wm, column) is owned by exactly one lane of one warp
           sstat[wm * 2 * BN + BN + c] = b;
-#else
-          atomicAdd(&sstat[c], a);
-          atomicAdd(&sstat[BN + c], b);
-#endif
         }
       }
     __syncthreads();
@@ -275,7 +266,6 @@ __global__ void __launch_bounds__(THREADS) igemm_conv_kernel(const __grid_consta
     for (int c = tid; c < BN; c += THREADS) {
       int col = n0 + c;
       if (col < p.Ngemm) {
-#ifdef SGB_DETERMINISTIC_STATS
         float v1 = sstat[c], v2 = sstat[BN + c];
 #pragma unroll
         for (int q = 1; q < WARPS_M; ++q) {  // fixed order
@@ -284,10 +274,6 @@ __global__ void __launch_bounds__(THREADS) igemm_conv_kernel(const __grid_consta
         }
         atomicAdd(&st[col], (double)v1);
         atomicAdd(&st[p.Ngemm + col], (double)v2);
-#else
-        atomicAdd(&st[col], (double)sstat[c]);
-        atomicAdd(&st[p.Ngemm + col], (double)sstat[BN + c]);
-#endif
       }
     }
   }
@@ -509,7 +495,7 @@ extern "C" int sgb_conv_fprop(const SgbConvDesc* d, const sgb_bf16* x, const sgb
     // patches do not overlap, so the tensor viewed as an image [N * H/2][2][W/2][2C] -- row pair, row parity, column pair, (column
     // parity, channel) -- turns the layer into a 2-tap (rows 0 and 1), stride-1 valid convolution with 2C channels per tap whose
     // B columns are the filter's own (dh, dw, c) order: the im2col tcgen05 kernel serves it through its explicit tap table.
-    if (sm100::enabled() && d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
+    if (d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
         d->W % 2 == 0 && d->P == d->H / 2 && d->Q == d->W / 2 && (2 * d->C) % 16 == 0 && d->K % 8 == 0 && d->y_pitch % 8 == 0 && d->y_off % 8 == 0 &&
         (long long)d->N * (d->H / 2) < (1ll << 31)) {
       q.N = d->N * (d->H / 2); q.H = 2; q.W = d->W / 2; q.C = 2 * d->C; q.a_pitch = 2 * d->C;
@@ -576,7 +562,7 @@ extern "C" int sgb_convt2x2_fprop(const SgbConvDesc* d, const sgb_bf16* x_small,
   if (int rc = check_desc(d)) return rc;
   SGB_REQUIRE(d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0, "convt2x2 needs R=S=2, stride 2, pad 0");
   SGB_REQUIRE(d->K % 8 == 0 && d->y_pitch % 8 == 0 && d->y_off % 8 == 0, "small-side channels must be multiples of 8");
-  if (d->K % 16 == 0 && d->C % 16 == 0 && sm100::enabled()) {
+  if (d->K % 16 == 0 && d->C % 16 == 0) {
     // tcgen05 path: the transposed convolution is four 1x1 GEMMs, one per output parity (dh, dw), each writing the output pixels
     // (2h + dh, 2w + dw) through the strided-row epilogue the stride-2 input gradients use.  w_up rows are ordered (dh, dw, co).
     bool all_ok = true;
@@ -649,7 +635,7 @@ extern "C" int sgb_conv_dgrad(const SgbConvDesc* d, const sgb_bf16* dy, const sg
     if (sm100::supported(q)) return sm100::launch(q, (cudaStream_t)stream);
   }
   if (s == 2 && d->K % 16 == 0 && d->R == 3 && d->S == 3 && d->pad == 1 && d->C % 8 == 0 && d->H % 2 == 0 &&
-      d->W % 2 == 0 && d->H == 2 * d->P && d->W == 2 * d->Q && sm100::enabled()) {
+      d->W % 2 == 0 && d->H == 2 * d->P && d->W == 2 * d->Q) {
     // stride-2 dgrad = 4 output-parity classes, each an exact stride-1 gather of dy with a subset of the taps
     bool all_ok = true;
     for (int cls = 0; cls < 4 && all_ok; ++cls) {
@@ -681,7 +667,7 @@ extern "C" int sgb_conv_dgrad(const SgbConvDesc* d, const sgb_bf16* dy, const sg
     if (all_ok) return SGB_OK;
   }
   if (s == 2 && d->K % 16 == 0 && d->R == 1 && d->S == 1 && d->pad == 0 && d->C % 8 == 0 && d->H == 2 * d->P &&
-      d->W == 2 * d->Q && sm100::enabled()) {
+      d->W == 2 * d->Q) {
     // 1x1 stride-2 dgrad: only the even/even input pixels receive a gradient.  With accumulate the other three parity
     // classes are untouched; otherwise they are zero-filled first.
     sm100::Problem q{};
@@ -764,7 +750,7 @@ extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb
     if (sm100::wgrad_supported(q)) return sm100::wgrad_launch(q, (cudaStream_t)stream);
     // 2 x 2 / stride 2 / no padding over a dense x: the same re-description as in sgb_conv_fprop -- a (2 x 1)-tap stride-1 valid
     // convolution over the image [N * H/2][2][W/2][2C]; dW rows [K][dh][(dw, c)] are the KRSC rows of the 2 x 2 filter.
-    if (sm100::enabled() && d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
+    if (d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
         d->W % 2 == 0 && d->P == d->H / 2 && d->Q == d->W / 2 && (2 * d->C) % 16 == 0 && d->K % 8 == 0 && (long long)d->N * (d->H / 2) < (1ll << 31)) {
       q.N = d->N * (d->H / 2); q.H = 2; q.W = d->W / 2; q.C = 2 * d->C; q.x_pitch = 2 * d->C;
       q.R = 2; q.S = 1; q.stride = 1; q.pad = 0; q.P = 1; q.Q = d->W / 2;

@@ -201,7 +201,6 @@ __device__ __forceinline__ void flush_stats(const Params& p, const float* s_stat
 template <int BN, bool SKIP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
-  SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = BN * p.KC * 2;
@@ -228,7 +227,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   if (p.stats)
     for (int i = threadIdx.x; i < 2 * p.N; i += NUM_THREADS) s_stats[i] = 0.f;
   __syncthreads();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (warp == 0) {
     // ===================================================================================== TMA producer
@@ -343,7 +341,6 @@ constexpr int HALO_MAX_STAGES = 6;
 template <int BN, bool SKIP>
 __global__ void __launch_bounds__(NUM_THREADS, BN <= 48 ? 2 : 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
-  SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int ksteps = p.C / 16;
@@ -378,7 +375,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   if (p.stats)
     for (int i = threadIdx.x; i < 4 * p.N; i += NUM_THREADS) s_stats[i] = 0.f;
   __syncthreads();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (warp == 0) {
     // ===================================================================================== TMA producer
@@ -494,7 +490,6 @@ __host__ __device__ __forceinline__ int wgrad_row_blocks(const WParams& p, int t
 template <int NB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WParams p) {
-  SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_bytes = 2 * WPIX * 128;                       // two 64-channel blocks of dy
@@ -531,7 +526,6 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (n_iters > 0) {
     if (warp == 0) {
@@ -700,7 +694,6 @@ __device__ __forceinline__ void wgrad_halo_consume(const WParams& p, uint32_t ri
 template <int NB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 wgrad3x3_halo_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WParams p) {
-  SGB_GRID_DEP_LAUNCH();
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t a_bytes = WH_A_BYTES, stage_bytes = wgrad_halo_stage_bytes(NB);
@@ -725,7 +718,6 @@ wgrad3x3_halo_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_co
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  SGB_GRID_DEP_WAIT();  // everything above touches only shared memory
 
   if (warp == 0) {
     // ===================================================================================== TMA producer
@@ -805,17 +797,7 @@ CUtensorMapSwizzle swizzle_for(int kc) {
   return kc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (kc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-bool enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SGB_DISABLE_SM100");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 bool supported(const Problem& q) {
-  if (!enabled()) return false;
   if (q.C % 16 != 0 || q.b_rows % 8 != 0) return false;
   if (!((q.R == 1 && q.S == 1) || (q.R == 3 && q.S == 3))) return false;
   if (q.stride != 1 && q.stride != 2) return false;
@@ -975,7 +957,7 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   int per_nt = g_num_sms * ctas_per_sm / p.n_tiles;
   if (per_nt > p.M) per_nt = p.M;
   if (per_nt < 1) per_nt = 1;
-  SGB_LAUNCH(var->fn, per_nt * p.n_tiles, NUM_THREADS, smem, st, map_a, map_b, p);
+  var->fn<<<per_nt * p.n_tiles, NUM_THREADS, smem, st>>>(map_a, map_b, p);
   ++g_launches;
   ++g_halo_launches;
   return sgb_cuda_check(cudaGetLastError(), "conv3x3_halo_kernel");
@@ -1084,13 +1066,12 @@ int launch(const Problem& q, cudaStream_t st) {
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   int grid = m_tiles * p.n_tiles;
   if (grid > g_num_sms * ctas_per_sm) grid = g_num_sms * ctas_per_sm;
-  SGB_LAUNCH(var->fn, grid, NUM_THREADS, smem, st, map_a, map_b, p);
+  var->fn<<<grid, NUM_THREADS, smem, st>>>(map_a, map_b, p);
   ++g_launches;
   return sgb_cuda_check(cudaGetLastError(), "conv_wgmma_kernel");
 }
 
 bool wgrad_supported(const WgradProblem& q) {
-  if (!enabled()) return false;
   if (q.C % 16 != 0 || q.K % 8 != 0) return false;
   if (!((q.R == 1 && q.S == 1) || (q.R == 3 && q.S == 3))) return false;
   if (q.pad != q.R / 2 || (q.stride != 1 && q.stride != 2)) return false;
@@ -1151,7 +1132,7 @@ int launch_wgrad_halo(const WgradProblem& q, const WParams& p0, int nb, cudaStre
     }
   }
   if (int rc = encode_halo_map(&map_x, q.x, q.N, q.H, q.W, q.C, q.x_pitch)) return rc;
-  SGB_LAUNCH(var->fn, splits * items, NUM_THREADS, smem, st, map_dy, map_x, p);
+  var->fn<<<splits * items, NUM_THREADS, smem, st>>>(map_dy, map_x, p);
   ++g_launches;
   ++g_wgrad_halo_launches;
   return sgb_cuda_check(cudaGetLastError(), "wgrad3x3_halo_kernel");
@@ -1230,7 +1211,7 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
     if (r != CUDA_SUCCESS) { sgb_set_error("cuTensorMapEncodeIm2col(x, wgrad) failed with %d", (int)r); return SGB_E_CUDA; }
   }
   const int grid = base_ctas * splits;
-  SGB_LAUNCH(var->fn, grid, NUM_THREADS, smem, st, map_dy, map_x, p);
+  var->fn<<<grid, NUM_THREADS, smem, st>>>(map_dy, map_x, p);
   ++g_launches;
   return sgb_cuda_check(cudaGetLastError(), "wgrad_wgmma_kernel");
 }

@@ -39,7 +39,6 @@ struct WgradProblem {
   int centre_from; // 0, or (3x3 only) rows from here on need only their centre tap: their off-centre dw entries are not written
 };
 
-bool enabled();
 bool wgrad_supported(const WgradProblem& q);
 int wgrad_launch(const WgradProblem& q, cudaStream_t st);
 bool supported(const Problem& q);

@@ -222,8 +222,6 @@ __device__ __forceinline__ void batch_walk(const Item* __restrict__ items, int n
 }
 
 __global__ void __launch_bounds__(TPB) weight_prepare_batch_kernel(const SgbWeightItem* __restrict__ items, int n, int64_t total) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   // every filter's index space has an even number of elements starting at an even offset: the walk runs over PAIRS (half the index
   // arithmetic, 32-bit stores)
   batch_walk<2>(items, n, total, [](const SgbWeightItem& it, int64_t local) {
@@ -233,14 +231,10 @@ __global__ void __launch_bounds__(TPB) weight_prepare_batch_kernel(const SgbWeig
 }
 
 __global__ void __launch_bounds__(TPB) wgrad_to_oihw_batch_kernel(const SgbWgradItem* __restrict__ items, int n, int64_t total) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   batch_walk(items, n, total, [](const SgbWgradItem& it, int64_t local) { wgrad_to_oihw_elem(it.dw, it.C, it.R, it.S, it.c_pad, it.g, it.accumulate, local); });
 }
 
 __global__ void __launch_bounds__(256) qarep_alpha_finish_kernel(const SgbAlphaItem* __restrict__ items) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const SgbAlphaItem it = items[blockIdx.x];
   const float alpha = *it.alpha;
   float acc = 0.f;
@@ -270,8 +264,6 @@ __global__ void __launch_bounds__(256) qarep_alpha_finish_kernel(const SgbAlphaI
 
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, int N, int C, int H, int W, bf16* y, int pitch,
                                     int off, int cpad) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   // one thread per (n, h, w, cvec) writes 8 channels; reads are strided by H*W but coalesced across w.
   const int64_t hw = (int64_t)H * W;
   const int cv = cpad / 8;
@@ -298,8 +290,6 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, int N, int C, i
 constexpr int STEM_QT = 128;
 __global__ void __launch_bounds__(256) stem_patches_kernel(const float* __restrict__ x, int N, int C, int H, int W, int R, int stride, int pad,
                                                            bf16* __restrict__ y, int P, int Q, int cout) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   extern __shared__ float srow[];  // [C][R][span]
   const int qtiles = (Q + STEM_QT - 1) / STEM_QT;
   const int qt = blockIdx.x % qtiles;
@@ -346,8 +336,6 @@ __global__ void __launch_bounds__(256) stem_patches_kernel(const float* __restri
 // assembles whole 64-byte pixels (4 vectors) from shared memory.  The generic kernel above spent its time in div / mod chains
 // (480 us for 32 x 3 x 640 x 640; the data is 157 MB in + 210 MB out = 56 us at the HBM peak).
 __global__ void __launch_bounds__(256) stem_patches_c3r3s2_kernel(const float* __restrict__ x, int H, int W, bf16* __restrict__ y, int P, int Q) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   extern __shared__ float srow[];  // [9 = (c, r)][span], span = 2 * Q + 1 (input columns -1 .. 2Q - 1)
   const int p = blockIdx.x % P, n = blockIdx.x / P;
   const int span = 2 * Q + 1;
@@ -386,8 +374,6 @@ __global__ void __launch_bounds__(256) stem_patches_c3r3s2_kernel(const float* _
 
 __global__ void nhwc_to_nchw_kernel(const bf16* __restrict__ x, int N, int C, int H, int W, int pitch, int off,
                                     float* y) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const int64_t hw = (int64_t)H * W;
   const int64_t total = (int64_t)N * C * hw;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -413,8 +399,6 @@ constexpr int red_depth() {
 }
 template <class F>
 __global__ void __launch_bounds__(TPB) chan_reduce_kernel(F f, int64_t M, int C, double* out, int out_stride) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   constexpr int NACC = F::NACC, NIN = F::NIN, D = red_depth<F>();
   extern __shared__ __align__(16) unsigned char smem_red[];
   float* sred = reinterpret_cast<float*>(smem_red + sgb_ring::bytes<NIN, red_unroll<F>(), D, TPB>());  // [TPB][NACC*8]
@@ -488,7 +472,7 @@ int launch_chan_reduce(F f, int64_t M, int C, double* out, int out_stride, cudaS
   if (cap > sgb_chan_grid_cap()) cap = sgb_chan_grid_cap();
   int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
   (void)cvb;
-  SGB_LAUNCH(chan_reduce_kernel<F>, grid, TPB, smem, st, f, M, C, out, out_stride);
+  chan_reduce_kernel<F><<<grid, TPB, smem, st>>>(f, M, C, out, out_stride);
   SGB_LAUNCH_CHECK("chan_reduce_kernel");
   return SGB_OK;
 }
@@ -533,8 +517,6 @@ struct QarepMomF {
 // ---------------------------------------------------------------------------------------------- pooling etc.
 __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, int N, int H, int W, int C, int xp, int xo, int k,
                                    int stride, int pad, bf16* y, int P, int Q, int yp, int yo, uint8_t* idx) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const int cvs = C / 8;
   const int64_t total = (int64_t)N * P * Q * cvs;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -580,8 +562,6 @@ __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, int N, int H, int
 // 2k instead of k^2 comparisons per output and with the plane read from HBM once (the direct kernel ran at 73 GB/s).
 __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __restrict__ x, int H, int W, int C, int xp, int xo, int k, int pad, bf16* y,
                                                               int P, int Q, int yp, int yo, uint8_t* idx) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   extern __shared__ __align__(16) unsigned char smem_mp[];
   uint4* plane = reinterpret_cast<uint4*>(smem_mp);                     // [H][W] 8 x bf16
   float* rmax = reinterpret_cast<float*>(plane + (size_t)H * W);        // [H][Q][8]
@@ -645,8 +625,6 @@ __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __rest
 
 __global__ void maxpool_bwd_kernel(const bf16* __restrict__ dy, int N, int H, int W, int C, int k, int stride, int pad,
                                    int P, int Q, int dyp, int dyo, const uint8_t* idx, float* dx) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const int64_t total = (int64_t)N * P * Q * C;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     int c = i % C;
@@ -668,8 +646,6 @@ __global__ void maxpool_bwd_kernel(const bf16* __restrict__ dy, int N, int H, in
 // tensor, fp32 atomics and a conversion pass afterwards (0.75 ms of a ResNet-50 step at batch 256: 822 MB memset + 416 us + copy).
 __global__ void __launch_bounds__(256) maxpool_bwd_gather_kernel(const bf16* __restrict__ dy, int N, int H, int W, int C, int k, int stride, int pad, int P,
                                                                  int Q, int dyp, int dyo, const uint8_t* __restrict__ idx, bf16* __restrict__ dx, int dxp) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const int cvs = C / 8;
   const int64_t total = (int64_t)N * H * W * cvs;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -712,8 +688,6 @@ __global__ void __launch_bounds__(256) maxpool_bwd_gather_kernel(const bf16* __r
 
 __global__ void axpby_kernel(const bf16* __restrict__ x1, int p1, int o1, float a, const bf16* __restrict__ x2, int p2,
                              int o2, float b, bf16* y, int py, int oy, int64_t M, int C) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const int cvs = C / 8;
   const int64_t total = M * cvs;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -734,8 +708,6 @@ __global__ void axpby_kernel(const bf16* __restrict__ x1, int p1, int o1, float 
 
 __global__ void scale_add_kernel(const bf16* __restrict__ x1, int p1, int o1, const float* a_dev,
                                  const bf16* __restrict__ x2, int p2, int o2, bf16* y, int py, int oy, int64_t M, int C) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const float a = *a_dev;
   const int cvs = C / 8;
   const int64_t total = M * cvs;
@@ -828,8 +800,6 @@ __global__ void avgpool_bwd_kernel(const bf16* __restrict__ dy, int N, int HW, i
 // sgd   hp: [lr, momentum, weight_decay, grad_scale, nesterov]
 // adamw hp: [lr, beta1, beta2, eps, weight_decay, 1-beta1^t, 1-beta2^t, grad_scale]
 __global__ void sgd_kernel(float* p, const float* g, float* mom, int64_t n, const float* hp) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const float lr = hp[0], mu = hp[1], wd = hp[2], gs = hp[3];
   const bool nesterov = hp[4] != 0.f;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -844,8 +814,6 @@ __global__ void sgd_kernel(float* p, const float* g, float* mom, int64_t n, cons
   }
 }
 __global__ void adamw_kernel(float* p, const float* g, float* m, float* v, int64_t n, const float* hp) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4], bc1 = hp[5], bc2 = hp[6], gs = hp[7];
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     float gr = g[i] * gs;
@@ -859,8 +827,6 @@ __global__ void adamw_kernel(float* p, const float* g, float* m, float* v, int64
   }
 }
 __global__ void ema_kernel(float* e, const float* p, int64_t n, const float* decay) {
-  SGB_GRID_DEP_LAUNCH();
-  SGB_GRID_DEP_WAIT();
   const float d = *decay;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     e[i] = e[i] * d + (1.f - d) * p[i];
@@ -892,21 +858,21 @@ extern "C" int sgb_wgrad_to_oihw(const float* dw, int K, int C, int R, int S, in
 
 extern "C" int sgb_weight_prepare_batch(const SgbWeightItem* items_dev, int n_items, int64_t total, void* stream) {
   SGB_REQUIRE(items_dev && n_items > 0 && total > 0, "bad args");
-  SGB_LAUNCH(weight_prepare_batch_kernel, grid_for(total, BATCH_CHUNK), TPB, 0, (cudaStream_t)stream, items_dev, n_items, total);
+  weight_prepare_batch_kernel<<<grid_for(total, BATCH_CHUNK), TPB, 0, (cudaStream_t)stream>>>(items_dev, n_items, total);
   SGB_LAUNCH_CHECK("weight_prepare_batch_kernel");
   return SGB_OK;
 }
 
 extern "C" int sgb_wgrad_to_oihw_batch(const SgbWgradItem* items_dev, int n_items, int64_t total, void* stream) {
   SGB_REQUIRE(items_dev && n_items > 0 && total > 0, "bad args");
-  SGB_LAUNCH(wgrad_to_oihw_batch_kernel, grid_for(total, BATCH_CHUNK), TPB, 0, (cudaStream_t)stream, items_dev, n_items, total);
+  wgrad_to_oihw_batch_kernel<<<grid_for(total, BATCH_CHUNK), TPB, 0, (cudaStream_t)stream>>>(items_dev, n_items, total);
   SGB_LAUNCH_CHECK("wgrad_to_oihw_batch_kernel");
   return SGB_OK;
 }
 
 extern "C" int sgb_qarep_alpha_finish_batch(const SgbAlphaItem* items_dev, int n_items, void* stream) {
   SGB_REQUIRE(items_dev && n_items > 0, "bad args");
-  SGB_LAUNCH(qarep_alpha_finish_kernel, n_items, 256, 0, (cudaStream_t)stream, items_dev);
+  qarep_alpha_finish_kernel<<<n_items, 256, 0, (cudaStream_t)stream>>>(items_dev);
   SGB_LAUNCH_CHECK("qarep_alpha_finish_kernel");
   return SGB_OK;
 }
@@ -918,7 +884,7 @@ extern "C" int sgb_nchw_f32_to_nhwc_bf16(const float* x, int N, int C, int H, in
   SGB_REQUIRE(c_out >= C && c_out % 8 == 0, "c_out must be >= C and a multiple of 8");
   int cpad = c_out;  // channels [C, c_out) are written as zeros
   SGB_REQUIRE(y_pitch >= y_off + cpad, "slice exceeds pitch");
-  SGB_LAUNCH(nchw_to_nhwc_kernel, grid_for((int64_t)N * H * W * (cpad / 8)), TPB, 0, (cudaStream_t)stream,  x, N, C, H, W, (bf16*)y, y_pitch, y_off, cpad);
+  nchw_to_nhwc_kernel<<<grid_for((int64_t)N * H * W * (cpad / 8)), TPB, 0, (cudaStream_t)stream>>>(x, N, C, H, W, (bf16*)y, y_pitch, y_off, cpad);
   SGB_LAUNCH_CHECK("nchw_to_nhwc_kernel");
   return SGB_OK;
 }
@@ -929,7 +895,7 @@ extern "C" int sgb_stem_patches_f32(const float* x, int N, int C, int H, int W, 
   SGB_REQUIRE(c_out % 8 == 0 && c_out >= C * R * R, "c_out must be a multiple of 8 and hold C * R * R patch entries");
   SGB_REQUIRE(P == (H + 2 * pad - R) / stride + 1 && Q == (W + 2 * pad - R) / stride + 1, "P/Q inconsistent");
   if (C == 3 && R == 3 && stride == 2 && pad == 1 && c_out == 32 && H % 2 == 0 && W % 2 == 0 && (size_t)9 * (2 * Q + 1) * sizeof(float) <= 48 * 1024) {
-    SGB_LAUNCH(stem_patches_c3r3s2_kernel, N * P, 256, (size_t)9 * (2 * Q + 1) * sizeof(float), (cudaStream_t)stream, x, H, W, (bf16*)y, P, Q);
+    stem_patches_c3r3s2_kernel<<<N * P, 256, (size_t)9 * (2 * Q + 1) * sizeof(float), (cudaStream_t)stream>>>(x, H, W, (bf16*)y, P, Q);
     SGB_LAUNCH_CHECK("stem_patches_c3r3s2_kernel");
     return SGB_OK;
   }
@@ -937,7 +903,7 @@ extern "C" int sgb_stem_patches_f32(const float* x, int N, int C, int H, int W, 
   SGB_REQUIRE(smem <= 48 * 1024, "patch rows do not fit shared memory");
   const int64_t ctas = (int64_t)N * P * ((Q + STEM_QT - 1) / STEM_QT);
   SGB_REQUIRE(ctas < (1ll << 31), "too many tiles");
-  SGB_LAUNCH(stem_patches_kernel, (int)ctas, 256, smem, (cudaStream_t)stream, x, N, C, H, W, R, stride, pad, (bf16*)y, P, Q, c_out);
+  stem_patches_kernel<<<(int)ctas, 256, smem, (cudaStream_t)stream>>>(x, N, C, H, W, R, stride, pad, (bf16*)y, P, Q, c_out);
   SGB_LAUNCH_CHECK("stem_patches_kernel");
   return SGB_OK;
 }
@@ -945,7 +911,7 @@ extern "C" int sgb_stem_patches_f32(const float* x, int N, int C, int H, int W, 
 extern "C" int sgb_nhwc_bf16_to_nchw_f32(const sgb_bf16* x, int N, int C, int H, int W, int x_pitch, int x_off,
                                          float* y, void* stream) {
   SGB_REQUIRE(x && y, "null pointer");
-  SGB_LAUNCH(nhwc_to_nchw_kernel, grid_for((int64_t)N * C * H * W), TPB, 0, (cudaStream_t)stream, (const bf16*)x, N, C, H, W, x_pitch, x_off, y);
+  nhwc_to_nchw_kernel<<<grid_for((int64_t)N * C * H * W), TPB, 0, (cudaStream_t)stream>>>((const bf16*)x, N, C, H, W, x_pitch, x_off, y);
   SGB_LAUNCH_CHECK("nhwc_to_nchw_kernel");
   return SGB_OK;
 }
@@ -979,11 +945,11 @@ extern "C" int sgb_maxpool_fwd(const sgb_bf16* x, int N, int H, int W, int C, in
       cudaFuncSetAttribute(maxpool_s1_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
       attr = true;
     }
-    SGB_LAUNCH(maxpool_s1_smem_kernel, N * (C / 8), 256, smem, (cudaStream_t)stream, (const bf16*)x, H, W, C, x_pitch, x_off, k, pad, (bf16*)y, P, Q, y_pitch, y_off, idx);
+    maxpool_s1_smem_kernel<<<N * (C / 8), 256, smem, (cudaStream_t)stream>>>((const bf16*)x, H, W, C, x_pitch, x_off, k, pad, (bf16*)y, P, Q, y_pitch, y_off, idx);
     SGB_LAUNCH_CHECK("maxpool_s1_smem_kernel");
     return SGB_OK;
   }
-  SGB_LAUNCH(maxpool_fwd_kernel, grid_for((int64_t)N * P * Q * (C / 8)), TPB, 0, (cudaStream_t)stream,  (const bf16*)x, N, H, W, C, x_pitch, x_off, k, stride, pad, (bf16*)y, P, Q, y_pitch, y_off, idx);
+  maxpool_fwd_kernel<<<grid_for((int64_t)N * P * Q * (C / 8)), TPB, 0, (cudaStream_t)stream>>>((const bf16*)x, N, H, W, C, x_pitch, x_off, k, stride, pad, (bf16*)y, P, Q, y_pitch, y_off, idx);
   SGB_LAUNCH_CHECK("maxpool_fwd_kernel");
   return SGB_OK;
 }
@@ -991,7 +957,7 @@ extern "C" int sgb_maxpool_fwd(const sgb_bf16* x, int N, int H, int W, int C, in
 extern "C" int sgb_maxpool_bwd(const sgb_bf16* dy, int N, int H, int W, int C, int k, int stride, int pad, int P,
                                int Q, int dy_pitch, int dy_off, const uint8_t* idx, float* dx_f32, void* stream) {
   SGB_REQUIRE(dy && idx && dx_f32, "null pointer");
-  SGB_LAUNCH(maxpool_bwd_kernel, grid_for((int64_t)N * P * Q * C), TPB, 0, (cudaStream_t)stream,  (const bf16*)dy, N, H, W, C, k, stride, pad, P, Q, dy_pitch, dy_off, idx, dx_f32);
+  maxpool_bwd_kernel<<<grid_for((int64_t)N * P * Q * C), TPB, 0, (cudaStream_t)stream>>>((const bf16*)dy, N, H, W, C, k, stride, pad, P, Q, dy_pitch, dy_off, idx, dx_f32);
   SGB_LAUNCH_CHECK("maxpool_bwd_kernel");
   return SGB_OK;
 }
@@ -1002,7 +968,7 @@ extern "C" int sgb_maxpool_bwd_bf16(const sgb_bf16* dy, int N, int H, int W, int
   SGB_REQUIRE(C % 8 == 0 && dy_pitch % 8 == 0 && dy_off % 8 == 0 && dx_pitch % 8 == 0 && dx_pitch >= C, "channels / pitches must be multiples of 8");
   SGB_REQUIRE(stride >= 1 && k >= 1 && k * k <= 255, "bad window");
   SGB_REQUIRE((int64_t)N * H * W * (C / 8) < (1ll << 32) && (int64_t)N * H * W < (1ll << 31), "tensor too large for the 32-bit index math");
-  SGB_LAUNCH(maxpool_bwd_gather_kernel, grid_for((int64_t)N * H * W * (C / 8), TPB * 2), 256, 0, (cudaStream_t)stream, (const bf16*)dy, N, H, W, C, k, stride, pad,
+  maxpool_bwd_gather_kernel<<<grid_for((int64_t)N * H * W * (C / 8), TPB * 2), 256, 0, (cudaStream_t)stream>>>((const bf16*)dy, N, H, W, C, k, stride, pad,
              P, Q, dy_pitch, dy_off, idx, (bf16*)dx, dx_pitch);
   SGB_LAUNCH_CHECK("maxpool_bwd_gather_kernel");
   return SGB_OK;
@@ -1012,7 +978,7 @@ extern "C" int sgb_axpby(const sgb_bf16* x1, int p1, int o1, float a, const sgb_
                          sgb_bf16* y, int py, int oy, int64_t M, int C, void* stream) {
   SGB_REQUIRE(x1 && y && C % 8 == 0 && p1 % 8 == 0 && o1 % 8 == 0 && py % 8 == 0 && oy % 8 == 0, "bad args");
   SGB_REQUIRE(!x2 || (p2 % 8 == 0 && o2 % 8 == 0), "bad args (x2)");
-  SGB_LAUNCH(axpby_kernel, grid_for(M * (C / 8), TPB * 4), TPB, 0, (cudaStream_t)stream,  (const bf16*)x1, p1, o1, a, (const bf16*)x2, p2, o2, b, (bf16*)y, py, oy, M, C);
+  axpby_kernel<<<grid_for(M * (C / 8), TPB * 4), TPB, 0, (cudaStream_t)stream>>>((const bf16*)x1, p1, o1, a, (const bf16*)x2, p2, o2, b, (bf16*)y, py, oy, M, C);
   SGB_LAUNCH_CHECK("axpby_kernel");
   return SGB_OK;
 }
@@ -1021,7 +987,7 @@ extern "C" int sgb_scale_add(const sgb_bf16* x1, int p1, int o1, const float* a_
                              sgb_bf16* y, int py, int oy, int64_t M, int C, void* stream) {
   SGB_REQUIRE(x1 && y && a_dev && C % 8 == 0 && p1 % 8 == 0 && o1 % 8 == 0 && py % 8 == 0 && oy % 8 == 0, "bad args");
   SGB_REQUIRE(!x2 || (p2 % 8 == 0 && o2 % 8 == 0), "bad args (x2)");
-  SGB_LAUNCH(scale_add_kernel, grid_for(M * (C / 8), TPB * 4), TPB, 0, (cudaStream_t)stream,  (const bf16*)x1, p1, o1, a_dev, (const bf16*)x2, p2, o2, (bf16*)y, py, oy, M, C);
+  scale_add_kernel<<<grid_for(M * (C / 8), TPB * 4), TPB, 0, (cudaStream_t)stream>>>((const bf16*)x1, p1, o1, a_dev, (const bf16*)x2, p2, o2, (bf16*)y, py, oy, M, C);
   SGB_LAUNCH_CHECK("scale_add_kernel");
   return SGB_OK;
 }
@@ -1065,19 +1031,19 @@ extern "C" int sgb_avgpool_bwd(const sgb_bf16* dy, int N, int HW, int C, sgb_bf1
 
 extern "C" int sgb_sgd_step(float* p, const float* g, float* mom, int64_t n, const float* hp, void* stream) {
   SGB_REQUIRE(p && g && mom && hp, "null pointer");
-  SGB_LAUNCH(sgd_kernel, grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream, p, g, mom, n, hp);
+  sgd_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, mom, n, hp);
   SGB_LAUNCH_CHECK("sgd_kernel");
   return SGB_OK;
 }
 extern "C" int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream) {
   SGB_REQUIRE(p && g && m && v && hp, "null pointer");
-  SGB_LAUNCH(adamw_kernel, grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream, p, g, m, v, n, hp);
+  adamw_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, m, v, n, hp);
   SGB_LAUNCH_CHECK("adamw_kernel");
   return SGB_OK;
 }
 extern "C" int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream) {
   SGB_REQUIRE(ema && p && decay, "null pointer");
-  SGB_LAUNCH(ema_kernel, grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream, ema, p, n, decay);
+  ema_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(ema, p, n, decay);
   SGB_LAUNCH_CHECK("ema_kernel");
   return SGB_OK;
 }

@@ -576,14 +576,9 @@ __global__ void __launch_bounds__(NT, 1) nms_kernel(SgbNmsDesc d, const float* _
 
 }  // namespace
 
-// multi-label rows longer than this go through the pre-filter (SGB_NMS_PREFILTER=0 disables it: a tuning / A-B hook)
+// multi-label rows longer than this go through the pre-filter
 static bool prefilter_wanted(const SgbNmsDesc* d) {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("SGB_NMS_PREFILTER");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on && d->multi_label && (int64_t)d->L * d->ncls > 4 * PF_SLICE && (int64_t)d->L * d->ncls < (1ll << 30) && isfinite(d->score_thr);
+  return d->multi_label && (int64_t)d->L * d->ncls > 4 * PF_SLICE && (int64_t)d->L * d->ncls < (1ll << 30) && isfinite(d->score_thr);
 }
 static int prefilter_slices(const SgbNmsDesc* d, int* slice_len) {
   const int64_t n = (int64_t)d->L * d->ncls;
@@ -594,14 +589,9 @@ static int prefilter_slices(const SgbNmsDesc* d, int* slice_len) {
   return (int)((n + sl - 1) / sl);
 }
 
-// more than this many candidates per image: front / IoU-matrix / back as three launches (SGB_NMS_SPLIT=0 disables it)
+// more than this many candidates per image: front / IoU-matrix / back as three launches
 static bool split_wanted(const SgbNmsDesc* d) {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("SGB_NMS_SPLIT");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on && d->top_k > 512;
+  return d->top_k > 512;
 }
 static int64_t align256(int64_t v) { return (v + 255) / 256 * 256; }
 // workspace layout: [single-label conf / labels  |  pre-filter candidates] [stages] [masks]

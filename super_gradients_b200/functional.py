@@ -253,7 +253,7 @@ class StagedWeightCache:
 # launches per bottleneck around the dgrad.  With a token the shortcut's backward only parks (dout, alpha, x); cv1's backward runs its
 # dgrad as before and then ONE pass dx = alpha * dout + dx, dot = sum(dout * x) in place (reads dout, x, dx; writes dx): 4 passes, one
 # launch, no ATen add (20 bottlenecks per YOLO-NAS-S step).
-DEFER_SHORTCUT = [__import__("os").environ.get("SGB_DEFER_SHORTCUT", "1") != "0"]
+DEFER_SHORTCUT = [True]  # False: the plain shortcut backward, which test_dual_conv_and_deferred_shortcut_are_the_same_csp_layer compares against
 
 
 class _DeferTok:
@@ -373,7 +373,7 @@ def _scalar(v) -> int:
 def _gemm_stats(kout, pixels, device, sync):
     """BatchNorm statistics buffer for the producing GEMM's epilogue, or None for wide layers: the BatchNorm launch computes them
     (kernels.stats_in_bn).  With cross-rank statistics the buffer carries the local element count too."""
-    return None if K.stats_in_bn(kout, pixels) else K.new_stats(kout, device, **({"count": pixels} if sync is not None else {}))
+    return None if K.stats_in_bn(kout) else K.new_stats(kout, device, **({"count": pixels} if sync is not None else {}))
 
 
 def _bump_batches_tracked(*nbts):
@@ -562,7 +562,7 @@ def conv_bn_act(x, w, gamma, beta, running_mean, running_var, num_batches_tracke
 # refreshed when the parameter changes), the output allocated with that pitch and handed on as its first K channels, and in the
 # backward the incoming gradient re-described with the padded channel count when its producer marked the padding as zero
 # (`_sgb_zero_pad`, set by the head-decode backward), else copied into a zeroed buffer.
-KPAD = [__import__("os").environ.get("SGB_KPAD", "1") != "0"]
+KPAD = [True]  # False: the unpadded convolution, which test_k_padded_prediction_conv_is_the_same_conv compares against
 
 
 # ------------------------------------------------------------------------------------------------------------ conv + BN stem on patches
@@ -633,7 +633,7 @@ def conv_bn_act_stem(x, conv, bn, *, act, cache: StagedWeightCache):
 # gradients in place (SgbBnDesc.dy2), 1 dgrad (no add), 1 wgrad whose rows are the two filters' gradients.  The two layers keep their
 # own parameters / state-dict keys; the BatchNorm parameters, statistics and gradient slots of the pair must be adjacent in memory
 # (training/flat_state.py lays them out so on request: YoloNASCSPLayer.sgb_adjacent_tensors) -- dual_conv_bn_act_ready() checks.
-DUAL_CONV = [__import__("os").environ.get("SGB_DUAL_CONV", "1") != "0"]
+DUAL_CONV = [True]  # False: two separate layers, which test_dual_conv_and_deferred_shortcut_are_the_same_csp_layer compares against
 
 
 def _follows(a, b) -> bool:
@@ -787,15 +787,14 @@ def conv_bias(x, w, b, *, stride, pad, cache: WeightCache, act=None):
 
 
 # ------------------------------------------------------------------------------------------------------------ QARepVGG
-# Folded QARepVGG (default; SGB_QAREP_FOLD=0 restores the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
+# Folded QARepVGG (QAREP_FOLD; test_folded_qarepvgg_path_is_the_same_block holds the two-convolution form): a stride-1 block runs its 1x1 branch as the centre tap
 # of ONE 3x3 convolution with 2K output channels (rows [0, K) = the 3x3 filters, rows [K, 2K) = alpha * K1 + I embedded at the centre),
 # so y3 and u come out of one convolution launch that reads x once, dgrad consumes [dy3 | du] in one launch (no accumulating
 # epilogue) and wgrad produces both gradients in one launch.  The eight off-centre taps of rows [K, 2K) are zeros: the three calls
 # pass centre_from=K, and the kernels skip the products with those zeros (and, in wgrad, the off-centre gradients of those rows,
 # which nobody reads).  The folded filters are written in place by the step's batched re-layout launch (WeightCache.get_blocks) and
 # the weight gradient goes to the side stream.
-QAREP_FOLD = [__import__("os").environ.get("SGB_QAREP_FOLD", "1") != "0"]
-QAREP_FOLD_MAXPIX = [int(__import__("os").environ.get("SGB_QAREP_FOLD_MAXPIX", "0"))]  # > 0: fold only maps of at most this many pixels (N*H*W)
+QAREP_FOLD = [True]
 _FOLD_CHANNELS = (32, 48, 64, 96, 128, 192)  # channel counts of the YOLO-NAS stride-1 blocks that fold
 
 
@@ -827,8 +826,6 @@ class _QARepVGG(torch.autograd.Function):
         x = K.as_nhwc(x)
         kout = w3.shape[0]
         fold = QAREP_FOLD[0] and qarep_fold_supported(w3.shape[1], x.shape[1], kout, cfg.stride)
-        if fold and QAREP_FOLD_MAXPIX[0] > 0 and x.shape[0] * x.shape[2] * x.shape[3] > QAREP_FOLD_MAXPIX[0]:
-            fold = False
         if fold:
             # one filter [2K, 3, 3, C]: rows [0, K) = K3, rows [K, 2K) = alpha * K1 + I at the centre tap (tap 4 of 9)
             srcs = [(w3, None, False, slice(None, kout), (0, 0)), (w1, alpha, cfg.residual, slice(kout, None), (9, 4))]
@@ -901,7 +898,7 @@ class _QARepVGG(torch.autograd.Function):
         return dx, dw3, _unless_slot(sg3, dg3), _unless_slot(sb3, db3), dw1, dbias1, dalpha, *post, None
 
 
-FUSE_SHORTCUT = [__import__("os").environ.get("SGB_FUSE_SHORTCUT", "1") != "0"]
+FUSE_SHORTCUT = [True]  # False: the separate shortcut add, which test_csp_layer_merged_launches_match_the_separate_layers compares against
 
 
 def qarepvgg_block(x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg):
@@ -911,7 +908,7 @@ def qarepvgg_block(x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg):
 
 
 # ------------------------------------------------------------------------------------------------------------ QARepVGG stem on patches
-STEM_PATCHES = [__import__("os").environ.get("SGB_STEM_PATCHES", "1") != "0"]
+STEM_PATCHES = [True]  # False: the direct convolution, which test_patch_stem_is_the_same_block compares against
 
 
 def stem_patch_channels(cin: int, r: int) -> int:

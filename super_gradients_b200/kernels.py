@@ -5,7 +5,6 @@ Activation tensors are NCHW-shaped torch tensors in channels_last memory format 
 slice ``buf[:, a:b]`` of such a tensor is a valid operand: its channel pitch is ``buf.shape[1]``.
 """
 import ctypes
-import os
 from typing import Optional
 
 import torch
@@ -86,10 +85,6 @@ ARENA = NO_ARENA        # the arena of the TrainStep that is executing (training
 def zeros(shape, dtype, device):
     return ARENA.zeros(tuple(shape) if not isinstance(shape, int) else (shape,), dtype, device)
 
-
-# BatchNorm / QARepVGG backward as one cooperative launch per layer instead of a reduction launch + an apply launch (SGB_FUSED_BWD=0: two passes)
-FUSED_BWD = [os.environ.get("SGB_FUSED_BWD", "1") != "0"]
-FUSED_FWD = [os.environ.get("SGB_FUSED_FWD", "1") != "0"]  # QARepVGG forward: moments + apply as one cooperative launch
 
 _ACT = {None: ACT_NONE, "none": ACT_NONE, "relu": ACT_RELU, "silu": ACT_SILU}
 
@@ -609,16 +604,14 @@ def bn_desc(x, y, eps, momentum, act, residual=None, stats_repl=STATS_REPL, samp
 # and im2col fast paths); wider layers ran the im2col kernel's general epilogue (a 32-lane butterfly per 16 columns: 1.2-1.5 TB/s on
 # 1x1 layers that move the same bytes as 4.4 TB/s ones).  Those layers now run WITHOUT epilogue statistics and their BatchNorm forward
 # is one cooperative launch (sums, grid barrier, apply).  Every such layer of YOLO-NAS at batch 32 is below 40 MB, so the apply pass's
-# re-read hits L2; ResNet-50's (up to 411 MB at batch 256) re-read from HBM and still win: 7819 -> 8509 img/s with the size bound
-# (SGB_STATS_IN_BN_MAX_BYTES, default: none) lifted.  SGB_STATS_IN_BN=0 restores the epilogue statistics everywhere.
-STATS_IN_BN = [os.environ.get("SGB_STATS_IN_BN", "1") != "0"]
-STATS_IN_BN_MAX_BYTES = [int(os.environ.get("SGB_STATS_IN_BN_MAX_BYTES", str(1 << 62)))]
+# re-read hits L2; ResNet-50's (up to 411 MB at batch 256) re-read from HBM and still win: 7819 -> 8509 img/s
+# without a size bound.
 _EPILOGUE_STATS_CHANNELS = (32, 48, 64, 96)
 
 
-def stats_in_bn(kout: int, pixels: int) -> bool:
+def stats_in_bn(kout: int) -> bool:
     """True: the layer's convolution runs without epilogue statistics and bn_act_fwd(stats=None) computes them itself."""
-    return STATS_IN_BN[0] and kout not in _EPILOGUE_STATS_CHANNELS and kout % 8 == 0 and 2 * kout * pixels <= STATS_IN_BN_MAX_BYTES[0]
+    return kout not in _EPILOGUE_STATS_CHANNELS and kout % 8 == 0
 
 
 def bn_act_fwd(x, stats, gamma, beta, running_mean, running_var, eps, momentum, act, residual=None, sample_scale=None, sync=None):
@@ -697,7 +690,7 @@ def bn_act_bwd(dy, x, y, gamma, mean, rstd, eps, act, want_residual_grad=False, 
     sums = zeros((2, c), torch.float64, x.device)
     # the forward output is only read when a residual entered the activation; otherwise the mask is recomputed from x
     y_arg = y if (want_residual_grad or beta is None or sample_scale is not None) else None
-    fused = FUSED_BWD[0] and nhwc_pitch(x) == c and sync is None
+    fused = nhwc_pitch(x) == c and sync is None
     if not fused:
         _timed("sgb_bn_act_bwd_reduce", ctypes.byref(d), _ptr(dy), _ptr(x), _ptr(y_arg), _ptr(gamma), _ptr(beta), _ptr(mean), _ptr(rstd), _ptr(sums), _stream())
     if sync is not None:
@@ -768,11 +761,8 @@ def qarep_fwd(y3, u, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp,
         return out, coef
     mom = zeros((5, c), torch.float64, y3.device)
     coef = torch.empty((9, c), dtype=torch.float32, device=y3.device)
-    if FUSED_FWD[0]:  # moments, grid barrier, apply in one cooperative launch
-        _timed("sgb_qarep_fwd_fused", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _ptr(gamma3), _ptr(beta3), _ptr(bias1a), _ptr(gamma_p), _ptr(beta_p), _ptr(rm3), _ptr(rv3), _ptr(rmp), _ptr(rvp), _ptr(out), _ptr(coef), _stream())
-        return out, coef
-    _timed("sgb_qarep_moments", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _stream())
-    _timed("sgb_qarep_fwd", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _ptr(gamma3), _ptr(beta3), _ptr(bias1a), _ptr(gamma_p), _ptr(beta_p), _ptr(rm3), _ptr(rv3), _ptr(rmp), _ptr(rvp), _ptr(out), _ptr(coef), _stream())
+    # moments, grid barrier, apply in one cooperative launch
+    _timed("sgb_qarep_fwd_fused", ctypes.byref(d), _ptr(y3), _ptr(u), _ptr(mom), _ptr(gamma3), _ptr(beta3), _ptr(bias1a), _ptr(gamma_p), _ptr(beta_p), _ptr(rm3), _ptr(rv3), _ptr(rmp), _ptr(rvp), _ptr(out), _ptr(coef), _stream())
     return out, coef
 
 
@@ -793,7 +783,7 @@ def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_
         else:
             dout = dout.contiguous(memory_format=torch.channels_last)
     sums = zeros((3, c), torch.float64, y3.device)
-    fused = FUSED_BWD[0] and sync is None
+    fused = sync is None
     if not fused:
         _timed("sgb_qarep_bwd_reduce", ctypes.byref(d), _ptr(dout), _ptr(out), _ptr(y3), _ptr(u), _ptr(coef), _ptr(sums), _stream())
     if sync is not None:

@@ -8,7 +8,7 @@ import os
 from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("SGB200_LIB") or os.path.join(_HERE, "libsgb200.so")  # SGB200_LIB: a variant build (developer hook)
+LIB_PATH = os.path.join(_HERE, "libsgb200.so")
 
 ACT_NONE, ACT_RELU, ACT_SILU = 0, 1, 2
 

@@ -235,7 +235,7 @@ class TrainStep:
         self.batched_plumbing = True
         self.arena = K.StepArena()   # zero-initialised scratch of one step (owned here: a captured graph replays its addresses)
         self.ctx = SF.StepContext()  # filter caches + batched work tables of this model
-        if self.device.type == "cuda" and os.environ.get("SGB_SIDE_WGRAD", "1") != "0":
+        if self.device.type == "cuda":
             self.ctx.side_stream = torch.cuda.Stream(device=self.device)  # weight gradients overlap the dgrad / BN-backward chain
         self._nbt = [b for n, b in model.named_buffers() if n.endswith("num_batches_tracked")]
 
@@ -404,7 +404,7 @@ class TrainStep:
         self.opt_steps = steps0
         torch.cuda.synchronize()
         SF.bump_weight_epoch()
-        split = (self.world > 1 and os.environ.get("SGB_NCCL_IN_GRAPH") != "1") or os.environ.get("SGB_SPLIT_GRAPH") == "1"
+        split = self.world > 1 or os.environ.get("SGB_SPLIT_GRAPH") == "1"
         if split:
             # Data parallel: TWO graphs around an eagerly issued all-reduce (forward + backward | NCCL | optimizer + EMA).  Capturing
             # the collective inside the graph saves one launch but depends on NCCL's capture support and on nothing else in the

@@ -194,8 +194,8 @@ def test_predict_on_raw_images_gpu(golden):
             assert float(o[:, :4].min()) > -0.35 * max(im.shape[:2]) and float(o[:, [0, 2]].max()) < 1.35 * im.shape[1]
 
 
-# 1x1 stride 1 on the channel counts of the halo variants (served by the im2col kernel; by the 16 x 16-tile kernel in the
-# -DSGB_HALO_1X1 experiment build): ragged edges, statistics with K == C and K != C, tiles > CTAs.  Kept here (not in
+# 1x1 stride 1 on the channel counts of the halo variants (served by the im2col wgmma kernel): ragged edges, statistics with
+# K == C and K != C, tiles > CTAs.  Kept here (not in
 # test_kernels_gpu.CONV_CASES) until their first hardware run.
 ONE_BY_ONE_CASES = [(8, 32, 40, 40, 32, 1, 1, 0), (4, 96, 40, 40, 96, 1, 1, 0), (3, 48, 13, 37, 48, 1, 1, 0), (2, 128, 19, 16, 64, 1, 1, 0), (40, 32, 64, 64, 32, 1, 1, 0),
                     (4, 96, 40, 40, 32, 1, 1, 0), (4, 64, 24, 24, 96, 1, 1, 0), (2, 192, 20, 20, 64, 1, 1, 0)]  # fmt: skip

@@ -43,7 +43,7 @@ def bench(fn, flush, iters=5):
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "fprop"
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-    print(f"sm100 enabled: {os.environ.get('SGB_DISABLE_SM100', '0') != '1'}  mode={which}")
+    print(f"mode={which}")
     shapes = SHAPES[: int(os.environ.get('NSHAPES', len(SHAPES)))]
     if os.environ.get("SHAPES"):
         shapes = [tuple(int(v) for v in t.split(",")) for t in os.environ["SHAPES"].split(";")]
