@@ -527,7 +527,14 @@ int sgb_resample_crop_u8(const int64_t* table_host, const int64_t* table, const 
  *   horizontal flip flag
  *   mixup: flag, partner byte offset / h / w, partner flip flag, first resize size, canvas size (target_dim), border value,
  *          second resize size (jit_factor), crop offsets x / y
- *   padded rescale: resized size (int(h * r), int(w * r)) of the affine-size image inside the out_h x out_w canvas */
+ *   padded rescale: resized size (int(h * r), int(w * r)) of the affine-size image inside the out_h x out_w canvas
+ *   mosaic (transforms.py:513-599 DetectionMosaic, get_mosaic_coordinate detection_utils.py:738-768): flag, canvas size
+ *          (2 * input_dim; the image size the affine, or the chain when the affine is off, receives), centre xc / yc, border
+ *          value, then SGB_AUG_MOS_TILES tiles of SGB_AUG_MOS_TILE_FIELDS from SGB_AUG_MOS_TILE (top-left, top-right,
+ *          bottom-left, bottom-right, tile 0 being the sample's own image): byte offset in src, source h / w, resized size
+ *          (int(h0 * scale), int(w0 * scale)), placement rectangle [x1, x2) x [y1, y2) on the canvas and the resized tile's
+ *          pixel (sx, sy) that lands on (x1, y1).  Each rectangle lies in its quadrant of (xc, yc).  With the flag set, the
+ *          source image fields (offset, h, w) repeat tile 0 and the affine reads the canvas instead of the source image. */
 #define SGB_AUG_OFFSET 0
 #define SGB_AUG_H 1
 #define SGB_AUG_W 2
@@ -559,16 +566,41 @@ int sgb_resample_crop_u8(const int64_t* table_host, const int64_t* table, const 
 #define SGB_AUG_MIX_Y 33
 #define SGB_AUG_RS_H 34
 #define SGB_AUG_RS_W 35
-#define SGB_AUG_FIELDS 36
+#define SGB_AUG_MOS 36
+#define SGB_AUG_MOS_CANVAS_H 37
+#define SGB_AUG_MOS_CANVAS_W 38
+#define SGB_AUG_MOS_XC 39
+#define SGB_AUG_MOS_YC 40
+#define SGB_AUG_MOS_BORDER 41
+#define SGB_AUG_MOS_TILE 42
+#define SGB_AUG_MOS_TILES 4
+/* fields of one mosaic tile, relative to SGB_AUG_MOS_TILE + i * SGB_AUG_MOS_TILE_FIELDS */
+#define SGB_AUG_T_OFFSET 0
+#define SGB_AUG_T_H 1
+#define SGB_AUG_T_W 2
+#define SGB_AUG_T_RH 3
+#define SGB_AUG_T_RW 4
+#define SGB_AUG_T_X1 5
+#define SGB_AUG_T_Y1 6
+#define SGB_AUG_T_X2 7
+#define SGB_AUG_T_Y2 8
+#define SGB_AUG_T_SX 9
+#define SGB_AUG_T_SY 10
+#define SGB_AUG_MOS_TILE_FIELDS 11
+#define SGB_AUG_FIELDS 86
 /* table_host: the table in host memory (validated here); table: the same table in device memory.  src: device uint8 buffer of
- * src_bytes holding every source and mixup-partner image (channels == 3).  out: device bf16 [batch, out_h, out_w, out_pitch]
- * (out_pitch >= 3, a multiple of 8; channels >= 3 written as 0).  ONE launch for the batch.  Per output pixel: cv2.warpAffine
+ * src_bytes holding every source, mosaic-tile and mixup-partner image (channels == 3).  out: device bf16 [batch, out_h, out_w,
+ * out_pitch] (out_pitch >= 3, a multiple of 8; channels >= 3 written as 0).  ONE launch for the batch.  Per output pixel: [mosaic:
+ * each source pixel read below is a canvas pixel, i.e. the cv2.resize (INTER_LINEAR) of the one tile whose rectangle holds it,
+ * else the mosaic border value; the affine's border value applies only outside the canvas] -> cv2.warpAffine
  * (INTER_LINEAR, BORDER_CONSTANT, fixed point) -> channel swap -> augment_hsv (cv2 BGR2HSV / HSV2BGR; hsv_simd_block: the pixel
  * count of one vector block of cv2's HSV2BGR, whose columns below w - w % block truncate and whose tail rounds) -> horizontal flip
  * -> mixup with the partner's canvas, each cv2.resize on the way recomputed -> bottom-right placement, resized (INTER_LINEAR)
  * when the rescale size differs from the affine size, onto pad_value -> v / max_value -> round-to-nearest bf16.  Bit-exact with
  * the reference's cv2 / numpy chain.  A table naming bytes outside src, a degenerate or non-finite matrix, a matrix mapping
- * the output outside +-2^20 source pixels, or a bad size or flag is refused with SGB_E_INVALID.  batch == 0 is a no-op. */
+ * the output outside +-2^20 source pixels, or a bad size or flag is refused with SGB_E_INVALID; so is a mosaic whose tile lies
+ * outside src, whose resized size is not in [1, 32768), whose rectangle leaves its quadrant of the canvas or reads outside the
+ * resized tile, whose centre lies outside the canvas or whose border value is not in [0, 255].  batch == 0 is a no-op. */
 int sgb_detection_augment(const int64_t* table_host, const int64_t* table, const uint8_t* src, int64_t src_bytes, int32_t batch,
                           int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t pad_value, double max_value,
                           int32_t hsv_simd_block, sgb_bf16* out, void* stream);

@@ -1,7 +1,7 @@
 // Arithmetic of the detection train augmentation (augment.cu), host+device like preprocess_math.cuh: the kernel calls
 // augment_pixel() per output pixel and the CPU suite compiles this header with g++ to check it, bit for bit, against cv2 4.x and
-// the reference's numpy chain (transforms.py random_affine :1464-1534, augment_hsv :1623-1634, DetectionMixup :729-797,
-// _rescale_and_pad_to_size utils.py:203-226).
+// the reference's numpy chain (transforms.py DetectionMosaic :536-588, random_affine :1464-1534, augment_hsv :1623-1634,
+// DetectionMixup :729-797, _rescale_and_pad_to_size utils.py:203-226).
 //
 // cv2.warpAffine, uint8, INTER_LINEAR, BORDER_CONSTANT (imgproc/src/imgwarp.cpp): M is inverted in double, then per output row
 //   X0 = rint((A12 * y + b1) * 1024) + 16, per column adelta = rint(A11 * x * 1024), X = (X0 + adelta) >> 5 (Y likewise);
@@ -64,6 +64,50 @@ struct RemapTabs {
   const int16_t* cubic;    // [1024][16]
   const int16_t* lanczos;  // [1024][64]
 };
+
+// DetectionMosaic's canvas pixel (y, x) of table row t (its tiles in src) into q[3].  The tiles do not overlap and tile i lies in
+// quadrant i of (xc, yc), so only that tile can hold the pixel.  Inside its rectangle the value is cv2.resize (INTER_LINEAR) of the
+// tile's source to (rh, rw) at the pixel shifted by the placement; outside, the mosaic border value.
+SGB_HD void mosaic_pixel(const uint8_t* src, const int64_t* t, int y, int x, int q[3]) {
+  const int i = (y >= (int)t[SGB_AUG_MOS_YC] ? 2 : 0) + (x >= (int)t[SGB_AUG_MOS_XC] ? 1 : 0);
+  const int64_t* k = t + SGB_AUG_MOS_TILE + i * SGB_AUG_MOS_TILE_FIELDS;
+  if (y < (int)k[SGB_AUG_T_Y1] || y >= (int)k[SGB_AUG_T_Y2] || x < (int)k[SGB_AUG_T_X1] || x >= (int)k[SGB_AUG_T_X2]) {
+    q[0] = q[1] = q[2] = (int)t[SGB_AUG_MOS_BORDER];
+    return;
+  }
+  const int H = (int)k[SGB_AUG_T_H], W = (int)k[SGB_AUG_T_W], rh = (int)k[SGB_AUG_T_RH], rw = (int)k[SGB_AUG_T_RW];
+  const int ry = y - (int)k[SGB_AUG_T_Y1] + (int)k[SGB_AUG_T_SY], rx = x - (int)k[SGB_AUG_T_X1] + (int)k[SGB_AUG_T_SX];
+  const uint8_t* img = src + k[SGB_AUG_T_OFFSET];
+  if (rh == H && rw == W) {
+    for (int c = 0; c < 3; ++c) q[c] = img[((int64_t)ry * W + rx) * 3 + c];
+    return;
+  }
+  const sgb_prep::Taps r = sgb_prep::resize_taps(H, W, rh, rw, ry, rx);
+  const uint8_t* r0 = img + (int64_t)r.y0 * W * 3;
+  const uint8_t* r1 = img + (int64_t)r.y1 * W * 3;
+  for (int c = 0; c < 3; ++c) q[c] = sgb_prep::resize_combine(r, r0[r.x0 * 3 + c], r0[r.x1 * 3 + c], r1[r.x0 * 3 + c], r1[r.x1 * 3 + c]);
+}
+
+// cv2.warpAffine INTER_LINEAR pixel (y, x) of the mosaic canvas (MOS_CANVAS_H x MOS_CANVAS_W) into p[3]: warp_pixel's four taps,
+// each a mosaic_pixel, the taps outside the canvas reading border
+SGB_HD void warp_mosaic_pixel(const uint8_t* src, const int64_t* t, const Inverse& a, int border, int y, int x, int p[3]) {
+  const int H = (int)t[SGB_AUG_MOS_CANVAS_H], W = (int)t[SGB_AUG_MOS_CANVAS_W];
+  int X, Y;
+  warp_coord(a, y, x, X, Y);
+  const int fx = X & 31, fy = Y & 31, sx = X >> 5, sy = Y >> 5;
+  const int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
+  int acc[3] = {0, 0, 0};
+  for (int k = 0; k < 4; ++k) {
+    const int ty = sy + (k >> 1), tx = sx + (k & 1);
+    int q[3] = {border, border, border};
+    if (ty >= 0 && ty < H && tx >= 0 && tx < W) mosaic_pixel(src, t, ty, tx, q);
+    for (int c = 0; c < 3; ++c) acc[c] += q[c] * w[k];
+  }
+  for (int c = 0; c < 3; ++c) {
+    const int v = (acc[c] + (1 << 14)) >> 15;
+    p[c] = v < 0 ? 0 : (v > 255 ? 255 : v);
+  }
+}
 
 // cv2.warpAffine pixel (y, x) of an H x W x 3 image (dense rows) into p[3], BORDER_CONSTANT with border[3].  mode: cv2's
 // interpolation flag, 0 INTER_NEAREST, 1 INTER_LINEAR, 2 INTER_CUBIC, 3 INTER_AREA (warpAffine runs it as INTER_LINEAR),
@@ -200,12 +244,18 @@ SGB_HD int mix_value(const uint8_t* mix, const int64_t* t, int y, int x, int c) 
                                   mix_canvas1(mix, t, k.y1, k.x1, c));
 }
 
-// uint8 pixel (y, x) of the sample after affine -> swap -> HSV -> flip -> mixup (the image DetectionPaddedRescale receives)
+// uint8 pixel (y, x) of the sample after [mosaic] -> affine -> swap -> HSV -> flip -> mixup (the image DetectionPaddedRescale
+// receives).  With the mosaic, the affine (or, without it, the chain) reads the canvas instead of the sample's image.  kMosaic ==
+// false compiles the mosaic out: the kernel instance for batches without a mosaic sample.
+template <bool kMosaic>
 SGB_HD void chain_pixel(const uint8_t* src, const int64_t* t, const Inverse& a, int block, int y, int x, int p[3]) {
   const int H = (int)t[SGB_AUG_H], W = (int)t[SGB_AUG_W], aw = (int)t[SGB_AUG_AFF_W];
   const uint8_t* img = src + t[SGB_AUG_OFFSET];
   const int xs = t[SGB_AUG_FLIP] ? aw - 1 - x : x;
-  if (t[SGB_AUG_AFFINE]) {
+  if (kMosaic && t[SGB_AUG_MOS]) {
+    if (t[SGB_AUG_AFFINE]) warp_mosaic_pixel(src, t, a, (int)t[SGB_AUG_AFF_BORDER], y, xs, p);
+    else mosaic_pixel(src, t, y, xs, p);
+  } else if (t[SGB_AUG_AFFINE]) {
     warp_pixel(img, H, W, a, (int)t[SGB_AUG_AFF_BORDER], y, xs, p);
   } else {
     for (int c = 0; c < 3; ++c) p[c] = img[((int64_t)y * W + xs) * 3 + c];
@@ -226,6 +276,8 @@ SGB_HD void chain_pixel(const uint8_t* src, const int64_t* t, const Inverse& a, 
 }
 
 // uint8 pixel (oy, ox) of the out_h x out_w padded-rescale canvas: the chain image resized to (RS_H, RS_W) at the top left
+// (kMosaic as for chain_pixel; augment_pixel<true> serves every table row)
+template <bool kMosaic = true>
 SGB_HD void augment_pixel(const uint8_t* src, const int64_t* t, const Inverse& a, int block, int pad_value, int oy, int ox, int p[3]) {
   const int rh = (int)t[SGB_AUG_RS_H], rw = (int)t[SGB_AUG_RS_W], ah = (int)t[SGB_AUG_AFF_H], aw = (int)t[SGB_AUG_AFF_W];
   if (oy >= rh || ox >= rw) {
@@ -233,15 +285,15 @@ SGB_HD void augment_pixel(const uint8_t* src, const int64_t* t, const Inverse& a
     return;
   }
   if (rh == ah && rw == aw) {
-    chain_pixel(src, t, a, block, oy, ox, p);
+    chain_pixel<kMosaic>(src, t, a, block, oy, ox, p);
     return;
   }
   const sgb_prep::Taps k = sgb_prep::resize_taps(ah, aw, rh, rw, oy, ox);
   int q[4][3];
-  chain_pixel(src, t, a, block, k.y0, k.x0, q[0]);
-  chain_pixel(src, t, a, block, k.y0, k.x1, q[1]);
-  chain_pixel(src, t, a, block, k.y1, k.x0, q[2]);
-  chain_pixel(src, t, a, block, k.y1, k.x1, q[3]);
+  chain_pixel<kMosaic>(src, t, a, block, k.y0, k.x0, q[0]);
+  chain_pixel<kMosaic>(src, t, a, block, k.y0, k.x1, q[1]);
+  chain_pixel<kMosaic>(src, t, a, block, k.y1, k.x0, q[2]);
+  chain_pixel<kMosaic>(src, t, a, block, k.y1, k.x1, q[3]);
   for (int c = 0; c < 3; ++c) p[c] = sgb_prep::resize_combine(k, q[0][c], q[1][c], q[2][c], q[3][c]);
 }
 

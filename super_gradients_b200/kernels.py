@@ -432,7 +432,7 @@ def resample_crop_u8(table_host, table, src, out, max_value=255.0, reverse_chann
     return out
 
 
-AUG_FIELDS = 36  # SGB_AUG_FIELDS: per-image draws of the detection train augmentation (include/sgb200.h)
+AUG_FIELDS = 86  # SGB_AUG_FIELDS: per-image draws of the detection train augmentation (include/sgb200.h)
 HSV_SIMD_BLOCK = 32  # pixels per vector block of cv2's 8-bit HSV2BGR in its x86 builds (the row tail is rounded, the blocks truncated)
 
 

@@ -3,7 +3,7 @@
 `DetectionAugmentDataset` wraps any map-style dataset with `__len__` and `get_sample(index)` returning the reference's raw sample
 dict (`image` uint8 H x W x 3, `target` [n, 5] xyxy + label, optional `crowd_target`).  In DataLoader workers it runs the host half
 of the transforms the way the reference's DetectionDataset.apply_transforms does (detection_dataset.py:394-450): the draws, the
-mixup partner index, the box arithmetic.  `DetectionAugmentCollateFN` packs a batch into one uint8 buffer (table + images) plus
+mosaic's three and the mixup's one extra sample index, the box arithmetic.  `DetectionAugmentCollateFN` packs a batch into one uint8 buffer (table + images) plus
 the targets, touching no CUDA state; `PackedDetectionBatch.to_model_input(device)` then makes the model input with one copy and
 one kernel launch."""
 import random

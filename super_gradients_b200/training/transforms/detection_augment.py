@@ -1,12 +1,12 @@
 """Pixels of the YOLO-NAS COCO train augmentation on the GPU.
 
-An `AugmentPlan` holds the draws of one sample of the recipe chain DetectionRandomAffine -> DetectionRGB2BGR -> DetectionHSV ->
-DetectionHorizontalFlip -> DetectionMixup -> DetectionPaddedRescale -> DetectionStandardize (the reference's
-training/transforms/transforms.py).  `BatchAugmenter` (and `PackedDetectionBatch`, built by `DetectionAugmentCollateFN` in DataLoader
+An `AugmentPlan` holds the draws of one sample of the recipe chain DetectionMosaic -> DetectionRandomAffine -> DetectionRGB2BGR ->
+DetectionHSV -> DetectionHorizontalFlip -> DetectionMixup -> DetectionPaddedRescale -> DetectionStandardize (the reference's
+training/transforms/transforms.py); a mosaic sample carries its four source images.  `BatchAugmenter` (and `PackedDetectionBatch`, built by `DetectionAugmentCollateFN` in DataLoader
 workers) packs the images and the per-image table of a batch into one buffer, sends it with one copy and runs one kernel launch (csrc/augment.cu) that writes the bf16 NHWC [B, 16, H, W] model input,
 bit-exact with the reference's cv2 / numpy chain followed by DetectionCollateFN and functional.to_nhwc."""
 from dataclasses import dataclass
-from typing import Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -18,6 +18,9 @@ OFFSET, H, W, AFFINE, AFF_H, AFF_W, M, AFF_BORDER = 0, 1, 2, 3, 4, 5, 6, 12
 SWAP, HSV, DH, DS, DV, BGR, FLIP = 13, 14, 15, 16, 17, 18, 19
 MIX, MIX_OFFSET, MIX_H, MIX_W, MIX_FLIP, MIX_R1_H, MIX_R1_W, MIX_CANVAS_H, MIX_CANVAS_W, MIX_BORDER = 20, 21, 22, 23, 24, 25, 26, 27, 28, 29
 MIX_R2_H, MIX_R2_W, MIX_X, MIX_Y, RS_H, RS_W = 30, 31, 32, 33, 34, 35
+MOS, MOS_CANVAS_H, MOS_CANVAS_W, MOS_XC, MOS_YC, MOS_BORDER, MOS_TILE, MOS_TILE_FIELDS = 36, 37, 38, 39, 40, 41, 42, 11
+# columns of a mosaic tile relative to MOS_TILE + i * MOS_TILE_FIELDS
+T_OFFSET, T_H, T_W, T_RH, T_RW, T_X1, T_Y1, T_X2, T_Y2, T_SX, T_SY = range(11)
 
 
 @dataclass
@@ -36,10 +39,35 @@ class MixupPlan:
 
 
 @dataclass
+class MosaicTile:
+    """One of DetectionMosaic's four images: the source (uint8 H x W x 3), its resized size (int(h0 * scale), int(w0 * scale)),
+    its rectangle (x1, y1, x2, y2) on the canvas and the resized tile's pixel (sx, sy) placed at (x1, y1)
+    (get_mosaic_coordinate's large and small coordinates)."""
+
+    image: np.ndarray
+    resized: Tuple[int, int]
+    rect: Tuple[int, int, int, int]
+    origin: Tuple[int, int]
+
+
+@dataclass
+class MosaicPlan:
+    """DetectionMosaic's draws: the four tiles (top-left, top-right, bottom-left, bottom-right; tile 0 holds the sample's own
+    image), the canvas size (2 * input_dim), the centre (xc, yc) and the border value."""
+
+    tiles: List[MosaicTile]
+    canvas: Tuple[int, int]
+    xc: int
+    yc: int
+    border_value: int = 114
+
+
+@dataclass
 class AugmentPlan:
-    """One sample's draws.  `affine`: the forward 2 x 3 matrix of random_affine (None: DetectionRandomAffine closed) with its output
-    size (rows, cols) and border value; `hsv`: the int16 gains (dh, ds, dv) with bgr_channels (None: not applied);
-    `rescaled`: (int(h * r), int(w * r)) of DetectionPaddedRescale."""
+    """One sample's draws.  `mosaic`: DetectionMosaic's canvas (None: no mosaic; its tile 0 holds `image`); `affine`: the forward
+    2 x 3 matrix of random_affine (None: DetectionRandomAffine closed) with its output size (rows, cols) and border value; `hsv`:
+    the int16 gains (dh, ds, dv) with bgr_channels (None: not applied); `rescaled`: (int(h * r), int(w * r)) of
+    DetectionPaddedRescale."""
 
     image: np.ndarray
     rescaled: Tuple[int, int]
@@ -48,9 +76,22 @@ class AugmentPlan:
     hsv: Optional[Tuple[int, int, int, Tuple[int, int, int]]] = None
     flip: bool = False
     mixup: Optional[MixupPlan] = None
+    mosaic: Optional[MosaicPlan] = None
+
+    def size_before_affine(self) -> Tuple[int, int]:
+        return tuple(self.mosaic.canvas) if self.mosaic is not None else tuple(self.image.shape[:2])
 
     def size_after_affine(self) -> Tuple[int, int]:
-        return tuple(self.affine[1]) if self.affine is not None else tuple(self.image.shape[:2])
+        return tuple(self.affine[1]) if self.affine is not None else self.size_before_affine()
+
+    def images(self) -> List[np.ndarray]:
+        """The images the kernel reads, in packing order: the sample's, the mosaic's three others, the mixup partner."""
+        out = [self.image]
+        if self.mosaic is not None:
+            out += [t.image for t in self.mosaic.tiles[1:]]
+        if self.mixup is not None:
+            out.append(self.mixup.image)
+        return out
 
 
 def _check_image(im, what):
@@ -58,12 +99,12 @@ def _check_image(im, what):
         raise ValueError(f"{what} must be a uint8 H x W x 3 array, got {getattr(im, 'dtype', type(im))} {getattr(im, 'shape', '')}")
 
 
-def fill_table(plans: Sequence[AugmentPlan], offsets: Sequence[Tuple[int, Optional[int]]], table: np.ndarray) -> None:
-    """Writes the int64 [B, AUG_FIELDS] table of `plans`; offsets[b] = (byte offset of the image, of the mixup partner or None)."""
+def fill_table(plans: Sequence[AugmentPlan], offsets: Sequence[Sequence[int]], table: np.ndarray) -> None:
+    """Writes the int64 [B, AUG_FIELDS] table of `plans`; offsets[b]: the byte offset of each of plans[b].images()."""
     table[:] = 0
-    for b, (p, (off, moff)) in enumerate(zip(plans, offsets)):
+    for b, (p, offs) in enumerate(zip(plans, offsets)):
         t = table[b]
-        t[OFFSET], t[H], t[W] = off, p.image.shape[0], p.image.shape[1]
+        t[OFFSET], t[H], t[W] = offs[0], p.image.shape[0], p.image.shape[1]
         t[AFF_H], t[AFF_W] = p.size_after_affine()
         if p.affine is not None:
             m, _, border = p.affine
@@ -77,36 +118,49 @@ def fill_table(plans: Sequence[AugmentPlan], offsets: Sequence[Tuple[int, Option
             t[HSV], t[DH], t[DS], t[DV], t[BGR] = 1, dh, ds, dv, bgr[0] | bgr[1] << 2 | bgr[2] << 4
         if p.mixup is not None:
             x = p.mixup
-            t[MIX], t[MIX_OFFSET], t[MIX_H], t[MIX_W], t[MIX_FLIP] = 1, moff, x.image.shape[0], x.image.shape[1], int(x.flip)
+            t[MIX], t[MIX_OFFSET], t[MIX_H], t[MIX_W], t[MIX_FLIP] = 1, offs[-1], x.image.shape[0], x.image.shape[1], int(x.flip)
             t[MIX_R1_H], t[MIX_R1_W] = x.resized
             t[MIX_CANVAS_H], t[MIX_CANVAS_W] = x.canvas
             t[MIX_BORDER] = x.border_value
             t[MIX_R2_H], t[MIX_R2_W] = x.jittered
             t[MIX_X], t[MIX_Y] = x.x_offset, x.y_offset
         t[RS_H], t[RS_W] = p.rescaled
+        if p.mosaic is not None:
+            mo = p.mosaic
+            t[MOS], (t[MOS_CANVAS_H], t[MOS_CANVAS_W]), t[MOS_XC], t[MOS_YC], t[MOS_BORDER] = 1, mo.canvas, mo.xc, mo.yc, mo.border_value
+            for i, (tile, off) in enumerate(zip(mo.tiles, offs)):
+                k = t[MOS_TILE + i * MOS_TILE_FIELDS : MOS_TILE + (i + 1) * MOS_TILE_FIELDS]
+                k[T_OFFSET], k[T_H], k[T_W] = off, tile.image.shape[0], tile.image.shape[1]
+                k[T_RH], k[T_RW] = tile.resized
+                k[T_X1], k[T_Y1], k[T_X2], k[T_Y2] = tile.rect
+                k[T_SX], k[T_SY] = tile.origin
 
 
 def packed_size(plans: Sequence[AugmentPlan]) -> int:
-    """Bytes of the packed form of `plans`: the int64 table, then every image and mixup partner."""
-    return len(plans) * K.AUG_FIELDS * 8 + sum(p.image.nbytes + (p.mixup.image.nbytes if p.mixup is not None else 0) for p in plans)
+    """Bytes of the packed form of `plans`: the int64 table, then every image, mosaic tile and mixup partner."""
+    return len(plans) * K.AUG_FIELDS * 8 + sum(im.nbytes for p in plans for im in p.images())
 
 
 def pack_into(plans: Sequence[AugmentPlan], raw: np.ndarray) -> None:
     """Writes the packed form of `plans` into the uint8 array `raw` (at least packed_size(plans) bytes)."""
     for p in plans:
         _check_image(p.image, "the image")
+        if p.mosaic is not None:
+            if len(p.mosaic.tiles) != 4 or p.mosaic.tiles[0].image is not p.image:
+                raise ValueError("a mosaic has four tiles, the first holding the sample's own image")
+            for tile in p.mosaic.tiles[1:]:
+                _check_image(tile.image, "a mosaic tile")
         if p.mixup is not None:
             _check_image(p.mixup.image, "the mixup image")
     head = len(plans) * K.AUG_FIELDS * 8
     offsets, pos = [], 0
     for p in plans:
-        off, pos = pos, pos + p.image.nbytes
-        raw[head + off : head + pos] = np.ascontiguousarray(p.image).reshape(-1)
-        moff = None
-        if p.mixup is not None:
-            moff, pos = pos, pos + p.mixup.image.nbytes
-            raw[head + moff : head + pos] = np.ascontiguousarray(p.mixup.image).reshape(-1)
-        offsets.append((off, moff))
+        offs = []
+        for im in p.images():
+            offs.append(pos)
+            raw[head + pos : head + pos + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
+            pos += im.nbytes
+        offsets.append(offs)
     fill_table(plans, offsets, raw[:head].view(np.int64).reshape(len(plans), K.AUG_FIELDS))
 
 

@@ -1,11 +1,11 @@
-"""The YOLO-NAS COCO train transforms (reference: training/transforms/transforms.py:490-1330, 1345-1554, 1579-1590, 1623-1634,
-transforms/utils.py:45-57, 183-226, utils/detection_utils.py:174-185, 771-785), split in two halves.
+"""The YOLO-NAS COCO and Roboflow fine-tuning train transforms (reference: training/transforms/transforms.py:490-1330, 1345-1554,
+1579-1590, 1623-1634, transforms/utils.py:45-57, 183-226, utils/detection_utils.py:174-185, 738-785), split in two halves.
 
 On the host, in DataLoader workers, each transform draws its random numbers from the global `random` / `np.random` in the
 reference's order and transforms the boxes with the reference's numpy arithmetic.  The pixels are not touched: every transform
 records its draws in the sample's `AugmentPlan`, and `BatchAugmenter` later turns a batch of plans into the model input with one
 kernel launch (csrc/augment.cu).  The kernel applies the steps in the recipe's order, so a pipeline must list these transforms in
-that order (`check_order`)."""
+that order (`check_order`); DetectionMosaic, when present, comes first and the kernel reads its canvas as the chain's source."""
 import math
 import random
 from numbers import Number
@@ -15,10 +15,10 @@ import cv2
 import numpy as np
 
 from ...common.registry import register_transform
-from .detection_augment import AugmentPlan, MixupPlan
+from .detection_augment import AugmentPlan, MixupPlan, MosaicPlan, MosaicTile
 
-RECIPE_ORDER = ("DetectionRandomAffine", "DetectionRGB2BGR", "DetectionHSV", "DetectionHorizontalFlip", "DetectionMixup", "DetectionPaddedRescale",
-                "DetectionStandardize", "DetectionTargetsFormatTransform")  # fmt: skip
+RECIPE_ORDER = ("DetectionMosaic", "DetectionRandomAffine", "DetectionRGB2BGR", "DetectionHSV", "DetectionHorizontalFlip", "DetectionMixup",
+                "DetectionPaddedRescale", "DetectionStandardize", "DetectionTargetsFormatTransform")  # fmt: skip
 
 
 def _tuple_of_two(v):
@@ -95,6 +95,65 @@ class _Transform:
 
     def close(self):
         pass
+
+
+def get_mosaic_coordinate(mosaic_index, xc, yc, w, h, input_h, input_w):
+    """Where tile `mosaic_index` (0 top-left, 1 top-right, 2 bottom-left, 3 bottom-right) of a resized w x h image lands on the
+    2 * input_h x 2 * input_w canvas: (x1, y1, x2, y2) on the canvas and (x1s, y1s, x2s, y2s) in the tile."""
+    if mosaic_index == 0:
+        x1, y1, x2, y2 = max(xc - w, 0), max(yc - h, 0), xc, yc
+        small_coord = w - (x2 - x1), h - (y2 - y1), w, h
+    elif mosaic_index == 1:
+        x1, y1, x2, y2 = xc, max(yc - h, 0), min(xc + w, input_w * 2), yc
+        small_coord = 0, h - (y2 - y1), min(w, x2 - x1), h
+    elif mosaic_index == 2:
+        x1, y1, x2, y2 = max(xc - w, 0), yc, xc, min(input_h * 2, yc + h)
+        small_coord = w - (x2 - x1), 0, w, min(y2 - y1, h)
+    else:
+        x1, y1, x2, y2 = xc, yc, min(xc + w, input_w * 2), min(input_h * 2, yc + h)
+        small_coord = 0, 0, min(w, x2 - x1), min(y2 - y1, h)
+    return (x1, y1, x2, y2), small_coord
+
+
+@register_transform()
+class DetectionMosaic(_Transform):
+    """Four samples (this one and three random others), each resized to fit input_dim, placed around a random centre of a
+    2 * input_dim canvas of border_value.  The coin flip happens in get_number_of_additional_samples, so a failed flip (or a closed
+    mosaic) leaves the sample as it is."""
+
+    def __init__(self, input_dim, prob: float = 1.0, enable_mosaic: bool = True, border_value=114):
+        self.prob, self.input_dim, self.enable_mosaic, self.border_value = prob, _tuple_of_two(input_dim), enable_mosaic, border_value
+
+    def close(self):
+        self.enable_mosaic = False
+
+    def get_number_of_additional_samples(self) -> int:
+        return 3 if self.enable_mosaic and random.random() < self.prob else 0
+
+    @property
+    def may_require_additional_samples(self) -> bool:
+        return self.enable_mosaic
+
+    def apply_to_sample(self, sample: HostSample) -> HostSample:
+        if not sample.additional_samples or not self.enable_mosaic:
+            return sample
+        input_h, input_w = self.input_dim
+        yc = int(random.uniform(0.5 * input_h, 1.5 * input_h))
+        xc = int(random.uniform(0.5 * input_w, 1.5 * input_w))
+        tiles, boxes, labels, is_crowd = [], [], [], []
+        for i, s in enumerate([sample] + sample.additional_samples):
+            h0, w0 = s.shape
+            scale = min(1.0 * input_h / h0, 1.0 * input_w / w0)
+            h, w = int(h0 * scale), int(w0 * scale)
+            (l_x1, l_y1, l_x2, l_y2), (s_x1, s_y1, _, _) = get_mosaic_coordinate(i, xc, yc, w, h, input_h, input_w)
+            tiles.append(MosaicTile(s.plan.image, (h, w), (l_x1, l_y1, l_x2, l_y2), (s_x1, s_y1)))
+            padw, padh = l_x1 - s_x1, l_y1 - s_y1
+            boxes.append(s.bboxes_xyxy * scale + np.array([[padw, padh, padw, padh]], dtype=np.float32))
+            labels.append(s.labels)
+            is_crowd.append(s.is_crowd)
+        canvas = (input_h * 2, input_w * 2)
+        sample.plan.mosaic = MosaicPlan(tiles, canvas, xc, yc, int(self.border_value))
+        return HostSample(sample.plan, canvas, np.concatenate(boxes, 0), np.concatenate(labels, 0), np.concatenate(is_crowd, 0))
 
 
 def get_aug_params(value: Union[tuple, float], center: float = 0) -> float:
