@@ -605,6 +605,54 @@ int sgb_detection_augment(const int64_t* table_host, const int64_t* table, const
                           int32_t channels, int32_t out_h, int32_t out_w, int32_t out_pitch, int32_t pad_value, double max_value,
                           int32_t hsv_simd_block, sgb_bf16* out, void* stream);
 
+/* ---- ImageNet train augmentation (recipes/dataset_params/imagenet_resnet50_dataset_params.yaml train chain:
+ *      datasets/datasets_utils.py:316-354 RandomResizedCropAndInterpolation, RandomHorizontalFlip, datasets/auto_augment.py:271-447
+ *      RandAugment, ToTensor, Normalize; datasets/mixup.py:104-313 CollateMixup, batch mode) ---- */
+/* Per-image table: int64 [batch][SGB_IN_FIELDS].
+ *   crop window: byte offset in src, h, w (dense rows of w * 3 bytes: only the window RandomResizedCrop chose), filter (0 bilinear,
+ *   1 bicubic), horizontal flip flag, byte offset in the workspace of the window's horizontally resized rows (h * size * 3 bytes)
+ *   then SGB_IN_OPS RandAugment ops in order, SGB_IN_OP_FIELDS each from SGB_IN_OP: the op code, then its arguments:
+ *     AFFINE: Pillow's inverse 2 x 3 matrix as six float64 values stored bit for bit (ShearX / Y, TranslateXRel / YRel, Rotate)
+ *     POSTERIZE: bits kept in [0, 8); SOLARIZE: threshold in [0, 256]; SOLARIZE_ADD: the addend in [0, 255]
+ *     BRIGHTNESS, CONTRAST, COLOR, SHARPNESS: the enhance factor as a float64 value stored bit for bit
+ *     NONE, INVERT, AUTOCONTRAST, EQUALIZE: none */
+#define SGB_IN_OFFSET 0
+#define SGB_IN_H 1
+#define SGB_IN_W 2
+#define SGB_IN_FILTER 3
+#define SGB_IN_FLIP 4
+#define SGB_IN_WS_OFFSET 5
+#define SGB_IN_OP 6
+#define SGB_IN_OP_FIELDS 7
+#define SGB_IN_OPS 2
+#define SGB_IN_FIELDS 20
+#define SGB_IN_OP_NONE 0
+#define SGB_IN_OP_AFFINE 1
+#define SGB_IN_OP_INVERT 2
+#define SGB_IN_OP_POSTERIZE 3
+#define SGB_IN_OP_SOLARIZE 4
+#define SGB_IN_OP_SOLARIZE_ADD 5
+#define SGB_IN_OP_BRIGHTNESS 6
+#define SGB_IN_OP_CONTRAST 7
+#define SGB_IN_OP_AUTOCONTRAST 8
+#define SGB_IN_OP_EQUALIZE 9
+#define SGB_IN_OP_COLOR 10
+#define SGB_IN_OP_SHARPNESS 11
+/* table_host: the table in host memory (validated here); table: the same table in device memory.  src: device uint8 buffer of
+ * src_bytes holding every crop window.  workspace: caller-owned device uint8 buffer of workspace_bytes receiving each window's
+ * horizontal resize pass.  out: device bf16 [batch, size, size, out_pitch] (out_pitch >= 3, a multiple of 8; channels >= 3 written
+ * as 0).  fill_host[3]: RandAugment's fill colour (img_mean in uint8); mean_host[3] / std_host[3]: Normalize.  mix_mode 0: no mix,
+ * 1: mixup with lam / one_minus_lam (float32 values of lam and 1 - lam), 2: cutmix of the box box_host[4] = (yl, yh, xl, xh);
+ * image i mixes with image batch - 1 - i.  ONE launch for the batch (batch even): a thread-block cluster of two CTAs holds the
+ * pair (i, batch - 1 - i), each CTA its image in shared memory: Pillow's 8-bit crop resize -> flip -> the two RandAugment ops ->
+ * ToTensor / Normalize in float32 -> the mix, reading the partner's pixels from its CTA's shared memory -> round-to-nearest
+ * bf16.  Bit-exact with the reference's PIL chain and CollateMixup.  Bytes outside src or the workspace, an unknown op or filter,
+ * a bad argument, size, flag, mix mode or box, or an odd batch is refused with SGB_E_INVALID.  batch == 0 is a no-op. */
+int sgb_imagenet_augment(const int64_t* table_host, const int64_t* table, const uint8_t* src, int64_t src_bytes, uint8_t* workspace,
+                         int64_t workspace_bytes, int32_t batch, int32_t size, int32_t out_pitch, const int32_t* fill_host,
+                         const float* mean_host, const float* std_host, int32_t mix_mode, float lam, float one_minus_lam,
+                         const int32_t* box_host, sgb_bf16* out, void* stream);
+
 /* ---- pose train augmentation (training/transforms/keypoints/*.py of the YOLO-NAS-POSE recipes: KeypointsRandomHorizontalFlip,
  *      KeypointsBrightnessContrast, KeypointsReverseImageChannels, KeypointsHSV, KeypointsRandomRotate90,
  *      KeypointsRandomAffineTransform, KeypointsMosaic, KeypointsLongestMaxSize, KeypointsPadIfNeeded, KeypointsImageStandardize) ---- */

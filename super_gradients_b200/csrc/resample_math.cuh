@@ -7,11 +7,13 @@
 // StandardizeImage -> NormalizeImage -> ImagePermute.
 //
 // Pillow's 8-bit resample (libImaging/Resample.c) is integer arithmetic on coefficients computed in double.  Per axis, for output
-// index xx of an in -> out resize:
-//   scale = in / out;  fs = max(scale, 1);  support = fs;  ss = 1 / fs;  center = (xx + 0.5) * scale
+// index xx of an in -> out resize with a filter of support s (bilinear 1, bicubic 2):
+//   scale = in / out;  fs = max(scale, 1);  support = s * fs;  ss = 1 / fs;  center = (xx + 0.5) * scale
 //   xmin = max((int)(center - support + 0.5), 0);  n = min((int)(center + support + 0.5), in) - xmin
-//   w[x] = tri((x + xmin - center + 0.5) * ss), tri(t) = max(0, 1 - |t|);  w[x] /= sum(w)   (double)
-//   k[x] = (int)(0.5 + w[x] * 2^22)   (22-bit fixed point; the weights are never negative)
+//   w[x] = f((x + xmin - center + 0.5) * ss);  w[x] /= sum(w)   (double)
+//   bilinear f(t) = max(0, 1 - |t|);  bicubic (a = -0.5) f(t) = ((a + 2)|t| - (a + 3))|t|^2 + 1 for |t| < 1,
+//   (((|t| - 5)|t| + 8)|t| - 4) a for |t| < 2, else 0
+//   k[x] = (int)(0.5 + w[x] * 2^22), or (int)(-0.5 + w[x] * 2^22) for a negative weight (22-bit fixed point)
 // The horizontal pass runs first and stores uint8: clip8((2^21 + sum src * k) >> 22); the vertical pass runs on that uint8
 // intermediate with the same rounding.  An axis whose size does not change gets the one-tap weight 2^22, which reproduces
 // Pillow's skipped pass exactly ((v << 22) + 2^21) >> 22 == v).
@@ -58,21 +60,25 @@ SGB_HD double ddiv(double a, double b) {
 #endif
 }
 
+enum Filter { kBilinear = 0, kBicubic = 1 };
+
 struct Axis {
   double scale, support, ss;
+  int filter;
 };
 
-SGB_HD Axis axis(int in, int out) {
+SGB_HD Axis axis(int in, int out, int filter = kBilinear) {
   Axis a;
+  a.filter = filter;
   a.scale = ddiv((double)in, (double)out);
   const double fs = a.scale < 1.0 ? 1.0 : a.scale;
-  a.support = fs;  // the bilinear filter's support is 1
+  a.support = filter == kBicubic ? dmul(2.0, fs) : fs;
   a.ss = ddiv(1.0, fs);
   return a;
 }
 
 // most taps any output index of an in -> out resize can have (Pillow's ksize)
-SGB_HD int max_taps(int in, int out) { return (int)ceil(axis(in, out).support) * 2 + 1; }
+SGB_HD int max_taps(int in, int out, int filter = kBilinear) { return (int)ceil(axis(in, out, filter).support) * 2 + 1; }
 
 // first source index and tap count of output index xx
 SGB_HD void bounds(const Axis& a, int xx, int in, int& xmin, int& n) {
@@ -84,10 +90,13 @@ SGB_HD void bounds(const Axis& a, int xx, int in, int& xmin, int& n) {
   n = xmax - xmin;
 }
 
-SGB_HD double tri_weight(const Axis& a, int x, int xmin, double center) {
+SGB_HD double filter_weight(const Axis& a, int x, int xmin, double center) {
   double t = dmul(dadd(dadd((double)(x + xmin), -center), 0.5), a.ss);
   if (t < 0.0) t = -t;
-  return t < 1.0 ? dadd(1.0, -t) : 0.0;
+  if (a.filter != kBicubic) return t < 1.0 ? dadd(1.0, -t) : 0.0;
+  if (t < 1.0) return dadd(dmul(dmul(dadd(dmul(1.5, t), -2.5), t), t), 1.0);
+  if (t < 2.0) return dmul(dadd(dmul(dadd(dmul(dadd(t, -5.0), t), 8.0), t), -4.0), -0.5);
+  return 0.0;
 }
 
 // fixed-point weights of output index xx into k[0..n); returns n, and the first source index in xmin
@@ -96,11 +105,11 @@ SGB_HD int coeffs(const Axis& a, int xx, int in, int32_t* k, int& xmin) {
   bounds(a, xx, in, xmin, n);
   const double center = dmul((double)xx + 0.5, a.scale);
   double ww = 0.0;
-  for (int x = 0; x < n; ++x) ww = dadd(ww, tri_weight(a, x, xmin, center));
+  for (int x = 0; x < n; ++x) ww = dadd(ww, filter_weight(a, x, xmin, center));
   for (int x = 0; x < n; ++x) {
-    double w = tri_weight(a, x, xmin, center);
+    double w = filter_weight(a, x, xmin, center);
     if (ww != 0.0) w = ddiv(w, ww);
-    k[x] = (int32_t)dadd(0.5, dmul(w, (double)(1 << kPrecisionBits)));
+    k[x] = (int32_t)dadd(w < 0.0 ? -0.5 : 0.5, dmul(w, (double)(1 << kPrecisionBits)));
   }
   return n;
 }

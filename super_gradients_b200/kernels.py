@@ -7,6 +7,7 @@ slice ``buf[:, a:b]`` of such a tensor is a valid operand: its channel pitch is 
 import ctypes
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import lib as L
@@ -454,6 +455,37 @@ def detection_augment(table_host, table, src, out, pad_value=114, max_value=255.
         raise L.SgbError("out must be a dense bf16 NHWC batch [B, c_pad, out_h, out_w]")
     _timed("sgb_detection_augment", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel(), B, 3, out.shape[2], out.shape[3], pitch,
            int(pad_value), float(max_value), HSV_SIMD_BLOCK, _ptr(out), _stream())  # fmt: skip
+    return out
+
+
+IN_FIELDS = 20  # SGB_IN_FIELDS: per-image draws of the ImageNet train augmentation (include/sgb200.h)
+
+
+def imagenet_augment(table_host, table, src, workspace, out, fill, mean, std, mix_mode=0, lam=1.0, box=(0, 0, 0, 0)):
+    """ImageNet train augmentation of a whole batch in one launch.  table_host: int64 [B, IN_FIELDS] CPU tensor (sgb200.h SGB_IN_*),
+    table: the same on the device; src: device uint8 buffer of every crop window; workspace: device uint8 buffer of the horizontal
+    resize pass (h * S * 3 bytes per window at its WS_OFFSET); out: bf16 NHWC [B, c_pad, S, S] (channels >= 3 are zeroed).  fill:
+    RandAugment's uint8 fill colour; mean / std: Normalize's; mix_mode 0 none, 1 mixup with `lam`, 2 cutmix of box (yl, yh, xl, xh)
+    with partner B - 1 - i."""
+    for t, n in ((src, "src"), (table, "table"), (workspace, "workspace"), (out, "out")):
+        require_cuda(t, n)
+    if out.data_ptr() % 16:
+        raise L.SgbError("out must be 16-byte aligned (the kernel stores 8 channels at a time)")
+    if table_host.dtype != torch.int64 or table_host.dim() != 2 or table_host.shape[1] != IN_FIELDS or not table_host.is_contiguous() or table_host.is_cuda:
+        raise L.SgbError(f"table_host must be a contiguous int64 [B, {IN_FIELDS}] host tensor")
+    if table.dtype != torch.int64 or tuple(table.shape) != tuple(table_host.shape) or not table.is_contiguous():
+        raise L.SgbError("table must be the device copy of table_host")
+    if src.dtype != torch.uint8 or workspace.dtype != torch.uint8 or not src.is_contiguous() or not workspace.is_contiguous():
+        raise L.SgbError("src and workspace must be contiguous uint8 buffers")
+    B, pitch = table_host.shape[0], nhwc_pitch(out)
+    if out.dtype != torch.bfloat16 or out.shape[0] != B or out.shape[1] != pitch or out.shape[2] != out.shape[3]:
+        raise L.SgbError("out must be a dense square bf16 NHWC batch [B, c_pad, S, S]")
+    f = (ctypes.c_int32 * 3)(*[int(v) for v in fill])
+    m, s = (ctypes.c_float * 3)(*[float(v) for v in mean]), (ctypes.c_float * 3)(*[float(v) for v in std])
+    bx = (ctypes.c_int32 * 4)(*[int(v) for v in box])
+    lam32 = float(np.float32(lam))
+    _timed("sgb_imagenet_augment", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel(), _ptr(workspace), workspace.numel(), B, out.shape[2],
+           pitch, f, m, s, int(mix_mode), lam32, float(np.float32(1.0 - lam)), bx, _ptr(out), _stream())  # fmt: skip
     return out
 
 
