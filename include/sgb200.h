@@ -737,6 +737,15 @@ int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, cons
 /* ema = ema * (*decay) + (1 - *decay) * p   (training/utils/ema.py:126-142) */
 int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream);
 
+/* ---- best-snapshot average (training/utils/weight_averaging_utils.py:89-95, sg_trainer.py:732-739) ----------------------- */
+#define SGB_AVG_MAX_SLOTS 64
+/* slots: DEVICE array of k device pointers, each to n float32 values (snapshot slots 0 .. k-1, in slot order).  out[i] is the
+ * reference's running mean  a <- s_0[i];  for m = 1 .. k-1: a <- (a * m + s_m[i]) / (m + 1),  every multiply, add and divide
+ * rounded to float32 on its own (no FMA contraction), so the result is bit-identical to the reference's torch loop on the CPU,
+ * Inf and subnormals included; NaN stays NaN.  One pass: k * n * 4 bytes read, n * 4 written.  k outside [1, SGB_AVG_MAX_SLOTS],
+ * n < 0 or a NULL pointer is refused with SGB_E_INVALID; n == 0 is a no-op.  out may not alias a slot. */
+int sgb_average_snapshots(const float* const* slots, int32_t k, int64_t n, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1103,3 +1103,13 @@ def adamw_step(p, g, m, v, hp):
 
 def ema_update(ema, p, decay_dev):
     _timed("sgb_ema_update", _ptr(ema), _ptr(p), p.numel(), _ptr(decay_dev), _stream())
+
+
+def average_snapshots(slot_ptr_table, k, out):
+    """out (device float32, n values) = the reference's running mean of the k snapshot slots whose device addresses are the first k
+    entries of slot_ptr_table (device int64); each slot holds out.numel() float32 values."""
+    require_cuda(slot_ptr_table, "slot_ptr_table")
+    require_cuda(out, "out")
+    if slot_ptr_table.dtype != torch.int64 or slot_ptr_table.numel() < k or out.dtype != torch.float32 or not out.is_contiguous():
+        raise L.SgbError("average_snapshots: slot_ptr_table must be int64 with >= k entries and out a contiguous float32 tensor")
+    _timed("sgb_average_snapshots", _ptr(slot_ptr_table), int(k), out.numel(), _ptr(out), _stream())

@@ -231,6 +231,7 @@ _SIGNATURES = {
     "sgb_sgd_step": (c_int, [P, P, P, _L, P, P]),
     "sgb_adamw_step": (c_int, [P, P, P, P, _L, P, P]),
     "sgb_ema_update": (c_int, [P, P, _L, P, P]),
+    "sgb_average_snapshots": (c_int, [P, c_int32, _L, P, P]),
 }
 
 _lib = None

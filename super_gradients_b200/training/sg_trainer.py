@@ -15,6 +15,7 @@ import inspect
 import math
 import os
 import time
+import warnings
 from typing import Any, Callable, Dict, Mapping, Optional
 
 import torch
@@ -23,8 +24,10 @@ from torch import nn
 from .. import functional as SF
 from .. import kernels as K
 from ..common.factories import LossesFactory, MetricsFactory, _fuzzy
+from ..common.registry import CALLBACKS
 from .flat_state import FlatState
 from .utils.callbacks import CallbackHandler, PhaseContext
+from .utils.weight_averaging_utils import ModelWeightAveraging
 
 DEFAULT_TRAINING_PARAMS = {
     "max_epochs": 1,
@@ -65,7 +68,13 @@ DEFAULT_TRAINING_PARAMS = {
     "resume_path": None,  # ... or from an explicit checkpoint file
     "ckpt_name": "ckpt_latest.pth",
     "resume_strict_load": True,
+    # keep the best validated snapshots, write their average to average_model.pth and validate it once at the end (reference
+    # sg_trainer.py:603-609, 732-739, 1645-1653).  The reference's default is True (training/params.py:28); here it is False so that
+    # runs which do not ask for it write the files they always wrote.
+    "average_best_models": False,
 }
+
+AVERAGE_MODEL_FILENAME = "average_model.pth"
 
 # defaults merged under user optimizer_params (reference: training/params.py:84-90)
 OPTIMIZER_DEFAULTS = {"SGD": {"weight_decay": 1e-4, "momentum": 0.9}, "Adam": {"weight_decay": 1e-4}, "AdamW": {"weight_decay": 1e-2}}
@@ -159,6 +168,21 @@ def setup_device(device: Optional[str] = None):
         # a finite timeout turns a lost rank / mismatched collective into an error instead of an endless wait
         torch.distributed.init_process_group("nccl", init_method="env://", device_id=torch.device("cuda", local_rank), timeout=datetime.timedelta(minutes=4))
     return torch.device("cuda", local_rank)
+
+
+def _resolve_callbacks(entries) -> list:
+    """phase_callbacks entries: callback objects as they are, recipe entries {name: kwargs} built through the CALLBACKS registry."""
+    from .utils import early_stopping as _registered_callbacks  # noqa: F401  (fills the CALLBACKS registry)
+
+    out = []
+    for cb in entries or []:
+        if isinstance(cb, Mapping):
+            if len(cb) != 1 or next(iter(cb)) not in CALLBACKS:
+                raise ValueError(f"phase_callbacks entry {cb} is not {{name: kwargs}} with a registered name; registered: {sorted(CALLBACKS)}")
+            name, kwargs = next(iter(cb.items()))
+            cb = CALLBACKS[name](**dict(kwargs or {}))
+        out.append(cb)
+    return out
 
 
 def _update_metrics(metrics, fields: Mapping[str, Any]):
@@ -447,6 +471,7 @@ class Trainer:
         self.device = setup_device(device)
         self.net: Optional[nn.Module] = None
         self.step: Optional[TrainStep] = None
+        self.model_weight_averaging: Optional[ModelWeightAveraging] = None
         self.history: Dict[str, list] = {"train_loss": [], "valid_loss": [], "lr": []}
 
     @property
@@ -465,6 +490,10 @@ class Trainer:
     # ------------------------------------------------------------------------------------------------ train
     def train(self, model: nn.Module, training_params: Mapping[str, Any], train_loader, valid_loader=None, test_loaders=None, additional_configs_to_log=None):
         tp = {**DEFAULT_TRAINING_PARAMS, **dict(training_params or {})}
+        if tp["average_best_models"] and not tp["save_model"]:
+            warnings.warn("'training_params.average_best_models' is enabled, but 'training_params.save_model' is disabled: model averaging "
+                          "writes its snapshots next to the checkpoints, so 'average_best_models' is disabled")  # reference sg_trainer.py:1428-1434
+            tp["average_best_models"] = False
         ckpt = None
         if tp["resume"] or tp["resume_path"]:
             path = tp["resume_path"] or os.path.join(self.checkpoints_dir_path, tp["ckpt_name"])
@@ -490,7 +519,7 @@ class Trainer:
         train_metrics = [MetricsFactory().get(m) for m in tp["train_metrics_list"] or []]
         self.step = TrainStep(self.net, criterion, tp["optimizer"], tp["optimizer_params"], bool(tp["zero_weight_decay_on_bias_and_bn"]), ema=bool(tp["ema"]), batch_accumulate=int(tp["batch_accumulate"]),
                               keep_outputs=bool(train_metrics))  # fmt: skip
-        handler = CallbackHandler(tp["phase_callbacks"])
+        handler = CallbackHandler(_resolve_callbacks(tp["phase_callbacks"]))
         context = PhaseContext(net=self.net, criterion=criterion, device=self.device, experiment_name=self.experiment_name, ckpt_dir=self.checkpoints_dir_path,
                                train_loader=train_loader, valid_loader=valid_loader, training_params=tp, optimizer=None, context_methods=self)  # fmt: skip
         steps_per_epoch = len(train_loader) if tp["max_train_batches"] is None else min(len(train_loader), int(tp["max_train_batches"]))
@@ -503,9 +532,19 @@ class Trainer:
             start_epoch = int(ckpt.get("epoch", -1)) + 1
             best = ckpt.get("acc")
             self._restore_training_state(ckpt)
+        self.model_weight_averaging = None
+        if tp["average_best_models"] and not self.ddp_silent_mode:  # the snapshots live on rank 0 only
+            os.makedirs(self.checkpoints_dir_path, exist_ok=True)
+            watched = bool(tp["metric_to_watch"])
+            self.model_weight_averaging = ModelWeightAveraging(self.checkpoints_dir_path, greater_is_better=watched and bool(tp["greater_metric_to_watch_is_better"]),
+                                                               metric_to_watch=tp["metric_to_watch"] if watched else "valid_loss", load_checkpoint=ckpt is not None)  # fmt: skip
         t0 = time.time()
         handler.fire("on_training_start", context)
         for epoch in range(start_epoch, int(tp["max_epochs"])):
+            if handler.callbacks and is_distributed():  # a callback may stop the run: every rank stops with rank 0 (reference sg_trainer.py:1524)
+                flag = torch.tensor([int(bool(context.stop_training))], device=self.device)
+                torch.distributed.broadcast(flag, 0)
+                context.stop_training = bool(flag.item())
             if context.stop_training:
                 break
             self.net.train()
@@ -535,8 +574,6 @@ class Trainer:
                         self.step.capture(inputs, targets)
                     elif not getattr(self, "_warned_no_graph", False):
                         # detection / pose targets stay on the host (ragged per-image lists padded by the loss): the step runs eagerly
-                        import warnings
-
                         warnings.warn("training_params['cuda_graph'] is set but the targets are not a device tensor (detection / pose losses pad them on the "
                                       "host): the train step runs without a CUDA graph; TrainStep.capture() with device-resident padded targets (bench.py) captures it")
                         self._warned_no_graph = True
@@ -586,13 +623,45 @@ class Trainer:
                     watch, greater = None, False
                 is_best = watch is not None and (best is None or (watch > best if greater else watch < best))
                 best = watch if is_best else best
-                self._save_checkpoint(epoch, metrics, tp, is_best, acc=best if best is not None else watch)
+                self._save_checkpoint(epoch, metrics, tp, is_best, acc=best if best is not None else watch, watched=watch if validated else None)
                 if is_best and "valid_loss" in metrics:
                     handler.fire("on_validation_end_best_epoch", context)
             if not tp["silent_mode"] and not self.ddp_silent_mode:
                 print(f"[{self.experiment_name}] epoch {epoch} " + " ".join(f"{k}={v:.5f}" for k, v in metrics.items()) + f" ({time.time() - t0:.1f}s)")
+        if tp["average_best_models"]:
+            handler.fire("on_average_best_models_validation_start", context)
+            self._validate_final_average_model(valid_loader, tp, handler, context)
+            handler.fire("on_average_best_models_validation_end", context)
+            if self.model_weight_averaging is not None:
+                self.model_weight_averaging.cleanup()
         handler.fire("on_training_end", context)
         return self.history
+
+    def _validate_final_average_model(self, valid_loader, tp, handler, context):
+        """Validates average_model.pth once after the last epoch (reference sg_trainer.py:1785-1822): every rank loads it into the
+        live model after rank 0 has written it, the results go to history["average_model"] and context.metrics_dict, then the live
+        weights come back bit for bit.  Skipped with a warning when there is nothing to validate: no validation loader, or no
+        snapshot was ever taken (every validated metric was non-finite, so the file's net is None)."""
+        if is_distributed():
+            torch.distributed.barrier()
+        path = os.path.join(self.checkpoints_dir_path, AVERAGE_MODEL_FILENAME)
+        average_sd = torch.load(path, map_location="cpu", weights_only=False)["net"] if os.path.isfile(path) else None
+        if valid_loader is None or average_sd is None:
+            warnings.warn("average_best_models: no averaged model to validate (no validation loader, or no validated epoch had a finite watched metric)")
+            return
+        keep = {k: v.detach().clone() for k, v in self.net.state_dict().items()}
+        try:
+            self.net.load_state_dict(average_sd)
+            SF.bump_weight_epoch()
+            context.update_context(epoch=int(tp["max_epochs"]))
+            results = {"valid_loss": self._validate(valid_loader, tp, handler, context)}
+            results.update(self.valid_metric_values)
+        finally:
+            self.net.load_state_dict(keep)
+            SF.bump_weight_epoch()
+            self.step._filters_stale = True
+        self.history["average_model"] = results
+        context.update_context(metrics_dict=results)
 
     @torch.no_grad()
     def _validate(self, loader, tp, handler=None, context=None) -> float:
@@ -722,9 +791,11 @@ class Trainer:
                     st.ema_buffers[off : off + k].copy_(ema[name].reshape(-1).to(st.ema_buffers.device))
                     off += k
 
-    def _save_checkpoint(self, epoch: int, metrics: dict, tp, is_best: bool, acc=None):
+    def _save_checkpoint(self, epoch: int, metrics: dict, tp, is_best: bool, acc=None, watched=None):
         """Same dictionary keys as the reference (sg_trainer.py:649-739): net, acc, epoch, metrics, optimizer_state_dict,
-        ema_net, ..."""
+        ema_net, ...  watched: this epoch's watched validation value (None when validation did not run); with average_best_models
+        it updates the snapshots, and average_model.pth gets the checkpoint without the optimizer, scaler and EMA entries and with
+        the average as net (reference :732-739)."""
         os.makedirs(self.checkpoints_dir_path, exist_ok=True)
         state = {
             "net": self._state_dict(False),
@@ -743,3 +814,9 @@ class Trainer:
             torch.save(state, os.path.join(self.checkpoints_dir_path, "ckpt_best.pth"))
         if epoch in tp["save_ckpt_epoch_list"]:
             torch.save(state, os.path.join(self.checkpoints_dir_path, f"ckpt_epoch_{epoch}.pth"))
+        if self.model_weight_averaging is not None and watched is not None:
+            mwa = self.model_weight_averaging
+            average = mwa.get_average_model(state["ema_net"] if self.step.ema_on else state["net"], {mwa.metric_to_watch: watched})
+            averaged = {k: v for k, v in state.items() if k not in ("optimizer_state_dict", "scaler_state_dict", "ema_net")}
+            averaged["net"] = average
+            torch.save(averaged, os.path.join(self.checkpoints_dir_path, AVERAGE_MODEL_FILENAME))

@@ -18,6 +18,8 @@ class Phase(Enum):
     VALIDATION_END_BEST_EPOCH = "VALIDATION_END_BEST_EPOCH"
     TEST_BATCH_END = "TEST_BATCH_END"
     TEST_END = "TEST_END"
+    AVERAGE_BEST_MODELS_VALIDATION_START = "AVERAGE_BEST_MODELS_VALIDATION_START"
+    AVERAGE_BEST_MODELS_VALIDATION_END = "AVERAGE_MODEL_VALIDATION_END"  # the reference's value (base_callbacks.py:25)
     POST_TRAINING = "POST_TRAINING"
 
     @staticmethod
@@ -26,6 +28,17 @@ class Phase(Enum):
             return Phase[phase_str]
         except KeyError:
             raise ValueError(f"Invalid phase string: '{phase_str}'. Must be one of: {[p.name for p in Phase]}")
+
+
+def to_phase(phase) -> Phase:
+    """A Phase, its name, or a recipe's {"_target_": "...Phase", "value": "<name>"} entry (hydra instantiates it as Phase(value))."""
+    if isinstance(phase, Phase):
+        return phase
+    if isinstance(phase, dict):
+        if not str(phase.get("_target_", "")).endswith("Phase") or "value" not in phase:
+            raise ValueError(f"not a Phase entry: {phase}")
+        return Phase(phase["value"])
+    return Phase.from_string(phase)
 
 
 class PhaseContext:
@@ -62,6 +75,8 @@ class Callback:
     def on_test_batch_start(self, context: PhaseContext) -> None: ...
     def on_test_batch_end(self, context: PhaseContext) -> None: ...
     def on_test_loader_end(self, context: PhaseContext) -> None: ...
+    def on_average_best_models_validation_start(self, context: PhaseContext) -> None: ...
+    def on_average_best_models_validation_end(self, context: PhaseContext) -> None: ...
     def on_training_end(self, context: PhaseContext) -> None: ...
 
 
@@ -69,7 +84,8 @@ _PHASE_OF_EVENT = {
     "on_training_start": Phase.PRE_TRAINING, "on_train_loader_start": Phase.TRAIN_EPOCH_START, "on_train_batch_loss_end": Phase.TRAIN_BATCH_END,
     "on_train_batch_gradient_step_end": Phase.TRAIN_BATCH_STEP, "on_train_loader_end": Phase.TRAIN_EPOCH_END, "on_validation_batch_end": Phase.VALIDATION_BATCH_END,
     "on_validation_loader_end": Phase.VALIDATION_EPOCH_END, "on_validation_end_best_epoch": Phase.VALIDATION_END_BEST_EPOCH, "on_test_batch_end": Phase.TEST_BATCH_END,
-    "on_test_loader_end": Phase.TEST_END, "on_training_end": Phase.POST_TRAINING,
+    "on_test_loader_end": Phase.TEST_END, "on_average_best_models_validation_start": Phase.AVERAGE_BEST_MODELS_VALIDATION_START,
+    "on_average_best_models_validation_end": Phase.AVERAGE_BEST_MODELS_VALIDATION_END, "on_training_end": Phase.POST_TRAINING,
 }  # fmt: skip
 
 
