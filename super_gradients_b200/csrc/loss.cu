@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(256) tal_topk_kernel(SgbLossDesc d, const floa
           bi = sidx[q];
         }
       w.topk[bg * d.topk + k] = bi;
-      smet[bi] = -2.f;  // remove from further rounds
+      if (bi < d.L) smet[bi] = -2.f;  // remove from further rounds (none left, or only NaN metrics: bi stays 0x7fffffff)
     }
     __syncthreads();
   }
@@ -617,6 +617,8 @@ int check_loss(const SgbLossDesc* d) {
   SGB_REQUIRE(d && d->B > 0 && d->L > 0 && d->ncls > 0, "bad desc");
   SGB_REQUIRE(d->reg_max + 1 <= MAXBINS, "reg_max + 1 must be <= 32");
   SGB_REQUIRE(d->n_max >= 0 && d->topk > 0 && d->topk <= 64, "n_max / topk");
+  // tal_topk_kernel takes one anchor per round: with every anchor taken it would write past the metric row (torch.topk raises)
+  SGB_REQUIRE(d->topk <= d->L, "topk must not exceed the number of anchors");
   return SGB_OK;
 }
 

@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(256) pose_topk_kernel(SgbPoseLossDesc d, const
           bi = sidx[q];
         }
       w.topk[bg * d.topk + k] = bi;
-      smet[bi] = -2.f;  // remove from further rounds
+      if (bi < d.L) smet[bi] = -2.f;  // remove from further rounds (none left, or only NaN metrics: bi stays 0x7fffffff)
     }
     __syncthreads();
   }
@@ -220,6 +220,7 @@ int check_desc(const SgbPoseLossDesc* d) {
   SGB_REQUIRE(d->J <= MAXJ, "at most 64 joints");
   SGB_REQUIRE(d->reg_max + 1 <= MAXBINS, "reg_max + 1 must be <= 32");
   SGB_REQUIRE(d->n_max >= 0 && d->topk > 0 && d->topk <= 64, "n_max / topk");
+  SGB_REQUIRE(d->topk <= d->L, "topk must not exceed the number of anchors");  // torch.topk raises there
   SGB_REQUIRE(d->iou_type == 0 || d->iou_type == 1, "iou_type");
   return SGB_OK;
 }
