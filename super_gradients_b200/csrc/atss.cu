@@ -1,78 +1,42 @@
 // ATSS assigner (row L2's static variant: ppyolo_loss.py:301-434) with the outputs of sgb_tal_assign, so that the fused
 // varifocal / IoU / DFL kernel (loss.cu) runs unchanged behind either assigner.  Two launches:
-//   atss_candidates_kernel  one CTA per (image, gt): per pyramid level the topk anchors closest to the GT centre (distance row in
-//                           shared memory, iterative arg-min, ties -> lowest index), IoU threshold = mean + std over the
+//   atss_candidates_kernel  one CTA per (image, gt): per pyramid level the topk anchors closest to the GT centre (negated distance
+//                           row in shared memory, block-wide top-k, ties -> lowest index), IoU threshold = mean + std over the
 //                           levels x topk candidates, positives counted / owned per anchor with atomics
 //   atss_resolve_kernel     one thread per (image, anchor): 0 / 1 / several claiming GTs -> label, box, IoU(gt, predicted box)
 // instead of the reference's [B, n, L] float tensors (IoU, distance, one-hot top-k, masks: ~10 x B*n*L*4 bytes each way).
 // Algorithmic traffic: reg_distri read once (B*L*68*4 B) + anchors; everything else is per-GT shared-memory work.
-// The arithmetic is in atss_math.cuh (shared with the CPU test build).
+// The arithmetic is in atss_math.cuh and tal_math.cuh (shared with the CPU test build).
 #include "atss_math.cuh"
 #include "common.cuh"
 
 namespace {
 
-using sgb_atss::Box;
+using namespace sgb_tal;
 using sgb_atss::Levels;
 
 __global__ void __launch_bounds__(256) atss_candidates_kernel(SgbLossDesc d, Levels lv, const float* __restrict__ anchors,
                                                               const float* __restrict__ gtb, const uint8_t* __restrict__ gtv,
                                                               int* __restrict__ count, int* __restrict__ owner) {
-  extern __shared__ float sdist[];  // distance row of one level
-  __shared__ float sval[8];
-  __shared__ int sidx[8];
+  extern __shared__ float sdist[];  // negated distance row of one level: the nearest anchors are the largest entries
   __shared__ int cand[sgb_atss::kMaxLevels * sgb_atss::kMaxTopk];
   __shared__ float ciou[sgb_atss::kMaxLevels * sgb_atss::kMaxTopk];
   __shared__ float thr_s;
   const int bg = blockIdx.x, b = bg / d.n_max, g = bg - b * d.n_max, t = threadIdx.x;
   if (!gtv[bg]) return;
-  const Box gt = sgb_atss::load_box(gtb + (int64_t)bg * 4);
+  const Box gt = load_box(gtb + (int64_t)bg * 4);
   for (int lvl = 0; lvl < lv.n; ++lvl) {
     const int base = lv.start[lvl], num = lv.start[lvl + 1] - base;
-    for (int a = t; a < num; a += blockDim.x) sdist[a] = sgb_atss::center_distance(gt, sgb_atss::load_box(anchors + (int64_t)(base + a) * 4));
+    for (int a = t; a < num; a += blockDim.x) sdist[a] = -sgb_atss::center_distance(gt, load_box(anchors + (int64_t)(base + a) * 4));
     __syncthreads();
-    for (int k = 0; k < d.topk; ++k) {
-      float bv = INFINITY;
-      int bi = 0x7fffffff;
-      for (int a = t; a < num; a += blockDim.x) {
-        const float v = sdist[a];
-        if (v < bv) {  // strict: keeps the lowest index within a thread
-          bv = v;
-          bi = a;
-        }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov < bv || (ov == bv && oi < bi)) {
-          bv = ov;
-          bi = oi;
-        }
-      }
-      if ((t & 31) == 0) {
-        sval[t >> 5] = bv;
-        sidx[t >> 5] = bi;
-      }
-      __syncthreads();
-      if (t == 0) {
-        for (int q = 1; q < 8; ++q)
-          if (sval[q] < bv || (sval[q] == bv && sidx[q] < bi)) {
-            bv = sval[q];
-            bi = sidx[q];
-          }
-        cand[lvl * d.topk + k] = base + bi;
-        sdist[bi] = INFINITY;  // remove from further rounds (a selected distance is finite, so this never re-selects)
-      }
-      __syncthreads();
-    }
+    block_topk(sdist, num, d.topk, [&](int k, int a) { cand[lvl * d.topk + k] = base + a; });
   }
   const int K = lv.n * d.topk;
-  if (t < K) ciou[t] = sgb_atss::iou(gt, sgb_atss::load_box(anchors + (int64_t)cand[t] * 4), 1e-10f);
+  if (t < K) ciou[t] = iou(gt, load_box(anchors + (int64_t)cand[t] * 4), 1e-10f);
   __syncthreads();
   if (t == 0) thr_s = sgb_atss::iou_threshold(ciou, K);
   __syncthreads();
-  if (t < K && ciou[t] > thr_s && sgb_atss::center_inside(sgb_atss::load_box(anchors + (int64_t)cand[t] * 4), gt)) {
+  if (t < K && ciou[t] > thr_s && sgb_atss::center_inside(load_box(anchors + (int64_t)cand[t] * 4), gt)) {
     const int64_t i = (int64_t)b * d.L + cand[t];
     atomicAdd(&count[i], 1);
     atomicMin(&owner[i], g);
@@ -92,19 +56,15 @@ __global__ void atss_resolve_kernel(SgbLossDesc d, const float* __restrict__ reg
     const int c = count[i];
     int ag = -1;
     if (c == 1) ag = owner[i];
-    else if (c > 1) ag = sgb_atss::argmax_iou_gt(sgb_atss::load_box(anchors + (int64_t)l * 4), gts, d.n_max);
+    else if (c > 1) ag = sgb_atss::argmax_iou_gt(load_box(anchors + (int64_t)l * 4), gts, d.n_max);
     // the reference gathers gt 0's box for unassigned anchors (argmax of an all-zero column)
-    const float* gb = gts + (ag >= 0 ? ag : 0) * 4;
-    abox[i * 4 + 0] = gb[0];
-    abox[i * 4 + 1] = gb[1];
-    abox[i * 4 + 2] = gb[2];
-    abox[i * 4 + 3] = gb[3];
+    const Box gb = load_box(gts + (ag >= 0 ? ag : 0) * 4);
+    store_box(abox + i * 4, gb);
     float sc = 0.f;
     int lab = d.ncls;
     if (ag >= 0) {
       lab = gtl[b * d.n_max + ag];
-      const Box p = sgb_atss::decode_box(reg + i * 4 * bins, bins, ap[l * 2], ap[l * 2 + 1], st[l]);
-      sc = sgb_atss::iou(sgb_atss::load_box(gb), p, 1e-9f);
+      sc = iou(gb, decode_box(reg + i * 4 * bins, bins, ap[l * 2], ap[l * 2 + 1], st[l]), 1e-9f);
     }
     alabel[i] = lab;
     ascore[i] = sc;
@@ -119,10 +79,6 @@ __global__ void atss_init_kernel(int* count, int* owner, int64_t n) {
     count[i] = 0;
     owner[i] = 0x7fffffff;
   }
-}
-
-__global__ void atss_fill_kernel(int* p, int64_t n, int v) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
 }  // namespace
@@ -170,14 +126,8 @@ extern "C" int sgb_atss_assign(const SgbLossDesc* d, const float* reg_distri, co
     atss_candidates_kernel<<<d->B * d->n_max, 256, smem, st>>>(*d, lv, anchors, gt_boxes, gt_valid, count, owner);
     SGB_LAUNCH_CHECK("atss_candidates_kernel");
   }
-  if (d->n_max == 0) {
-    // negative batch (ppyolo_loss.py:352-357): every anchor is background, boxes and scores are zero
-    cudaMemsetAsync(assigned_box, 0, BL * 4 * sizeof(float), st);
-    cudaMemsetAsync(assigned_score, 0, BL * sizeof(float), st);
-    atss_fill_kernel<<<grid, 256, 0, st>>>(assigned_label, BL, d->ncls);
-    SGB_LAUNCH_CHECK("atss_fill_kernel");
-    return SGB_OK;
-  }
+  // negative batch (ppyolo_loss.py:352-357): every anchor is background, boxes and scores are zero
+  if (d->n_max == 0) return fill_background(assigned_label, d->ncls, assigned_score, assigned_box, BL, st);
   atss_resolve_kernel<<<grid, 256, 0, st>>>(*d, reg_distri, anchors, anchor_points, stride_tensor, gt_boxes, gt_labels, count, owner,
                                             assigned_label, assigned_box, assigned_score, sums);
   SGB_LAUNCH_CHECK("atss_resolve_kernel");

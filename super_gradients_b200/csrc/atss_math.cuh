@@ -1,6 +1,7 @@
-// Arithmetic of the ATSS assigner (row L2, the static assigner of PP-YOLOE recipes), host+device like pose_loss_math.cuh: the
-// kernels in atss.cu call these and the CPU suite compiles this header with g++ behind a serial driver
-// (tests/host_kernels/atss_host.cpp) to check the assignment against the reference's recorded outputs.
+// Arithmetic of the ATSS assigner (row L2, the static assigner of PP-YOLOE recipes) on top of the box arithmetic it shares with
+// the task-aligned assigners (tal_math.cuh), host+device like pose_loss_math.cuh: the kernels in atss.cu call these and the CPU
+// suite compiles this header with g++ behind a serial driver (tests/host_kernels/atss_host.cpp) to check the assignment against
+// the reference's recorded outputs.
 //
 // Reference: ATSSAssigner.forward, src/super_gradients/training/losses/ppyolo_loss.py:301-434, called by PPYoloELoss with
 // topk = 9, force_gt_matching = False and pred_bboxes given (:810-820); helpers iou_similarity :38-60 (eps 1e-10),
@@ -10,13 +11,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#ifndef SGB_HD
-#ifdef __CUDACC__
-#define SGB_HD __host__ __device__ __forceinline__
-#else
-#define SGB_HD static inline
-#endif
-#endif
+#include "tal_math.cuh"
 
 namespace sgb_atss {
 
@@ -28,18 +23,10 @@ struct Levels {
   int start[kMaxLevels + 1];  // start[n] = L
 };
 
-struct Box {
-  float x1, y1, x2, y2;
-};
-
-SGB_HD Box load_box(const float* p) { return Box{p[0], p[1], p[2], p[3]}; }
-
-SGB_HD float iou(const Box& g, const Box& p, float eps) {
-  const float ov = fmaxf(fminf(g.x2, p.x2) - fmaxf(g.x1, p.x1), 0.f) * fmaxf(fminf(g.y2, p.y2) - fmaxf(g.y1, p.y1), 0.f);
-  const float a1 = fmaxf(g.x2 - g.x1, 0.f) * fmaxf(g.y2 - g.y1, 0.f);
-  const float a2 = fmaxf(p.x2 - p.x1, 0.f) * fmaxf(p.y2 - p.y1, 0.f);
-  return ov / (a1 + a2 - ov + eps);
-}
+using sgb_tal::Box;
+using sgb_tal::decode_box;
+using sgb_tal::iou;
+using sgb_tal::load_box;
 
 SGB_HD float center_x(const Box& b) { return (b.x1 + b.x2) / 2.f; }
 SGB_HD float center_y(const Box& b) { return (b.y1 + b.y2) / 2.f; }
@@ -50,11 +37,7 @@ SGB_HD float center_distance(const Box& g, const Box& a) {
   return sqrtf(dx * dx + dy * dy);
 }
 
-// check_points_inside_bboxes: min(l, t, r, b) > 1e-9
-SGB_HD bool center_inside(const Box& a, const Box& g) {
-  const float cx = center_x(a), cy = center_y(a);
-  return fminf(fminf(cx - g.x1, cy - g.y1), fminf(g.x2 - cx, g.y2 - cy)) > 1e-9f;
-}
+SGB_HD bool center_inside(const Box& a, const Box& g) { return sgb_tal::inside_gt(center_x(a), center_y(a), g); }
 
 // mean + unbiased standard deviation of the candidates' IoUs (torch accumulates the variance in double)
 SGB_HD float iou_threshold(const float* v, int n) {
@@ -65,24 +48,6 @@ SGB_HD float iou_threshold(const float* v, int n) {
   for (int i = 0; i < n; ++i) q += ((double)v[i] - mean) * ((double)v[i] - mean);
   const float sd = n > 1 ? (float)sqrt(q / (n - 1)) : NAN;  // torch.std of one element is NaN: nothing is selected
   return (float)mean + sd;
-}
-
-// PPYoloELoss._bbox_decode for one anchor, in pixels: softmax-expectation distances (stride units) around the anchor point
-SGB_HD Box decode_box(const float* z, int bins, float ax, float ay, float stride) {
-  float d[4];
-  for (int s = 0; s < 4; ++s) {
-    float mx = -INFINITY;
-    for (int b = 0; b < bins; ++b) mx = fmaxf(mx, z[s * bins + b]);
-    float se = 0.f, sw = 0.f;
-    for (int b = 0; b < bins; ++b) {
-      const float e = expf(z[s * bins + b] - mx);
-      se += e;
-      sw += e * (float)b;
-    }
-    d[s] = sw / se;
-  }
-  const float px = ax / stride, py = ay / stride;
-  return Box{(px - d[0]) * stride, (py - d[1]) * stride, (px + d[2]) * stride, (py + d[3]) * stride};
 }
 
 // an anchor claimed by several GTs goes to the GT (padded rows included: they are zero boxes) of highest IoU with the anchor

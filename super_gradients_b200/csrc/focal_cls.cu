@@ -3,9 +3,9 @@
 // its final gradient (w_cls * grad_scale / normaliser folded in), so that the fused kernel -- measured and profiled with the
 // varifocal term every YOLO-NAS / PP-YOLOE recipe uses -- stays byte-identical.  Elementwise and HBM-bound: reads the logits and
 // the per-anchor label / score once, writes the gradient once (2 * 4 * B*L*C bytes).  The arithmetic (gamma = 2, weight not
-// detached, optional alpha_t) is sgb_pose::cls_term of pose_loss_math.cuh, shared with the pose loss and the CPU test build.
+// detached, optional alpha_t) is sgb_tal::cls_term of tal_math.cuh, shared with the pose loss and the CPU test build.
 #include "common.cuh"
-#include "pose_loss_math.cuh"
+#include "tal_math.cuh"
 
 namespace {
 
@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(256) focal_cls_kernel(SgbLossDesc d, const flo
     const int c = (int)(e - i * d.ncls);
     const float q = alabel[i] == c ? ascore[i] : 0.f;
     float loss, g;
-    sgb_pose::cls_term(1, alpha, cls[e], q, &loss, &g);
+    sgb_tal::cls_term(1, alpha, cls[e], q, &loss, &g);
     acc += loss;
     if (gcls) gcls[e] = g * d.w_cls * inv;
   }

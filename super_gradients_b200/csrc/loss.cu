@@ -11,8 +11,11 @@
 #include <math_constants.h>
 
 #include "common.cuh"
+#include "tal_math.cuh"
 
 namespace {
+
+using namespace sgb_tal;
 
 constexpr int MAXBINS = 32;  // reg_max + 1 <= 32
 
@@ -192,99 +195,23 @@ __global__ void head_grad_scatter_kernel(const float* __restrict__ g, int gC, in
   }
 }
 
-// ------------------------------------------------------------------------------------------------ shared math
-struct Box {
-  float x1, y1, x2, y2;
-};
-
-// softmax-expectation decode of one anchor: 4 distances in stride units (thread-serial version)
-__device__ __forceinline__ void decode_dist(const float* z, int nb, float (&d)[4]) {
-#pragma unroll
-  for (int s = 0; s < 4; ++s) {
-    float mx = -CUDART_INF_F;
-    for (int b = 0; b < nb; ++b) mx = fmaxf(mx, z[s * nb + b]);
-    float se = 0.f, sw = 0.f;
-    for (int b = 0; b < nb; ++b) {
-      float e = expf(z[s * nb + b] - mx);
-      se += e;
-      sw += e * (float)b;
-    }
-    d[s] = sw / se;
-  }
-}
-
-// ppyolo_loss.py:17-35 (eps = 1e-9)
-__device__ __forceinline__ float iou_similarity(const Box& g, const Box& p) {
-  float ix1 = fmaxf(g.x1, p.x1), iy1 = fmaxf(g.y1, p.y1), ix2 = fminf(g.x2, p.x2), iy2 = fminf(g.y2, p.y2);
-  float ov = fmaxf(ix2 - ix1, 0.f) * fmaxf(iy2 - iy1, 0.f);
-  float a1 = fmaxf(g.x2 - g.x1, 0.f) * fmaxf(g.y2 - g.y1, 0.f);
-  float a2 = fmaxf(p.x2 - p.x1, 0.f) * fmaxf(p.y2 - p.y1, 0.f);
-  return ov / (a1 + a2 - ov + 1e-9f);
-}
-
 // ------------------------------------------------------------------------------------------------ TAL
-// workspace layout (floats / ints), all [B][...]:
-//   pbox   [B][L][4]  decoded boxes in pixels
-//   topk   [B][n][topk] int   selected anchor index per gt (-1: none)
-//   gmax   [B][n][2]  int     float bits of max metric / max iou per gt (atomicMax)
-//   apair  [B][L][2]  float   metric, iou of the assigned (gt, anchor) pair
-//   agt    [B][L]     int     assigned gt index or -1
-struct TalWs {
-  float* pbox;
-  int* topk;
-  int* gmax;
-  float* apair;
-  int* agt;
-};
-__host__ __device__ inline int64_t tal_ws_floats(int B, int L, int n, int k) {
-  return (int64_t)B * L * 4 + (int64_t)B * n * k + (int64_t)B * n * 2 + (int64_t)B * L * 2 + (int64_t)B * L;
-}
-__host__ __device__ inline TalWs tal_ws_carve(void* ws, int B, int L, int n, int k) {
-  TalWs w;
-  float* p = reinterpret_cast<float*>(ws);
-  w.pbox = p;
-  p += (int64_t)B * L * 4;
-  w.topk = reinterpret_cast<int*>(p);
-  p += (int64_t)B * n * k;
-  w.gmax = reinterpret_cast<int*>(p);
-  p += (int64_t)B * n * 2;
-  w.apair = p;
-  p += (int64_t)B * L * 2;
-  w.agt = reinterpret_cast<int*>(p);
-  return w;
-}
-
 __global__ void tal_decode_kernel(SgbLossDesc d, const float* __restrict__ reg, const float* __restrict__ ap,
                                   const float* __restrict__ st, float* pbox) {
   const int nb = d.reg_max + 1;
   const int64_t total = (int64_t)d.B * d.L;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int l = i % d.L;
-    float dist[4];
-    decode_dist(reg + i * 4 * nb, nb, dist);
-    float s = st[l];
-    float ax = ap[l * 2] / s, ay = ap[l * 2 + 1] / s;
-    pbox[i * 4 + 0] = (ax - dist[0]) * s;
-    pbox[i * 4 + 1] = (ay - dist[1]) * s;
-    pbox[i * 4 + 2] = (ax + dist[2]) * s;
-    pbox[i * 4 + 3] = (ay + dist[3]) * s;
+    const int l = i % d.L;
+    store_box(pbox + i * 4, decode_box(reg + i * 4 * nb, nb, ap[l * 2], ap[l * 2 + 1], st[l]));
   }
 }
 
-__device__ __forceinline__ float tal_metric(const SgbLossDesc& d, float score, float iou) {
-  float a = d.alpha == 1.f ? score : powf(score, d.alpha);
-  float b = powf(iou, d.beta);
-  return a * b;
-}
-
-// one CTA per (image, gt): metric over all anchors -> iterative top-k (ties: lowest anchor index)
+// one CTA per (image, gt): metric over all anchors -> block-wide top-k
 __global__ void __launch_bounds__(256) tal_topk_kernel(SgbLossDesc d, const float* __restrict__ cls,
                                                        const float* __restrict__ ap, const float* __restrict__ gtb,
                                                        const int* __restrict__ gtl, const uint8_t* __restrict__ gtv,
-                                                       TalWs w) {
+                                                       Ws w) {
   extern __shared__ float smet[];  // [L]
-  __shared__ float sval[8];
-  __shared__ int sidx[8];
   const int bg = blockIdx.x;  // b * n_max + g
   const int b = bg / d.n_max;
   const int t = threadIdx.x;
@@ -293,108 +220,42 @@ __global__ void __launch_bounds__(256) tal_topk_kernel(SgbLossDesc d, const floa
     for (int j = t; j < d.topk; j += blockDim.x) w.topk[bg * d.topk + j] = -1;
     return;
   }
-  Box g{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
+  const Box g = load_box(gtb + bg * 4);
   const int label = gtl[bg];
   for (int l = t; l < d.L; l += blockDim.x) {
-    const float* pb = w.pbox + ((int64_t)b * d.L + l) * 4;
-    Box p{pb[0], pb[1], pb[2], pb[3]};
-    float iou = iou_similarity(g, p);
-    float x = cls[((int64_t)b * d.L + l) * d.ncls + label];
-    float score = 1.f / (1.f + expf(-x));
-    float ax = ap[l * 2], ay = ap[l * 2 + 1];
-    float mn = fminf(fminf(ax - g.x1, ay - g.y1), fminf(g.x2 - ax, g.y2 - ay));
-    float in_gt = mn > 1e-9f ? 1.f : 0.f;
-    smet[l] = tal_metric(d, score, iou) * in_gt;
+    const float iou_gp = iou(g, load_box(w.pbox + ((int64_t)b * d.L + l) * 4), 1e-9f);
+    const float score = sigmoid_f(cls[((int64_t)b * d.L + l) * d.ncls + label]);
+    const float in_gt = inside_gt(ap[l * 2], ap[l * 2 + 1], g) ? 1.f : 0.f;
+    smet[l] = tal_metric(d.alpha, d.beta, score, iou_gp) * in_gt;
   }
   __syncthreads();
-  for (int k = 0; k < d.topk; ++k) {
-    float bv = -1.f;
-    int bi = 0x7fffffff;
-    for (int l = t; l < d.L; l += blockDim.x) {
-      float v = smet[l];
-      if (v > bv) {  // strict: keeps the lowest index within a thread
-        bv = v;
-        bi = l;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) {
-        bv = ov;
-        bi = oi;
-      }
-    }
-    if ((t & 31) == 0) {
-      sval[t >> 5] = bv;
-      sidx[t >> 5] = bi;
-    }
-    __syncthreads();
-    if (t == 0) {
-      for (int q = 1; q < 8; ++q)
-        if (sval[q] > bv || (sval[q] == bv && sidx[q] < bi)) {
-          bv = sval[q];
-          bi = sidx[q];
-        }
-      w.topk[bg * d.topk + k] = bi;
-      if (bi < d.L) smet[bi] = -2.f;  // remove from further rounds (none left, or only NaN metrics: bi stays 0x7fffffff)
-    }
-    __syncthreads();
-  }
+  block_topk(smet, d.L, d.topk, [&](int k, int l) { w.topk[bg * d.topk + k] = l; });
 }
 
 // one thread per (image, anchor): positive mask, multi-assignment resolution, per-gt maxima
 __global__ void tal_resolve_kernel(SgbLossDesc d, const float* __restrict__ cls, const float* __restrict__ ap,
                                    const float* __restrict__ gtb, const int* __restrict__ gtl,
-                                   const uint8_t* __restrict__ gtv, TalWs w) {
+                                   const uint8_t* __restrict__ gtv, Ws w) {
   const int64_t total = (int64_t)d.B * d.L;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int l = i % d.L;
-    int b = i / d.L;
-    const float* pb = w.pbox + i * 4;
-    Box p{pb[0], pb[1], pb[2], pb[3]};
-    float ax = ap[l * 2], ay = ap[l * 2 + 1];
-    int npos = 0, first = -1;
-    float best_iou = -1.f;
-    int best_g = 0;
-    for (int g = 0; g < d.n_max; ++g) {
-      int bg = b * d.n_max + g;
-      Box gb{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
-      float iou = iou_similarity(gb, p);
-      if (iou > best_iou) {  // argmax over ALL gts (padded rows are zero boxes), first max wins
-        best_iou = iou;
-        best_g = g;
-      }
-      if (!gtv[bg]) continue;
-      bool in_topk = false;
-      for (int k = 0; k < d.topk; ++k) in_topk |= (w.topk[bg * d.topk + k] == l);
-      if (!in_topk) continue;
-      float mn = fminf(fminf(ax - gb.x1, ay - gb.y1), fminf(gb.x2 - ax, gb.y2 - ay));
-      if (!(mn > 1e-9f)) continue;
-      if (npos == 0) first = g;
-      ++npos;
-    }
-    int ag = -1;
-    if (npos == 1) ag = first;
-    else if (npos > 1) ag = best_g;
+    const int l = i % d.L, b = i / d.L, g0 = b * d.n_max;
+    const Box p = load_box(w.pbox + i * 4);
+    float met, iou_ag;
+    const int ag = resolve_anchor(
+        l, ap[l * 2], ap[l * 2 + 1], d.n_max, d.topk, gtb + g0 * 4, gtv + g0, w.topk + g0 * d.topk, d.alpha, d.beta,
+        [&](int, const Box& gb) { return iou(gb, p, 1e-9f); }, [&](int g) { return sigmoid_f(cls[i * d.ncls + gtl[g0 + g]]); }, &met,
+        &iou_ag);
     w.agt[i] = ag;
-    float met = 0.f, iou = 0.f;
-    if (ag >= 0) {
-      int bg = b * d.n_max + ag;
-      Box gb{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
-      iou = iou_similarity(gb, p);
-      float x = cls[i * d.ncls + gtl[bg]];
-      met = tal_metric(d, 1.f / (1.f + expf(-x)), iou);
-      atomicMax(&w.gmax[bg * 2 + 0], __float_as_int(met));
-      atomicMax(&w.gmax[bg * 2 + 1], __float_as_int(iou));
-    }
     w.apair[i * 2 + 0] = met;
-    w.apair[i * 2 + 1] = iou;
+    w.apair[i * 2 + 1] = iou_ag;
+    if (ag >= 0) {  // metric and iou are non-negative: their float bit patterns order like ints
+      atomicMax(&w.gmax[(g0 + ag) * 2 + 0], __float_as_int(met));
+      atomicMax(&w.gmax[(g0 + ag) * 2 + 1], __float_as_int(iou_ag));
+    }
   }
 }
 
-__global__ void tal_finish_kernel(SgbLossDesc d, const float* __restrict__ gtb, const int* __restrict__ gtl, TalWs w,
+__global__ void tal_finish_kernel(SgbLossDesc d, const float* __restrict__ gtb, const int* __restrict__ gtl, Ws w,
                                   int* alabel, float* abox, float* ascore, double* sums) {
   const int64_t total = (int64_t)d.B * d.L;
   float local = 0.f;
@@ -403,16 +264,12 @@ __global__ void tal_finish_kernel(SgbLossDesc d, const float* __restrict__ gtb, 
     int ag = w.agt[i];
     int bg = b * d.n_max + (ag >= 0 ? ag : 0);
     // the reference gathers gt 0's box for unassigned anchors (argmax of an all-zero column)
-    abox[i * 4 + 0] = gtb[bg * 4 + 0];
-    abox[i * 4 + 1] = gtb[bg * 4 + 1];
-    abox[i * 4 + 2] = gtb[bg * 4 + 2];
-    abox[i * 4 + 3] = gtb[bg * 4 + 3];
+    store_box(abox + i * 4, load_box(gtb + bg * 4));
     float sc = 0.f;
     int lab = d.ncls;
     if (ag >= 0) {
       lab = gtl[bg];
-      float mm = __int_as_float(w.gmax[bg * 2 + 0]), mi = __int_as_float(w.gmax[bg * 2 + 1]);
-      sc = w.apair[i * 2] / (mm + 1e-9f) * mi;
+      sc = assigned_score(w.apair[i * 2], __int_as_float(w.gmax[bg * 2 + 0]), __int_as_float(w.gmax[bg * 2 + 1]));
     }
     alabel[i] = lab;
     ascore[i] = sc;
@@ -484,79 +341,8 @@ __global__ void __launch_bounds__(256) loss_kernel(SgbLossDesc d, const float* _
       pside[sd] = prob;
       dist[sd] = warp_sum(prob * (float)lane);
     }
-    const float x1 = ax - dist[0], y1 = ay - dist[1], x2 = ax + dist[2], y2 = ay + dist[3];
-    // GIoU / CIoU forward + gradient wrt (x1, y1, x2, y2)   (computed redundantly by all lanes)
-    float ix1 = fmaxf(x1, gx1), iy1 = fmaxf(y1, gy1), ix2 = fminf(x2, gx2), iy2 = fminf(y2, gy2);
-    float wi = fmaxf(ix2 - ix1, 0.f), hi = fmaxf(iy2 - iy1, 0.f);
-    float ov = wi * hi;
-    float a1 = (x2 - x1) * (y2 - y1), a2 = (gx2 - gx1) * (gy2 - gy1);
     float liou, gb[4];
-    if (d.iou_type == 0) {
-      const float eps = 1e-10f;
-      float un = a1 + a2 - ov + eps;
-      float iou = ov / un;
-      float cx1 = fminf(x1, gx1), cy1 = fminf(y1, gy1), cx2 = fmaxf(x2, gx2), cy2 = fmaxf(y2, gy2);
-      float cw = cx2 - cx1, chh = cy2 - cy1;
-      float ac = cw * chh + eps;
-      liou = 1.f - (iou - (ac - un) / ac);  // = 2 - iou - un/ac
-      // partial derivatives
-      float dov[4], da1[4], dac[4];
-      bool pos = wi > 0.f && hi > 0.f;
-      dov[0] = (pos && x1 > gx1) ? -hi : 0.f;
-      dov[1] = (pos && y1 > gy1) ? -wi : 0.f;
-      dov[2] = (pos && x2 < gx2) ? hi : 0.f;
-      dov[3] = (pos && y2 < gy2) ? wi : 0.f;
-      da1[0] = -(y2 - y1);
-      da1[1] = -(x2 - x1);
-      da1[2] = (y2 - y1);
-      da1[3] = (x2 - x1);
-      dac[0] = x1 < gx1 ? -chh : 0.f;
-      dac[1] = y1 < gy1 ? -cw : 0.f;
-      dac[2] = x2 > gx2 ? chh : 0.f;
-      dac[3] = y2 > gy2 ? cw : 0.f;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        float dun = da1[k] - dov[k];
-        float diou = (dov[k] * un - ov * dun) / (un * un);
-        float dr = (dun * ac - un * dac[k]) / (ac * ac);
-        gb[k] = -diou - dr;
-      }
-    } else {
-      // CIoU (functional.py:82-133 with CIoULoss eps = 1e-10): (1 - iou) + rho2 / (cw^2 + ch^2 + eps) + v * alpha,
-      // alpha = v / max((1 - iou) + v, eps) is detached.
-      const float eps = 1e-10f;
-      float un = a1 + a2 - ov + eps;
-      float iou = ov / un;
-      float cw = fmaxf(x2, gx2) - fminf(x1, gx1), chh = fmaxf(y2, gy2) - fminf(y1, gy1);
-      float c2 = cw * cw + chh * chh + eps;
-      float dxc = (x1 + x2) * 0.5f - (gx1 + gx2) * 0.5f, dyc = (y1 + y2) * 0.5f - (gy1 + gy2) * 0.5f;
-      float rho2 = dxc * dxc + dyc * dyc;
-      float w1 = x2 - x1, h1 = y2 - y1, w2 = gx2 - gx1, h2 = gy2 - gy1;
-      const float k4pi2 = 4.f / (CUDART_PI_F * CUDART_PI_F);
-      float at = atanf(w2 / h2) - atanf(w1 / h1);
-      float v = k4pi2 * at * at;
-      float alpha = v / fmaxf((1.f - iou) + v, eps);
-      liou = (1.f - iou) + rho2 / c2 + v * alpha;
-      bool pos = wi > 0.f && hi > 0.f;
-      float dov[4] = {(pos && x1 > gx1) ? -hi : 0.f, (pos && y1 > gy1) ? -wi : 0.f, (pos && x2 < gx2) ? hi : 0.f,
-                      (pos && y2 < gy2) ? wi : 0.f};
-      float da1[4] = {-h1, -w1, h1, w1};
-      float dcw[4] = {x1 < gx1 ? -1.f : 0.f, 0.f, x2 > gx2 ? 1.f : 0.f, 0.f};
-      float dch[4] = {0.f, y1 < gy1 ? -1.f : 0.f, 0.f, y2 > gy2 ? 1.f : 0.f};
-      float drho[4] = {dxc, dyc, dxc, dyc};  // d rho2 / d coord = 2 * d * 0.5
-      float den = w1 * w1 + h1 * h1;
-      float dat_w = -h1 / den, dat_h = w1 / den;  // d at / d w1, d at / d h1
-      float dw1[4] = {-1.f, 0.f, 1.f, 0.f}, dh1[4] = {0.f, -1.f, 0.f, 1.f};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        float dun = da1[k] - dov[k];
-        float diou = (dov[k] * un - ov * dun) / (un * un);
-        float dc2 = 2.f * cw * dcw[k] + 2.f * chh * dch[k];
-        float dterm = (drho[k] * c2 - rho2 * dc2) / (c2 * c2);
-        float dv = k4pi2 * 2.f * at * (dat_w * dw1[k] + dat_h * dh1[k]);
-        gb[k] = -diou + dterm + alpha * dv;
-      }
-    }
+    iou_loss_grad(d.iou_type, ax - dist[0], ay - dist[1], ax + dist[2], ay + dist[3], gx1, gy1, gx2, gy2, &liou, gb);
     // ---- DFL
     float tgt[4] = {ax - gx1, ay - gy1, gx2 - ax, gy2 - ay};
     float ldfl = 0.f;
@@ -565,9 +351,7 @@ __global__ void __launch_bounds__(256) loss_kernel(SgbLossDesc d, const float* _
     const float sgn[4] = {-1.f, -1.f, 1.f, 1.f};
 #pragma unroll
     for (int sd = 0; sd < 4; ++sd) {
-      float tcl = fminf(fmaxf(tgt[sd], 0.f), (float)d.reg_max - 0.01f);
-      int tl = (int)tcl;  // trunc == floor (non-negative)
-      float wl = (float)(tl + 1) - tcl, wr = 1.f - wl;
+      const auto [tl, wl, wr] = dfl_target(tgt[sd], d.reg_max);
       float p = pside[sd];
       float lp = lane < nb ? logf(fmaxf(p, 1e-38f)) : 0.f;
       float ce = 0.f;
@@ -600,10 +384,6 @@ __global__ void __launch_bounds__(256) loss_kernel(SgbLossDesc d, const float* _
   }
 }
 
-__global__ void fill_i32_kernel(int* p, int64_t n, int v) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
-}
-
 __global__ void loss_finalize_kernel(SgbLossDesc d, const double* sums, float* out) {
   double nrm = sums[3] < 1.0 ? 1.0 : sums[3];
   float c = (float)(d.w_cls * sums[0] / nrm), i = (float)(d.w_iou * sums[1] / nrm), f = (float)(d.w_dfl * sums[2] / nrm);
@@ -623,6 +403,25 @@ int check_loss(const SgbLossDesc* d) {
 }
 
 }  // namespace
+
+namespace sgb_tal {
+
+__global__ void fill_background_kernel(int* label, int value, float* score, int64_t n) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    label[i] = value;
+    score[i] = 0.f;
+  }
+}
+
+int fill_background(int* label, int value, float* score, float* box, int64_t n, cudaStream_t st) {
+  if (box) cudaMemsetAsync(box, 0, n * 4 * sizeof(float), st);
+  const int grid = (int)((n + 255) / 256 > 132 * 8 ? 132 * 8 : (n + 255) / 256);
+  fill_background_kernel<<<grid, 256, 0, st>>>(label, value, score, n);
+  SGB_LAUNCH_CHECK("fill_background_kernel");
+  return SGB_OK;
+}
+
+}  // namespace sgb_tal
 
 extern "C" int sgb_dfl_decode(const sgb_bf16* reg, int reg_pitch, const sgb_bf16* cls, int cls_pitch, int N, int Hf,
                               int Wf, int L, int anchor_base, int ncls, int reg_max, float stride, float cell_offset,
@@ -692,7 +491,7 @@ extern "C" int sgb_head_grad_scatter(const float* grad, int gC, int N, int HW, i
 
 extern "C" int64_t sgb_tal_workspace_bytes(const SgbLossDesc* d) {
   if (!d) return 0;
-  return tal_ws_floats(d->B, d->L, d->n_max > 0 ? d->n_max : 1, d->topk) * 4 + 256;
+  return ws_floats(d->B, d->L, d->n_max > 0 ? d->n_max : 1, d->topk) * 4 + 256;
 }
 
 extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, const float* reg_distri,
@@ -708,7 +507,7 @@ extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, con
   SGB_REQUIRE(d->n_max > 0 ? (gt_boxes && gt_labels && gt_valid) : true, "gt pointers");
   cudaStream_t st = (cudaStream_t)stream;
   const int nmax = d->n_max > 0 ? d->n_max : 1;
-  TalWs w = tal_ws_carve(workspace, d->B, d->L, nmax, d->topk);
+  Ws w = ws_carve(workspace, d->B, d->L, nmax, d->topk);
   const int64_t BL = (int64_t)d->B * d->L;
   int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
   tal_decode_kernel<<<grid, 256, 0, st>>>(*d, reg_distri, anchor_points, stride_tensor, w.pbox);
@@ -725,14 +524,8 @@ extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, con
                                                         w);
     SGB_LAUNCH_CHECK("tal_topk_kernel");
   }
-  if (d->n_max == 0) {
-    // negative batch: every anchor is background (ppyolo_loss.py:499-503)
-    cudaMemsetAsync(assigned_box, 0, BL * 4 * sizeof(float), st);
-    cudaMemsetAsync(assigned_score, 0, BL * sizeof(float), st);
-    fill_i32_kernel<<<grid, 256, 0, st>>>(assigned_label, BL, d->ncls);
-    SGB_LAUNCH_CHECK("fill_i32_kernel");
-    return SGB_OK;
-  }
+  // negative batch: every anchor is background (ppyolo_loss.py:499-503)
+  if (d->n_max == 0) return fill_background(assigned_label, d->ncls, assigned_score, assigned_box, BL, st);
   tal_resolve_kernel<<<grid, 256, 0, st>>>(*d, cls_logits, anchor_points, gt_boxes, gt_labels, gt_valid, w);
   SGB_LAUNCH_CHECK("tal_resolve_kernel");
   tal_finish_kernel<<<grid, 256, 0, st>>>(*d, gt_boxes, gt_labels, w, assigned_label, assigned_box, assigned_score,

@@ -1,48 +1,20 @@
 // YoloNASPoseLoss (row L7) on the GPU: OKS-aware task-aligned assigner with crowd handling, then ONE kernel that computes
 // the five loss terms (person focal/BCE, GIoU/CIoU, DFL, joint-visibility BCE/focal, OKS keypoint regression) and their
 // final gradients.  HBM / latency bound: B*L anchors, 1 + 4*(reg_max+1) + 3*J floats each, read once; only the few
-// thousand positive anchors do more than the person-logit term.  The arithmetic lives in pose_loss_math.cuh (shared with
-// the CPU test harness); this file is the parallel schedule around it.
+// thousand positive anchors do more than the person-logit term.  The arithmetic lives in pose_loss_math.cuh and tal_math.cuh
+// (shared with the detection losses and the CPU test harness); this file is the parallel schedule around it.
 //
 // Reference: src/super_gradients/training/losses/yolo_nas_pose_loss.py (see pose_loss_math.cuh for line numbers).
-#include <math_constants.h>
-
 #include "common.cuh"
 #include "pose_loss_math.cuh"
 
 namespace {
 
 using namespace sgb_pose;
+using namespace sgb_tal;
 
 constexpr int MAXBINS = 32;  // reg_max + 1 <= 32
 constexpr int MAXJ = 64;
-
-// workspace (same shape as the detection assigner's): pbox [B][L][4] f32, topk [B][n][k] i32, gmax [B][n][2] i32 (float
-// bits: max metric / max iou per gt), apair [B][L][2] f32 (metric, iou of the assigned pair), agt [B][L] i32
-struct PoseWs {
-  float* pbox;
-  int* topk;
-  int* gmax;
-  float* apair;
-  int* agt;
-};
-inline int64_t ws_floats(int B, int L, int n, int k) {
-  return (int64_t)B * L * 4 + (int64_t)B * n * k + (int64_t)B * n * 2 + (int64_t)B * L * 2 + (int64_t)B * L;
-}
-inline PoseWs ws_carve(void* ws, int B, int L, int n, int k) {
-  PoseWs w;
-  float* p = reinterpret_cast<float*>(ws);
-  w.pbox = p;
-  p += (int64_t)B * L * 4;
-  w.topk = reinterpret_cast<int*>(p);
-  p += (int64_t)B * n * k;
-  w.gmax = reinterpret_cast<int*>(p);
-  p += (int64_t)B * n * 2;
-  w.apair = p;
-  p += (int64_t)B * L * 2;
-  w.agt = reinterpret_cast<int*>(p);
-  return w;
-}
 
 __global__ void pose_decode_kernel(SgbPoseLossDesc d, const float* __restrict__ reg, const float* __restrict__ ap,
                                    const float* __restrict__ st, float* pbox) {
@@ -59,10 +31,8 @@ __global__ void __launch_bounds__(256) pose_topk_kernel(SgbPoseLossDesc d, const
                                                         const float* __restrict__ pose, const float* __restrict__ ap,
                                                         const float* __restrict__ gtb, const float* __restrict__ gtp,
                                                         const uint8_t* __restrict__ gtv, const float* __restrict__ sigmas,
-                                                        PoseWs w) {
+                                                        Ws w) {
   extern __shared__ float smet[];  // [L]
-  __shared__ float sval[8];
-  __shared__ int sidx[8];
   __shared__ float sgp[MAXJ * 3];
   __shared__ float ssig[MAXJ];
   const int bg = blockIdx.x;  // b * n_max + g
@@ -76,56 +46,21 @@ __global__ void __launch_bounds__(256) pose_topk_kernel(SgbPoseLossDesc d, const
   for (int j = t; j < d.J * 3; j += blockDim.x) sgp[j] = gtp[(int64_t)bg * d.J * 3 + j];
   for (int j = t; j < d.J; j += blockDim.x) ssig[j] = sigmas[j];
   __syncthreads();
-  const PBox g{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
+  const Box g = load_box(gtb + bg * 4);
   for (int l = t; l < d.L; l += blockDim.x) {
     const int64_t i = (int64_t)b * d.L + l;
-    const PBox p{w.pbox[i * 4 + 0], w.pbox[i * 4 + 1], w.pbox[i * 4 + 2], w.pbox[i * 4 + 3]};
-    const float iou = pair_iou(d, g, sgp, p, pose + i * d.J * 2, ssig);
+    const float iou = pair_iou(d, g, sgp, load_box(w.pbox + i * 4), pose + i * d.J * 2, ssig);
     const float in_gt = inside_gt(ap[l * 2], ap[l * 2 + 1], g) ? 1.f : 0.f;
     smet[l] = tal_metric(d, sigmoid_f(cls[i]), iou) * in_gt;
   }
   __syncthreads();
-  for (int k = 0; k < d.topk; ++k) {
-    float bv = -1.f;
-    int bi = 0x7fffffff;
-    for (int l = t; l < d.L; l += blockDim.x) {
-      float v = smet[l];
-      if (v > bv) {  // strict: keeps the lowest index within a thread
-        bv = v;
-        bi = l;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) {
-        bv = ov;
-        bi = oi;
-      }
-    }
-    if ((t & 31) == 0) {
-      sval[t >> 5] = bv;
-      sidx[t >> 5] = bi;
-    }
-    __syncthreads();
-    if (t == 0) {
-      for (int q = 1; q < 8; ++q)
-        if (sval[q] > bv || (sval[q] == bv && sidx[q] < bi)) {
-          bv = sval[q];
-          bi = sidx[q];
-        }
-      w.topk[bg * d.topk + k] = bi;
-      if (bi < d.L) smet[bi] = -2.f;  // remove from further rounds (none left, or only NaN metrics: bi stays 0x7fffffff)
-    }
-    __syncthreads();
-  }
+  block_topk(smet, d.L, d.topk, [&](int k, int l) { w.topk[bg * d.topk + k] = l; });
 }
 
 __global__ void pose_resolve_kernel(SgbPoseLossDesc d, const float* __restrict__ cls, const float* __restrict__ pose,
                                     const float* __restrict__ ap, const float* __restrict__ gtb,
                                     const float* __restrict__ gtp, const uint8_t* __restrict__ gtv,
-                                    const float* __restrict__ sigmas, PoseWs w) {
+                                    const float* __restrict__ sigmas, Ws w) {
   const int64_t total = (int64_t)d.B * d.L;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int l = i % d.L, b = i / d.L;
@@ -143,7 +78,7 @@ __global__ void pose_resolve_kernel(SgbPoseLossDesc d, const float* __restrict__
   }
 }
 
-__global__ void pose_finish_kernel(SgbPoseLossDesc d, const uint8_t* __restrict__ gtc, PoseWs w, int* assigned_gt,
+__global__ void pose_finish_kernel(SgbPoseLossDesc d, const uint8_t* __restrict__ gtc, Ws w, int* assigned_gt,
                                    float* assigned_score, double* sums) {
   const int64_t total = (int64_t)d.B * d.L;
   float lsum = 0.f, lpos = 0.f;
@@ -165,13 +100,6 @@ __global__ void pose_finish_kernel(SgbPoseLossDesc d, const uint8_t* __restrict_
   if ((threadIdx.x & 31) == 0) {
     if (lsum != 0.f) atomicAdd(&sums[3], (double)lsum);
     if (lpos != 0.f) atomicAdd(&sums[6], (double)lpos);
-  }
-}
-
-__global__ void fill_assign_kernel(int* assigned_gt, float* assigned_score, int64_t n) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    assigned_gt[i] = -1;
-    assigned_score[i] = 0.f;
   }
 }
 
@@ -247,12 +175,9 @@ extern "C" int sgb_pose_tal_assign(const SgbPoseLossDesc* d, const float* cls_lo
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t BL = (int64_t)d->B * d->L;
   const int grid = (int)((BL + 255) / 256 > 132 * 8 ? 132 * 8 : (BL + 255) / 256);
-  if (d->n_max == 0) {  // no targets in the batch: every anchor is background (:118-131)
-    fill_assign_kernel<<<grid, 256, 0, st>>>(assigned_gt, assigned_score, BL);
-    SGB_LAUNCH_CHECK("fill_assign_kernel");
-    return SGB_OK;
-  }
-  PoseWs w = ws_carve(workspace, d->B, d->L, d->n_max, d->topk);
+  // no targets in the batch: every anchor is background (:118-131)
+  if (d->n_max == 0) return fill_background(assigned_gt, -1, assigned_score, nullptr, BL, st);
+  Ws w = ws_carve(workspace, d->B, d->L, d->n_max, d->topk);
   pose_decode_kernel<<<grid, 256, 0, st>>>(*d, reg_distri, anchor_points, stride_tensor, w.pbox);
   SGB_LAUNCH_CHECK("pose_decode_kernel");
   const size_t smem = (size_t)d->L * sizeof(float);

@@ -1,49 +1,35 @@
-// Per-pair / per-anchor arithmetic of YoloNASPoseLoss (row L7), written once as host+device inline functions: the CUDA
-// kernels in pose_loss.cu call them per thread, and the CPU test-suite compiles this very header with g++
-// (tests/host_kernels/pose_loss_host.cpp) to check the arithmetic against the oracle without a GPU.
+// Pose-specific arithmetic of YoloNASPoseLoss (row L7): OKS, the assigner's pair IoU, the keypoint terms of one anchor and the
+// finalisation, written once as host+device inline functions on top of the task-aligned assigner and box-loss arithmetic shared
+// with the detection losses (tal_math.cuh).  The CUDA kernels in pose_loss.cu call them per thread, and the CPU test-suite
+// compiles this very header with g++ (tests/host_kernels/pose_loss_host.cpp) to check the arithmetic against the oracle without
+// a GPU.
 //
 // Reference: src/super_gradients/training/losses/yolo_nas_pose_loss.py
 //   batch_pose_oks :45-74, YoloNASPoseTaskAlignedAssigner.forward :77-244, YoloNASPoseLoss.forward :404-494,
-//   _keypoint_loss :514-564, _bbox_loss :574-639, _df_loss :496-512, _focal_loss :663-682;
-//   GIoU: training/losses/ppyolo_loss.py:564-638, CIoU: training/losses/functional.py:82-133.
+//   _keypoint_loss :514-564, _bbox_loss :574-639, _df_loss :496-512, _focal_loss :663-682.
 #pragma once
 #include <math.h>
 #include <stdint.h>
 
 #include "sgb200.h"
-
-#ifdef __CUDACC__
-#define SGB_HD __host__ __device__ __forceinline__
-#else
-#define SGB_HD static inline
-#endif
+#include "tal_math.cuh"
 
 namespace sgb_pose {
 
-struct PBox {
-  float x1, y1, x2, y2;
-};
+using sgb_tal::Box;
+using PBox = sgb_tal::Box;
+using sgb_tal::cls_term;
+using sgb_tal::inside_gt;
+using sgb_tal::sigmoid_f;
 
 // unnormalised partial sums of one anchor: cls, iou, dfl, pose_cls, pose_reg
 struct AnchorSums {
   float cls, iou, dfl, pcls, preg;
 };
 
-SGB_HD float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
-SGB_HD float softplus_f(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }  // = BCE-with-logits(x, 0)
-
-// batch_iou_similarity (ppyolo_loss.py:17-35, eps = 1e-9)
-SGB_HD float iou_similarity(const PBox& g, const PBox& p) {
-  float ix1 = fmaxf(g.x1, p.x1), iy1 = fmaxf(g.y1, p.y1), ix2 = fminf(g.x2, p.x2), iy2 = fminf(g.y2, p.y2);
-  float ov = fmaxf(ix2 - ix1, 0.f) * fmaxf(iy2 - iy1, 0.f);
-  float a1 = fmaxf(g.x2 - g.x1, 0.f) * fmaxf(g.y2 - g.y1, 0.f);
-  float a2 = fmaxf(p.x2 - p.x1, 0.f) * fmaxf(p.y2 - p.y1, 0.f);
-  return ov / (a1 + a2 - ov + 1e-9f);
-}
-
 // batch_pose_oks (:45-74): mean over the VISIBLE joints of exp(-d^2 / (2 sigma)^2 / (0.53 * box area + eps) / 2).
 // gpose [J][3] = (x, y, visibility), ppose [J][2] in pixels.
-SGB_HD float oks(const float* gpose, const float* ppose, const float* sigmas, int J, const PBox& g) {
+SGB_HD float oks(const float* gpose, const float* ppose, const float* sigmas, int J, const Box& g) {
   const float area = (g.x2 - g.x1) * (g.y2 - g.y1) * 0.53f;
   float num = 0.f, nvis = 0.f;
   for (int j = 0; j < J; ++j) {
@@ -58,80 +44,34 @@ SGB_HD float oks(const float* gpose, const float* ppose, const float* sigmas, in
 }
 
 // the "iou" of the assigner: box IoU, times the pose OKS when assigner_multiply_by_pose_oks (:140-147)
-SGB_HD float pair_iou(const SgbPoseLossDesc& d, const PBox& g, const float* gpose, const PBox& p, const float* ppose,
+SGB_HD float pair_iou(const SgbPoseLossDesc& d, const Box& g, const float* gpose, const Box& p, const float* ppose,
                       const float* sigmas) {
-  float iou = iou_similarity(g, p);
+  float iou = sgb_tal::iou(g, p, 1e-9f);
   if (d.multiply_by_oks) iou *= oks(gpose, ppose, sigmas, d.J, g);
   return iou;
 }
 
-SGB_HD float tal_metric(const SgbPoseLossDesc& d, float score, float iou) {
-  float a = d.alpha == 1.f ? score : powf(score, d.alpha);
-  return a * powf(iou, d.beta);
-}
+SGB_HD float tal_metric(const SgbPoseLossDesc& d, float score, float iou) { return sgb_tal::tal_metric(d.alpha, d.beta, score, iou); }
 
-SGB_HD bool inside_gt(float ax, float ay, const PBox& g) {  // check_points_inside_bboxes, eps = 1e-9
-  return fminf(fminf(ax - g.x1, ay - g.y1), fminf(g.x2 - ax, g.y2 - ay)) > 1e-9f;
-}
-
-// softmax-expectation decode of one anchor's 4 x nb DFL logits -> xyxy in pixels
+// softmax-expectation decode of one anchor's 4 x nb DFL logits -> xyxy in pixels at out
 SGB_HD void decode_box(const float* z, int nb, float apx, float apy, float s, float* out) {
-  float dist[4];
-  for (int sd = 0; sd < 4; ++sd) {
-    float mx = -INFINITY;
-    for (int b = 0; b < nb; ++b) mx = fmaxf(mx, z[sd * nb + b]);
-    float se = 0.f, sw = 0.f;
-    for (int b = 0; b < nb; ++b) {
-      float e = expf(z[sd * nb + b] - mx);
-      se += e;
-      sw += e * (float)b;
-    }
-    dist[sd] = sw / se;
-  }
-  const float ax = apx / s, ay = apy / s;
-  out[0] = (ax - dist[0]) * s;
-  out[1] = (ay - dist[1]) * s;
-  out[2] = (ax + dist[2]) * s;
-  out[3] = (ay + dist[3]) * s;
+  sgb_tal::store_box(out, sgb_tal::decode_box(z, nb, apx, apy, s));
 }
 
-// One anchor of the assigner after the per-gt top-k selection (:166-206): which gt (if any) the anchor is assigned to,
-// and the (metric, iou) of that pair.  topk [B][n_max][topk] holds the selected anchor indices per gt (-1 = none).
+// One anchor of the assigner after the per-gt top-k selection (:166-206): the shared multi-assignment rule with the pose pair
+// IoU (box IoU, times OKS when multiply_by_oks) and the person score.  topk [B][n_max][topk] holds the selected anchor indices
+// per gt (-1 = none).
 SGB_HD void resolve_anchor(const SgbPoseLossDesc& d, int b, int l, const float* pbox, const float* cls, const float* pose,
                            const float* ap, const float* gtb, const float* gtp, const uint8_t* gtv, const float* sigmas,
                            const int* topk, int* ag_out, float* met_out, float* iou_out) {
   const int64_t i = (int64_t)b * d.L + l;
-  const PBox p{pbox[i * 4 + 0], pbox[i * 4 + 1], pbox[i * 4 + 2], pbox[i * 4 + 3]};
+  const int g0 = b * d.n_max;
+  const Box p = sgb_tal::load_box(pbox + i * 4);
   const float* pp = pose + i * d.J * 2;
-  const float ax = ap[l * 2], ay = ap[l * 2 + 1];
-  int npos = 0, first = -1, best_g = 0;
-  float best_iou = -1.f;
-  for (int g = 0; g < d.n_max; ++g) {
-    const int64_t bg = (int64_t)b * d.n_max + g;
-    const PBox gb{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
-    const float iou = pair_iou(d, gb, gtp + bg * d.J * 3, p, pp, sigmas);
-    if (iou > best_iou) {  // argmax over ALL gt rows (padded rows are zero boxes), first maximum wins
-      best_iou = iou;
-      best_g = g;
-    }
-    if (!gtv[bg]) continue;
-    bool in_topk = false;
-    for (int k = 0; k < d.topk; ++k) in_topk |= (topk[bg * d.topk + k] == l);
-    if (!in_topk || !inside_gt(ax, ay, gb)) continue;
-    if (npos == 0) first = g;
-    ++npos;
-  }
-  const int ag = npos == 1 ? first : (npos > 1 ? best_g : -1);
-  float met = 0.f, iou = 0.f;
-  if (ag >= 0) {
-    const int64_t bg = (int64_t)b * d.n_max + ag;
-    const PBox gb{gtb[bg * 4 + 0], gtb[bg * 4 + 1], gtb[bg * 4 + 2], gtb[bg * 4 + 3]};
-    iou = pair_iou(d, gb, gtp + bg * d.J * 3, p, pp, sigmas);
-    met = tal_metric(d, sigmoid_f(cls[i]), iou);
-  }
-  *ag_out = ag;
-  *met_out = met;
-  *iou_out = iou;
+  *ag_out = sgb_tal::resolve_anchor(
+      l, ap[l * 2], ap[l * 2 + 1], d.n_max, d.topk, gtb + (int64_t)g0 * 4, gtv + g0, topk + (int64_t)g0 * d.topk, d.alpha, d.beta,
+      [&](int g, const Box& gb) { return pair_iou(d, gb, gtp + (int64_t)(g0 + g) * d.J * 3, p, pp, sigmas); },
+      [&](int) { return sigmoid_f(cls[i]); }, met_out, iou_out);
 }
 
 // assigned score of one anchor (:208-222) and whether it is a positive for the box / keypoint terms (crowd targets keep
@@ -141,74 +81,7 @@ SGB_HD void finish_anchor(int ag, float met, float gt_max_metric, float gt_max_i
   *score = 0.f;
   if (ag >= 0 && !crowd) {
     *pos_gt = ag;
-    *score = met / (gt_max_metric + 1e-9f) * gt_max_iou;
-  }
-}
-
-// focal (gamma = 2, weight NOT detached) or plain BCE with logits against a soft / hard label q; alpha <= 0: no alpha_t
-SGB_HD void cls_term(int focal, float alpha, float x, float q, float* loss, float* grad) {
-  const float p = sigmoid_f(x);
-  const float bce = softplus_f(x) - x * q;
-  if (!focal) {
-    *loss = bce;
-    *grad = p - q;
-    return;
-  }
-  const float dq = p - q;
-  const float at = alpha > 0.f ? alpha * q + (1.f - alpha) * (1.f - q) : 1.f;
-  *loss = at * dq * dq * bce;
-  *grad = at * (2.f * dq * p * (1.f - p) * bce + dq * dq * dq);
-}
-
-// GIoU (iou_type 0) or CIoU (1) loss of a predicted box against a target, and its gradient w.r.t. (x1, y1, x2, y2)
-SGB_HD void iou_loss_grad(int iou_type, float x1, float y1, float x2, float y2, float gx1, float gy1, float gx2, float gy2,
-                          float* loss, float* gb) {
-  const float eps = 1e-10f;
-  const float ix1 = fmaxf(x1, gx1), iy1 = fmaxf(y1, gy1), ix2 = fminf(x2, gx2), iy2 = fminf(y2, gy2);
-  const float wi = fmaxf(ix2 - ix1, 0.f), hi = fmaxf(iy2 - iy1, 0.f);
-  const float ov = wi * hi;
-  const float w1 = x2 - x1, h1 = y2 - y1, w2 = gx2 - gx1, h2 = gy2 - gy1;
-  const float un = w1 * h1 + w2 * h2 - ov + eps;
-  const float iou = ov / un;
-  const bool pos = wi > 0.f && hi > 0.f;
-  const float dov[4] = {(pos && x1 > gx1) ? -hi : 0.f, (pos && y1 > gy1) ? -wi : 0.f, (pos && x2 < gx2) ? hi : 0.f,
-                        (pos && y2 < gy2) ? wi : 0.f};
-  const float da1[4] = {-h1, -w1, h1, w1};
-  const float cw = fmaxf(x2, gx2) - fminf(x1, gx1), chh = fmaxf(y2, gy2) - fminf(y1, gy1);
-  if (iou_type == 0) {
-    const float ac = cw * chh + eps;
-    *loss = 1.f - (iou - (ac - un) / ac);
-    const float dac[4] = {x1 < gx1 ? -chh : 0.f, y1 < gy1 ? -cw : 0.f, x2 > gx2 ? chh : 0.f, y2 > gy2 ? cw : 0.f};
-    for (int k = 0; k < 4; ++k) {
-      float dun = da1[k] - dov[k];
-      float diou = (dov[k] * un - ov * dun) / (un * un);
-      float dr = (dun * ac - un * dac[k]) / (ac * ac);
-      gb[k] = -diou - dr;
-    }
-    return;
-  }
-  // (1 - iou) + rho2 / (cw^2 + ch^2 + eps) + v * alpha, alpha = v / max((1 - iou) + v, eps) detached
-  const float c2 = cw * cw + chh * chh + eps;
-  const float dxc = (x1 + x2) * 0.5f - (gx1 + gx2) * 0.5f, dyc = (y1 + y2) * 0.5f - (gy1 + gy2) * 0.5f;
-  const float rho2 = dxc * dxc + dyc * dyc;
-  const float k4pi2 = 4.f / (3.14159265358979323846f * 3.14159265358979323846f);
-  const float at = atanf(w2 / h2) - atanf(w1 / h1);
-  const float v = k4pi2 * at * at;
-  const float alpha = v / fmaxf((1.f - iou) + v, eps);
-  *loss = (1.f - iou) + rho2 / c2 + v * alpha;
-  const float dcw[4] = {x1 < gx1 ? -1.f : 0.f, 0.f, x2 > gx2 ? 1.f : 0.f, 0.f};
-  const float dch[4] = {0.f, y1 < gy1 ? -1.f : 0.f, 0.f, y2 > gy2 ? 1.f : 0.f};
-  const float drho[4] = {dxc, dyc, dxc, dyc};  // d rho2 / d coord = 2 * d * 0.5
-  const float den = w1 * w1 + h1 * h1;
-  const float dat_w = -h1 / den, dat_h = w1 / den;  // d at / d w1, d at / d h1
-  const float dw1[4] = {-1.f, 0.f, 1.f, 0.f}, dh1[4] = {0.f, -1.f, 0.f, 1.f};
-  for (int k = 0; k < 4; ++k) {
-    float dun = da1[k] - dov[k];
-    float diou = (dov[k] * un - ov * dun) / (un * un);
-    float dc2 = 2.f * cw * dcw[k] + 2.f * chh * dch[k];
-    float dterm = (drho[k] * c2 - rho2 * dc2) / (c2 * c2);
-    float dv = k4pi2 * 2.f * at * (dat_w * dw1[k] + dat_h * dh1[k]);
-    gb[k] = -diou + dterm + alpha * dv;
+    *score = sgb_tal::assigned_score(met, gt_max_metric, gt_max_iou);
   }
 }
 
@@ -251,14 +124,12 @@ SGB_HD void anchor_loss(const SgbPoseLossDesc& d, int b, int l, const float* cls
     dist[sd] = e_w / e_sum;
   }
   float liou, gb[4];
-  iou_loss_grad(d.iou_type, ax - dist[0], ay - dist[1], ax + dist[2], ay + dist[3], gx1, gy1, gx2, gy2, &liou, gb);
+  sgb_tal::iou_loss_grad(d.iou_type, ax - dist[0], ay - dist[1], ax + dist[2], ay + dist[3], gx1, gy1, gx2, gy2, &liou, gb);
   const float tgt[4] = {ax - gx1, ay - gy1, gx2 - ax, gy2 - ay};
   const float sgn[4] = {-1.f, -1.f, 1.f, 1.f};  // x1 = ax - d0, y1 = ay - d1, x2 = ax + d2, y2 = ay + d3
   float ldfl = 0.f;
   for (int sd = 0; sd < 4; ++sd) {
-    const float tcl = fminf(fmaxf(tgt[sd], 0.f), (float)d.reg_max - 0.01f);
-    const int tl = (int)tcl;  // trunc == floor (non-negative)
-    const float wl = (float)(tl + 1) - tcl, wr = 1.f - wl;
+    const auto [tl, wl, wr] = sgb_tal::dfl_target(tgt[sd], d.reg_max);
     for (int k = 0; k < nb; ++k) {
       const float p = expf(z[sd * nb + k] - mx[sd]) / se[sd];
       if (k == tl) ldfl -= logf(fmaxf(p, 1e-38f)) * wl;
