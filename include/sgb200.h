@@ -734,6 +734,32 @@ int sgb_classify_rows(const void* logits, int64_t N, int32_t C, int64_t row_stri
  *   adamw hp[8] = {lr, beta1, beta2, eps, weight_decay, 1-beta1^t, 1-beta2^t, grad_scale}   (torch.optim semantics) */
 int sgb_sgd_step(float* p, const float* g, float* mom, int64_t n, const float* hp, void* stream);
 int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream);
+/* The other optimizers of the reference's registry (common/object_names.py:143-152), one launch per weight-decay range.  hp is ONE
+ * device float32 row in the layout of csrc/optim_math.cuh (ADAM_*, RMS_*, RTF_*, LION_*), grad_scale included; every element is
+ * computed op for op as the reference's single-tensor CPU step, each op rounded to float32 on its own (FMA exactly where torch's CPU
+ * kernels fuse: add with alpha, addcmul, lerp).  n == 0 is a no-op; a NULL required pointer is refused with SGB_E_INVALID.
+ *   adam        torch.optim.Adam, L2-coupled decay g + wd * p (training/params.py:90; torch/optim/adam.py _single_tensor_adam)
+ *   rmsprop     torch.optim.RMSprop: momentum_buffer only with momentum > 0, grad_avg only when centered, else NULL
+ *               (training/params.py:92; torch/optim/rmsprop.py _single_tensor_rmsprop)
+ *   rmsprop_tf  RMSpropTF: eps inside the sqrt, TF update order, decoupled_decay, lr_in_momentum
+ *               (training/utils/optimizers/rmsprop_tf.py:89-153)
+ *   lion        Lion: p *= 1 - lr * wd; p -= lr * sign(b1 * m + (1 - b1) * g); m = b2 * m + (1 - b2) * g  (lion.py:57-79) */
+int sgb_adam_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream);
+int sgb_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg, int64_t n, const float* hp, void* stream);
+int sgb_rmsprop_tf_step(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg, int64_t n, const float* hp, void* stream);
+int sgb_lion_step(float* p, const float* g, float* m, int64_t n, const float* hp, void* stream);
+/* Lamb (training/utils/optimizers/lamb.py:123-216) over EVERY live parameter at once: chunks is a device int64 [nchunk][4] table
+ * {start, len, first chunk of its tensor, chunks of its tensor} (a chunk lies inside one parameter tensor); hp is two LAMB_* rows,
+ * row 0 for elements before n_decay, row 1 after; partials is device float64 [3 * nchunk].
+ *   sgb_lamb_grad_sqnorm  (1 launch)  partials[c] = sum over chunk c of (g * grad_scale)^2
+ *   sgb_lamb_step         (2 launches) clip = max(||g|| / max_grad_norm, 1) over all chunks; m / v update with grad_averaging and
+ *                         bias_correction; update = m^ / (sqrt(v) / sqrt(bc2) + eps) + wd * p into `update`; per tensor
+ *                         trust = ||p|| / ||update|| with the reference's zero-norm branches and trust_clip (1 where the row does
+ *                         not adapt); p -= lr * trust * update.
+ * Every sum is float64 in a fixed order with no atomics: two runs of one step are bit-identical.  No host synchronisation. */
+int sgb_lamb_grad_sqnorm(const float* g, const int64_t* chunks, int32_t nchunk, const float* hp, double* partials, void* stream);
+int sgb_lamb_step(float* p, const float* g, float* m, float* v, float* update, int64_t n_decay, const int64_t* chunks, int32_t nchunk,
+                  const float* hp, double* partials, void* stream);
 /* ema = ema * (*decay) + (1 - *decay) * p   (training/utils/ema.py:126-142) */
 int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream);
 

@@ -1,0 +1,210 @@
+// Adam, RMSprop, RMSpropTF, Lion and Lamb over the flat fp32 parameter / gradient buffers (training/flat_state.py).  The
+// per-element arithmetic is optim_math.cuh; hyper-parameters are read from DEVICE memory so a CUDA-graph-captured step follows
+// the host's schedule.  The elementwise optimizers are one grid-stride pass per weight-decay range, like adamw_kernel.
+//
+// Lamb needs a global gradient norm and per-tensor norms of p and of the update.  Every reduction runs over a chunk table
+// (fused_optimizers.lamb_chunk_table: {start, len, first chunk of its tensor, chunks of its tensor}; a chunk lies inside one
+// tensor), one CTA per chunk, in float64, in a fixed order (thread-strided partial sums, then a fixed shuffle / shared-memory
+// tree), and without atomics, so two runs of one step are bit-identical:
+//   1. lamb_sqnorm_kernel   partials[c]             = sum over chunk c of (g * gs)^2
+//   2. lamb_update_kernel   every CTA adds partials[0 .. nchunk) itself -> clip; m / v update -> update buffer;
+//                           partials[nchunk + 2c .. +1] = sum over chunk c of p^2 and update^2
+//   3. lamb_apply_kernel    every CTA adds its tensor's chunk sums -> trust ratio; p -= lr * trust * update
+#include "common.cuh"
+#include "optim_math.cuh"
+
+namespace {
+
+using namespace sgb_optim;
+
+constexpr int TPB = 256;
+
+inline int grid_for(int64_t work, int per_cta = TPB * 4, int max_ctas = 132 * 8) {
+  int64_t g = (work + per_cta - 1) / per_cta;
+  if (g > max_ctas) g = max_ctas;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+__global__ void __launch_bounds__(TPB) adam_kernel(float* p, const float* g, float* m, float* v, int64_t n, const float* hp) {
+  float h[ADAM_HP];
+#pragma unroll
+  for (int j = 0; j < ADAM_HP; ++j) h[j] = hp[j];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float pi = p[i], mi = m[i], vi = v[i];
+    adam(pi, g[i], mi, vi, h);
+    p[i] = pi;
+    m[i] = mi;
+    v[i] = vi;
+  }
+}
+
+// TF: RMSpropTF when true, torch.optim.RMSprop otherwise; buf / ga may be null (no momentum / not centered)
+template <bool TF>
+__global__ void __launch_bounds__(TPB) rmsprop_kernel(float* p, const float* g, float* sa, float* buf, float* ga, int64_t n, const float* hp) {
+  float h[RMS_HP];
+#pragma unroll
+  for (int j = 0; j < RMS_HP; ++j) h[j] = hp[j];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float pi = p[i], si = sa[i], bi = buf ? buf[i] : 0.f, gi = ga ? ga[i] : 0.f;
+    if (TF) rmsprop_tf(pi, g[i], si, &bi, &gi, h);
+    else rmsprop(pi, g[i], si, &bi, &gi, h);
+    p[i] = pi;
+    sa[i] = si;
+    if (buf) buf[i] = bi;
+    if (ga) ga[i] = gi;
+  }
+}
+
+__global__ void __launch_bounds__(TPB) lion_kernel(float* p, const float* g, float* m, int64_t n, const float* hp) {
+  float h[LION_HP];
+#pragma unroll
+  for (int j = 0; j < LION_HP; ++j) h[j] = hp[j];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float pi = p[i], mi = m[i];
+    lion(pi, g[i], mi, h);
+    p[i] = pi;
+    m[i] = mi;
+  }
+}
+
+// block-wide sum of two doubles in a fixed order; the result is valid in every thread
+__device__ __forceinline__ double2 block_sum2(double a, double b) {
+  __shared__ double2 part[TPB / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_down_sync(0xffffffffu, a, o);
+    b += __shfl_down_sync(0xffffffffu, b, o);
+  }
+  const int w = threadIdx.x >> 5;
+  __syncthreads();  // part[] may still be read by a previous call
+  if ((threadIdx.x & 31) == 0) part[w] = make_double2(a, b);
+  __syncthreads();
+  double2 s = part[0];
+#pragma unroll
+  for (int k = 1; k < TPB / 32; ++k) {
+    s.x += part[k].x;
+    s.y += part[k].y;
+  }
+  return s;
+}
+
+__global__ void __launch_bounds__(TPB) lamb_sqnorm_kernel(const float* __restrict__ g, const int64_t* __restrict__ chunks, const float* __restrict__ hp,
+                                                          double* __restrict__ partials) {
+  const int64_t a = chunks[4 * blockIdx.x], b = a + chunks[4 * blockIdx.x + 1];
+  const float gs = hp[LAMB_GS];
+  double s = 0.0;
+  for (int64_t i = a + threadIdx.x; i < b; i += TPB) {
+    const double x = mul(g[i], gs);
+    s += x * x;
+  }
+  const double2 t = block_sum2(s, 0.0);
+  if (threadIdx.x == 0) partials[blockIdx.x] = t.x;
+}
+
+__global__ void __launch_bounds__(TPB) lamb_update_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                                          float* __restrict__ u, int64_t n_decay, const int64_t* __restrict__ chunks, int32_t nchunk,
+                                                          const float* __restrict__ hp, double* __restrict__ partials) {
+  double s = 0.0;
+  for (int c = threadIdx.x; c < nchunk; c += TPB) s += partials[c];
+  const double total = block_sum2(s, 0.0).x;
+  const int64_t a = chunks[4 * blockIdx.x], b = a + chunks[4 * blockIdx.x + 1];
+  const float* row = hp + (a < n_decay ? 0 : LAMB_HP);
+  float h[LAMB_HP];
+#pragma unroll
+  for (int j = 0; j < LAMB_HP; ++j) h[j] = row[j];
+  const float clip = lamb_clip(total, h);
+  double sp = 0.0, su = 0.0;
+  for (int64_t i = a + threadIdx.x; i < b; i += TPB) {
+    float mi = m[i], vi = v[i];
+    const float pi = p[i];
+    const float ui = lamb_update(pi, g[i], mi, vi, clip, h);
+    m[i] = mi;
+    v[i] = vi;
+    u[i] = ui;
+    sp += (double)pi * pi;
+    su += (double)ui * ui;
+  }
+  const double2 t = block_sum2(sp, su);
+  if (threadIdx.x == 0) {
+    partials[nchunk + 2 * blockIdx.x] = t.x;
+    partials[nchunk + 2 * blockIdx.x + 1] = t.y;
+  }
+}
+
+__global__ void __launch_bounds__(TPB) lamb_apply_kernel(float* __restrict__ p, const float* __restrict__ u, int64_t n_decay, const int64_t* __restrict__ chunks,
+                                                         int32_t nchunk, const float* __restrict__ hp, const double* __restrict__ partials) {
+  const int64_t a = chunks[4 * blockIdx.x], b = a + chunks[4 * blockIdx.x + 1];
+  const int64_t first = chunks[4 * blockIdx.x + 2], cnt = chunks[4 * blockIdx.x + 3];
+  const double* pu = partials + nchunk;
+  double sp = 0.0, su = 0.0;
+  for (int64_t k = first + threadIdx.x; k < first + cnt; k += TPB) {
+    sp += pu[2 * k];
+    su += pu[2 * k + 1];
+  }
+  const double2 t = block_sum2(sp, su);
+  const float* row = hp + (a < n_decay ? 0 : LAMB_HP);
+  float h[LAMB_HP];
+#pragma unroll
+  for (int j = 0; j < LAMB_HP; ++j) h[j] = row[j];
+  const float trust = lamb_trust(t.x, t.y, h);
+  for (int64_t i = a + threadIdx.x; i < b; i += TPB) p[i] = lamb_apply(p[i], u[i], trust, h);
+}
+
+}  // namespace
+
+// ================================================================================================== C ABI
+extern "C" int sgb_adam_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && m && v && hp, "null pointer");
+  SGB_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return SGB_OK;
+  adam_kernel<<<grid_for(n), TPB, 0, (cudaStream_t)stream>>>(p, g, m, v, n, hp);
+  SGB_LAUNCH_CHECK("adam_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && square_avg && hp, "null pointer");
+  SGB_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return SGB_OK;
+  rmsprop_kernel<false><<<grid_for(n), TPB, 0, (cudaStream_t)stream>>>(p, g, square_avg, momentum_buffer, grad_avg, n, hp);
+  SGB_LAUNCH_CHECK("rmsprop_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_rmsprop_tf_step(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && square_avg && hp, "null pointer");
+  SGB_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return SGB_OK;
+  rmsprop_kernel<true><<<grid_for(n), TPB, 0, (cudaStream_t)stream>>>(p, g, square_avg, momentum_buffer, grad_avg, n, hp);
+  SGB_LAUNCH_CHECK("rmsprop_tf_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_lion_step(float* p, const float* g, float* m, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && m && hp, "null pointer");
+  SGB_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return SGB_OK;
+  lion_kernel<<<grid_for(n), TPB, 0, (cudaStream_t)stream>>>(p, g, m, n, hp);
+  SGB_LAUNCH_CHECK("lion_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_lamb_grad_sqnorm(const float* g, const int64_t* chunks, int32_t nchunk, const float* hp, double* partials, void* stream) {
+  SGB_REQUIRE(g && chunks && hp && partials, "null pointer");
+  SGB_REQUIRE(nchunk >= 1, "nchunk must be >= 1");
+  lamb_sqnorm_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(g, chunks, hp, partials);
+  SGB_LAUNCH_CHECK("lamb_sqnorm_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_lamb_step(float* p, const float* g, float* m, float* v, float* update, int64_t n_decay, const int64_t* chunks, int32_t nchunk, const float* hp,
+                             double* partials, void* stream) {
+  SGB_REQUIRE(p && g && m && v && update && chunks && hp && partials, "null pointer");
+  SGB_REQUIRE(nchunk >= 1 && n_decay >= 0, "nchunk must be >= 1 and n_decay >= 0");
+  lamb_update_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(p, g, m, v, update, n_decay, chunks, nchunk, hp, partials);
+  SGB_LAUNCH_CHECK("lamb_update_kernel");
+  lamb_apply_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(p, update, n_decay, chunks, nchunk, hp, partials);
+  SGB_LAUNCH_CHECK("lamb_apply_kernel");
+  return SGB_OK;
+}

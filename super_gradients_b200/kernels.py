@@ -1101,6 +1101,38 @@ def adamw_step(p, g, m, v, hp):
     _timed("sgb_adamw_step", _ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), _ptr(hp), _stream())
 
 
+def adam_step(p, g, m, v, hp):
+    """torch.optim.Adam (L2-coupled decay) over one weight-decay range; hp: device float32 row (csrc/optim_math.cuh ADAM_*)."""
+    _timed("sgb_adam_step", _ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), _ptr(hp), _stream())
+
+
+def rmsprop_step(p, g, square_avg, buf, grad_avg, hp):
+    """torch.optim.RMSprop; buf with momentum > 0 and grad_avg when centered, else None; hp: RMS_* row."""
+    _timed("sgb_rmsprop_step", _ptr(p), _ptr(g), _ptr(square_avg), _ptr(buf), _ptr(grad_avg), p.numel(), _ptr(hp), _stream())
+
+
+def rmsprop_tf_step(p, g, square_avg, buf, grad_avg, hp):
+    """RMSpropTF (eps inside the sqrt, square_avg from ones); buf / grad_avg as rmsprop_step; hp: RTF_* row."""
+    _timed("sgb_rmsprop_tf_step", _ptr(p), _ptr(g), _ptr(square_avg), _ptr(buf), _ptr(grad_avg), p.numel(), _ptr(hp), _stream())
+
+
+def lion_step(p, g, m, hp):
+    """Lion; hp: LION_* row."""
+    _timed("sgb_lion_step", _ptr(p), _ptr(g), _ptr(m), p.numel(), _ptr(hp), _stream())
+
+
+def lamb_grad_sqnorm(g, chunks, hp, partials):
+    """Lamb, launch 1: partials[c] = sum of (g * grad_scale)^2 over chunk c of the chunk table (device int64 [nchunk, 4],
+    fused_optimizers.lamb_chunk_table) in float64; hp: device float32 [2, LAMB_HP]."""
+    _timed("sgb_lamb_grad_sqnorm", _ptr(g), _ptr(chunks), int(chunks.shape[0]), _ptr(hp), _ptr(partials), _stream())
+
+
+def lamb_step(p, g, m, v, update, n_decay, chunks, hp, partials):
+    """Lamb, launches 2 and 3 over every live parameter: the m / v update into `update` with per-chunk sums of p^2 and update^2,
+    then the trust-scaled apply.  Elements before n_decay use hp row 0, the others row 1.  partials: float64 [3 * nchunk]."""
+    _timed("sgb_lamb_step", _ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(update), int(n_decay), _ptr(chunks), int(chunks.shape[0]), _ptr(hp), _ptr(partials), _stream())
+
+
 def ema_update(ema, p, decay_dev):
     _timed("sgb_ema_update", _ptr(ema), _ptr(p), p.numel(), _ptr(decay_dev), _stream())
 

@@ -25,6 +25,7 @@ from .. import functional as SF
 from .. import kernels as K
 from ..common.factories import LossesFactory, MetricsFactory, _fuzzy
 from ..common.registry import CALLBACKS
+from . import fused_optimizers as FO
 from .flat_state import FlatState
 from .utils.callbacks import CallbackHandler, PhaseContext
 from .utils.weight_averaging_utils import ModelWeightAveraging
@@ -76,8 +77,8 @@ DEFAULT_TRAINING_PARAMS = {
 
 AVERAGE_MODEL_FILENAME = "average_model.pth"
 
-# defaults merged under user optimizer_params (reference: training/params.py:84-90)
-OPTIMIZER_DEFAULTS = {"SGD": {"weight_decay": 1e-4, "momentum": 0.9}, "Adam": {"weight_decay": 1e-4}, "AdamW": {"weight_decay": 1e-2}}
+# defaults merged under user optimizer_params (reference: training/params.py:84-94)
+OPTIMIZER_DEFAULTS = {"SGD": {"weight_decay": 1e-4, "momentum": 0.9}, "AdamW": {"weight_decay": 1e-2}, **FO.REGISTRY_DEFAULTS}
 
 
 def _match_metric_name(wanted: str, available: list) -> str:
@@ -231,16 +232,20 @@ class TrainStep:
         op = {**OPTIMIZER_DEFAULTS.get(optimizer, {}), **dict(optimizer_params)}
         self.op = op
         f = self.flat
+        self.fused = None  # Adam, RMSprop, RMSpropTF, Lion, Lamb (training/fused_optimizers.py)
         if optimizer == "SGD":
             self.state = [torch.zeros_like(f.params)]
             self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, 5), dtype=torch.float32).pin_memory()
-        elif optimizer in ("AdamW", "Adam"):
-            if optimizer == "Adam":
-                raise NotImplementedError("Adam (L2-coupled) is not implemented; use AdamW or SGD")
+        elif optimizer == "AdamW":
             self.state = [torch.zeros_like(f.params), torch.zeros_like(f.params)]
             self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, 8), dtype=torch.float32).pin_memory()
+        elif optimizer in FO.NAMES:
+            self.op, wd = FO.resolve(optimizer, optimizer_params, zero_wd_on_bias_and_bn)
+            self.fused = FO.FlatOptimizer(optimizer, self.op, wd, f)
+            self.state = self.fused.state
+            self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, self.fused.hp_len), dtype=torch.float32).pin_memory()
         else:
-            raise NotImplementedError(f"optimizer {optimizer} has no fused kernel (SGD, AdamW are implemented)")
+            raise NotImplementedError(f"optimizer {optimizer} has no fused kernel (SGD, Adam, AdamW, RMSprop, RMSpropTF, Lamb, Lion are implemented)")
         self.hp = torch.zeros_like(self.hp_host[0], device=self.device)
         self._slot, self._slot_events = 0, [None] * self.STAGING_SLOTS
         self.ema_on = ema
@@ -265,7 +270,7 @@ class TrainStep:
 
     # -------------------------------------------------------------------------------------------- host-side schedule
     def set_hyper_params(self, lr: float, ema_decay_value: Optional[float] = None):
-        """Writes this step's LR (and Adam bias corrections) to the device; must precede run()."""
+        """Writes this step's LR (and bias corrections / derived step sizes) to the device; must precede run()."""
         t = self.opt_steps + 1
         # the reference's _backward_step (sg_trainer.py:611-644) calls loss.backward() on every micro-batch without dividing
         # by batch_accumulate: accumulated gradients are SUMMED; only the data-parallel average (DDP) divides
@@ -282,6 +287,8 @@ class TrainStep:
             mu, nes = float(self.op.get("momentum", 0.0)), float(bool(self.op.get("nesterov", False)))
             hp_host[0] = torch.tensor([lr, mu, wd, gs, nes])
             hp_host[1] = torch.tensor([lr, mu, 0.0, gs, nes])
+        elif self.fused is not None:
+            hp_host.copy_(torch.tensor(self.fused.rows(lr, t, gs), dtype=torch.float32))
         else:
             b1, b2 = self.op.get("betas", (0.9, 0.999))
             eps = float(self.op.get("eps", 1e-8))
@@ -360,7 +367,9 @@ class TrainStep:
         """Optimizer + EMA over the (already reduced) flat gradients; no collective in here."""
         f = self.flat
         nd = f.n_decay
-        ranges = [(0, nd, 0), (nd, f.n_live, 1)]
+        ranges = [(0, nd, 0), (nd, f.n_live, 1)] if self.fused is None else []
+        if self.fused is not None:
+            self.fused.step(f, self.hp)
         for a, b, row in ranges:
             if b <= a:
                 continue
@@ -766,7 +775,7 @@ class Trainer:
         osd = ckpt.get("optimizer_state_dict") or {}
         if osd:
             saved_order, mine_order = list(osd.get("flat_order", [])), [n for n, _ in st.flat.order]
-            if osd.get("name") != st.opt_name or sorted(saved_order) != sorted(mine_order):
+            if osd.get("name") != st.opt_name or sorted(saved_order) != sorted(mine_order) or len(osd["state"]) != len(st.state):
                 raise ValueError("the checkpoint's optimizer state does not belong to this model / optimizer")
             if saved_order == mine_order:
                 for mine, saved in zip(st.state, osd["state"]):
