@@ -41,14 +41,15 @@ __device__ __forceinline__ unsigned okey(float f) { return sgb_nms::score_key(f)
 
 __device__ __forceinline__ bool passes(float s, float thr, int incl) { return incl ? (s >= thr) : (s > thr); }
 
-// argmax pre-pass for single-label mode (torch.max(dim=1): first maximal index)
+// argmax pre-pass for single-label mode (torch.max(dim=1): first maximal index, or the first NaN and its index -- a NaN maximum
+// then fails the threshold and drops the anchor)
 __global__ void nms_argmax_kernel(const float* __restrict__ scores, int64_t rows, int C, float* conf, int* lab) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows; i += (int64_t)gridDim.x * blockDim.x) {
     float best = scores[i * C];
     int bi = 0;
-    for (int c = 1; c < C; ++c) {
+    for (int c = 1; c < C && best == best; ++c) {
       float v = scores[i * C + c];
-      if (v > best) {
+      if (v > best || v != v) {
         best = v;
         bi = c;
       }
@@ -464,20 +465,20 @@ __global__ void __launch_bounds__(NT, 1) nms_kernel(SgbNmsDesc d, const float* _
     S.bx[3][i] = y2;
     S.label[i] = label;
     S.sflat[i] = f;
-    lmax = fmaxf(lmax, fmaxf(fmaxf(x1, y1), fmaxf(x2, y2)));
+    lmax = sgb_nms::max_nan(lmax, sgb_nms::max_nan(sgb_nms::max_nan(x1, y1), sgb_nms::max_nan(x2, y2)));
   }
   // batched_nms path selection exactly as torchvision (CPU): coordinate trick iff boxes.numel() <= 4000
   const bool trick = !d.class_agnostic && (4 * nsel <= 4000);
   trick_flag = trick;
   if (trick) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
+    for (int o = 16; o > 0; o >>= 1) lmax = sgb_nms::max_nan(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
     float* wmax = reinterpret_cast<float*>(S.hist);
     if (lane == 0) wmax[warp] = lmax;
     __syncthreads();
     if (t == 0) {
       float m = -INFINITY;
-      for (int w = 0; w < 32; ++w) m = fmaxf(m, wmax[w]);
+      for (int w = 0; w < 32; ++w) m = sgb_nms::max_nan(m, wmax[w]);
       S.fmisc[1] = sgb_nms::offset_step(m);  // max_coordinate + 1
     }
     __syncthreads();

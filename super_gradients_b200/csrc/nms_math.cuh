@@ -54,6 +54,10 @@ SGB_HD float area(float x1, float y1, float x2, float y2) { return mul_rn(sub_rn
 SGB_HD float offset_step(float max_coordinate) { return add_rn(max_coordinate, 1.0f); }
 SGB_HD float label_offset(int label, float step) { return mul_rn((float)label, step); }
 
+// Maximum that propagates NaN, as torch's boxes.max() does (fmaxf drops it): a NaN coordinate makes max_coordinate, and with it
+// every offset box, NaN, so that no IoU exceeds the threshold and nothing is suppressed.
+SGB_HD float max_nan(float a, float b) { return (a > b || a != a) ? a : b; }
+
 // Box i (kept, earlier in score order) suppresses box j: inter / (areas[i] + areas[j] - inter) > iou_threshold.
 SGB_HD bool suppresses(float ix1, float iy1, float ix2, float iy2, float ia, float jx1, float jy1, float jx2, float jy2, float ja, double thr) {
   const float xx1 = fmaxf(ix1, jx1), yy1 = fmaxf(iy1, jy1);
@@ -65,6 +69,7 @@ SGB_HD bool suppresses(float ix1, float iy1, float ix2, float iy2, float ia, flo
 }
 
 // Sort key of a candidate: ascending key = score descending, then list position ascending (torchvision's stable descending sort).
+// -0.0 and +0.0 compare equal in that sort, so both map to the key of +0.0 and fall back to list position.
 SGB_HD uint32_t score_key(float f) {
   uint32_t b;
 #ifdef __CUDA_ARCH__
@@ -77,6 +82,7 @@ SGB_HD uint32_t score_key(float f) {
   u.f = f;
   b = u.u;
 #endif
+  if (b == 0x80000000u) b = 0u;
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 SGB_HD uint64_t sort_key(float score, uint32_t pos) { return ((uint64_t)(~score_key(score)) << 32) | pos; }

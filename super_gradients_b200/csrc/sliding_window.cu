@@ -156,17 +156,17 @@ __global__ void __launch_bounds__(NT, 1) sw_compact_kernel(const float* __restri
       w.score[o + j] = row[4];
       w.label[o + j] = ok ? lab : 0;
       w.keys[(int64_t)b * np2 + j] = sgb_nms::sort_key(row[4], (uint32_t)j);
-      lmax = fmaxf(lmax, fmaxf(fmaxf(x1, y1), fmaxf(x2, y2)));
+      lmax = sgb_nms::max_nan(lmax, sgb_nms::max_nan(sgb_nms::max_nan(x1, y1), sgb_nms::max_nan(x2, y2)));
     }
   }
   for (int j = n + tid; j < np2; j += NT) w.keys[(int64_t)b * np2 + j] = ~0ull;
 #pragma unroll
-  for (int s = 16; s > 0; s >>= 1) lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, s));
+  for (int s = 16; s > 0; s >>= 1) lmax = sgb_nms::max_nan(lmax, __shfl_xor_sync(0xffffffffu, lmax, s));
   if (lane == 0) s_max[warp] = lmax;
   __syncthreads();
   if (tid == 0) {
     float m = -INFINITY;
-    for (int i = 0; i < 32; ++i) m = fmaxf(m, s_max[i]);
+    for (int i = 0; i < 32; ++i) m = sgb_nms::max_nan(m, s_max[i]);
     int* co = w.cls_off + (int64_t)b * (ncls + 1);
     int acc = 0;
     for (int c = 0; c < ncls; ++c) {

@@ -19,7 +19,7 @@ extern "C" int merge_nms_host(const float* boxes, const float* scores, const int
   std::sort(keys.begin(), keys.end());
   const bool trick = 4 * (int64_t)n <= 4000;
   float m = -INFINITY;
-  for (int j = 0; j < 4 * n; ++j) m = fmaxf(m, boxes[j]);
+  for (int j = 0; j < 4 * n; ++j) m = sgb_nms::max_nan(m, boxes[j]);
   const float step = sgb_nms::offset_step(m);
   std::vector<float> bx(4 * n), area(n);
   std::vector<int> lab(n), pos(n);

@@ -7,6 +7,7 @@ import pytest
 import torch
 import torchvision
 
+import nms_cases
 from sliding_window_cases import GOLDEN_CASES, StubDetector, golden_inputs, merge_case, merge_nms_host
 from super_gradients_b200.training.models.detection_models.sliding_window_detection_forward_wrapper import chunk_tiles, tile_origins
 
@@ -33,6 +34,20 @@ def test_merge_tied_scores_per_class_path_same_set():
     got = merge_nms_host(boxes, scores, labels, 0.6)
     assert torch.equal(got.sort().values, ref.sort().values)
     assert torch.equal(scores[got], scores[ref])
+
+
+@pytest.mark.parametrize("name", nms_cases.MERGE_EDGE_CASES)
+def test_merge_nan_boxes_and_signed_zero(name):
+    """NaN / +-inf boxes (a NaN maximum makes every offset box NaN on the coordinate-trick path: nothing is suppressed) and +-0.0
+    scores (equal in torchvision's sort: list order decides)."""
+    for b in range(2):
+        boxes, scores, labels = nms_cases.merge_candidates(name, b)
+        ref = torchvision.ops.batched_nms(boxes, scores, labels, 0.5)
+        got = merge_nms_host(boxes, scores, labels, 0.5)
+        if boxes.shape[0] > 1000:  # the per-class path: torchvision's final sort is not stable
+            assert torch.equal(got.sort().values, ref.sort().values) and torch.equal(scores[got], scores[ref])
+        else:
+            assert torch.equal(got, ref), (name, b)
 
 
 def test_tile_origin_edge_cases():
