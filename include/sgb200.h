@@ -760,6 +760,19 @@ int sgb_lion_step(float* p, const float* g, float* m, int64_t n, const float* hp
 int sgb_lamb_grad_sqnorm(const float* g, const int64_t* chunks, int32_t nchunk, const float* hp, double* partials, void* stream);
 int sgb_lamb_step(float* p, const float* g, float* m, float* v, float* update, int64_t n_decay, const int64_t* chunks, int32_t nchunk,
                   const float* hp, double* partials, void* stream);
+/* clip_grad_norm (sg_trainer.py:634-636; the value is refused when <= 0, :1416-1417): torch.nn.utils.clip_grad_norm_ with norm
+ * type 2 over every live gradient, run once per optimisation step after the all-reduce and before the optimizer.  The gradients
+ * are not rewritten: the coefficient is folded into the optimizer's grad_scale, column gs_col of both hp rows (hp is the
+ * optimizer's device table of two hp_len-wide rows: sgd 3, adamw 7, ADAM_GS / RMS_GS / RTF_GS / LION_GS / LAMB_GS of
+ * csrc/optim_math.cuh).  chunks / nchunk: the chunk table of sgb_lamb_step; partials: device float64 [nchunk].
+ *   launch 1  partials[c] = sum over chunk c of (g * hp[gs_col])^2                       (the kernel of sgb_lamb_grad_sqnorm)
+ *   launch 2  one CTA: total = (float)sqrt(sum of partials, float64, fixed order);
+ *             coef = min(reciprocal(total + 1e-6) * max_norm, 1) in float32 (torch's op order; NaN stays NaN, inf gives 0);
+ *             norm_coef[0] = total, norm_coef[1] = coef; hp[gs_col] *= coef; hp[hp_len + gs_col] *= coef.
+ * No host synchronisation and no branch on the norm on the host: capturable.  max_norm <= 0 or gs_col outside [0, hp_len) is
+ * refused with SGB_E_INVALID. */
+int sgb_clip_grad_norm(const float* g, const int64_t* chunks, int32_t nchunk, float* hp, int32_t hp_len, int32_t gs_col, float max_norm, double* partials,
+                       float* norm_coef, void* stream);
 /* ema = ema * (*decay) + (1 - *decay) * p   (training/utils/ema.py:126-142) */
 int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream);
 

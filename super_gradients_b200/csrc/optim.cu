@@ -6,10 +6,12 @@
 // (fused_optimizers.lamb_chunk_table: {start, len, first chunk of its tensor, chunks of its tensor}; a chunk lies inside one
 // tensor), one CTA per chunk, in float64, in a fixed order (thread-strided partial sums, then a fixed shuffle / shared-memory
 // tree), and without atomics, so two runs of one step are bit-identical:
-//   1. lamb_sqnorm_kernel   partials[c]             = sum over chunk c of (g * gs)^2
+//   1. grad_sqnorm_kernel   partials[c]             = sum over chunk c of (g * gs)^2
 //   2. lamb_update_kernel   every CTA adds partials[0 .. nchunk) itself -> clip; m / v update -> update buffer;
 //                           partials[nchunk + 2c .. +1] = sum over chunk c of p^2 and update^2
 //   3. lamb_apply_kernel    every CTA adds its tensor's chunk sums -> trust ratio; p -= lr * trust * update
+// clip_grad_norm runs grad_sqnorm_kernel over the same table with any optimizer's grad_scale column, then clip_finalize_kernel
+// multiplies the coefficient into that column, before the optimizer's own launches.
 #include "common.cuh"
 #include "optim_math.cuh"
 
@@ -89,10 +91,12 @@ __device__ __forceinline__ double2 block_sum2(double a, double b) {
   return s;
 }
 
-__global__ void __launch_bounds__(TPB) lamb_sqnorm_kernel(const float* __restrict__ g, const int64_t* __restrict__ chunks, const float* __restrict__ hp,
+// partials[c] = sum over chunk c of (g * *gs)^2; gs points at the grad_scale column of the optimizer's row 0 (Lamb's global norm
+// and clip_grad_norm's total norm)
+__global__ void __launch_bounds__(TPB) grad_sqnorm_kernel(const float* __restrict__ g, const int64_t* __restrict__ chunks, const float* __restrict__ gs_ptr,
                                                           double* __restrict__ partials) {
   const int64_t a = chunks[4 * blockIdx.x], b = a + chunks[4 * blockIdx.x + 1];
-  const float gs = hp[LAMB_GS];
+  const float gs = *gs_ptr;
   double s = 0.0;
   for (int64_t i = a + threadIdx.x; i < b; i += TPB) {
     const double x = mul(g[i], gs);
@@ -100,6 +104,21 @@ __global__ void __launch_bounds__(TPB) lamb_sqnorm_kernel(const float* __restric
   }
   const double2 t = block_sum2(s, 0.0);
   if (threadIdx.x == 0) partials[blockIdx.x] = t.x;
+}
+
+// one CTA: adds partials[0 .. nchunk) in the order lamb_update_kernel uses -> total norm and clip coefficient (norm_coef[0], [1]);
+// the coefficient is multiplied into the grad_scale column of both rows, so every optimizer kernel reads clipped gradients
+__global__ void __launch_bounds__(TPB) clip_finalize_kernel(const double* __restrict__ partials, int32_t nchunk, float* __restrict__ hp, int32_t hp_len,
+                                                            int32_t gs_col, float max_norm, float* __restrict__ norm_coef) {
+  double s = 0.0;
+  for (int c = threadIdx.x; c < nchunk; c += TPB) s += partials[c];
+  const double total = block_sum2(s, 0.0).x;
+  if (threadIdx.x == 0) {
+    const float norm = clip_total_norm(total), coef = clip_coef(norm, max_norm);
+    norm_coef[0] = norm;
+    norm_coef[1] = coef;
+    clip_scale_rows(hp, hp_len, gs_col, coef);
+  }
 }
 
 __global__ void __launch_bounds__(TPB) lamb_update_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
@@ -193,8 +212,21 @@ extern "C" int sgb_lion_step(float* p, const float* g, float* m, int64_t n, cons
 extern "C" int sgb_lamb_grad_sqnorm(const float* g, const int64_t* chunks, int32_t nchunk, const float* hp, double* partials, void* stream) {
   SGB_REQUIRE(g && chunks && hp && partials, "null pointer");
   SGB_REQUIRE(nchunk >= 1, "nchunk must be >= 1");
-  lamb_sqnorm_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(g, chunks, hp, partials);
-  SGB_LAUNCH_CHECK("lamb_sqnorm_kernel");
+  grad_sqnorm_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(g, chunks, hp + LAMB_GS, partials);
+  SGB_LAUNCH_CHECK("grad_sqnorm_kernel");
+  return SGB_OK;
+}
+
+extern "C" int sgb_clip_grad_norm(const float* g, const int64_t* chunks, int32_t nchunk, float* hp, int32_t hp_len, int32_t gs_col, float max_norm, double* partials,
+                                  float* norm_coef, void* stream) {
+  SGB_REQUIRE(g && chunks && hp && partials && norm_coef, "null pointer");
+  SGB_REQUIRE(nchunk >= 1, "nchunk must be >= 1");
+  SGB_REQUIRE(gs_col >= 0 && gs_col < hp_len, "gs_col must index a column of the hp_len-wide rows");
+  SGB_REQUIRE(max_norm > 0.f, "max_norm must be > 0");
+  grad_sqnorm_kernel<<<nchunk, TPB, 0, (cudaStream_t)stream>>>(g, chunks, hp + gs_col, partials);
+  SGB_LAUNCH_CHECK("grad_sqnorm_kernel");
+  clip_finalize_kernel<<<1, TPB, 0, (cudaStream_t)stream>>>(partials, nchunk, hp, hp_len, gs_col, max_norm, norm_coef);
+  SGB_LAUNCH_CHECK("clip_finalize_kernel");
   return SGB_OK;
 }
 

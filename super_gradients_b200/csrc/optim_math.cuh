@@ -1,6 +1,6 @@
-// Per-element arithmetic of the flat-buffer optimizers Adam, RMSprop, RMSpropTF, Lion and Lamb, host+device: the CUDA kernels in
-// optim.cu run it per element, and the CPU suite compiles this header with g++ (-ffp-contract=off) behind a serial driver
-// (tests/host_kernels/optim_host.cpp).
+// Per-element arithmetic of the flat-buffer optimizers Adam, RMSprop, RMSpropTF, Lion and Lamb, and of clip_grad_norm's
+// coefficient, host+device: the CUDA kernels in optim.cu run it per element, and the CPU suite compiles this header with g++
+// (-ffp-contract=off) behind serial drivers (tests/host_kernels/optim_host.cpp, clip_host.cpp).
 //
 // Each function restates, op for op, the reference's single-tensor CPU step in float32 (torch.optim.Adam / RMSprop, and the
 // RMSpropTF, Lion and Lamb classes of training/utils/optimizers/).  torch's CPU kernels round as follows, and so does this header:
@@ -186,5 +186,24 @@ SGB_HD float lamb_trust(double p_sqsum, double u_sqsum, const float* hp) {
 }
 // update.mul_(trust_ratio); p.add_(update, alpha=-lr)
 SGB_HD float lamb_apply(float p, float u, float trust, const float* hp) { return fma_(mul(u, trust), hp[LAMB_NEG_LR], p); }
+
+// ---- clip_grad_norm (sg_trainer.py:634-636: torch.nn.utils.clip_grad_norm_, norm type 2)
+// total = ||g||_2 from the float64 sum of squares, rounded to float32 once, as torch's float32 norm returns it.  torch adds the
+// squares in float32: a sum beyond float32's range is an infinite norm there (so coef 0), and here too.
+SGB_HD float clip_total_norm(double grad_sqsum) {
+  const float s = (float)grad_sqsum;
+  return isinf(s) ? s : (float)sqrt(grad_sqsum);
+}
+// clip_coef = max_norm / (total_norm + 1e-6), which torch's Tensor.__rtruediv__ evaluates as reciprocal(total + 1e-6) * max_norm;
+// clamp(max=1.0) keeps NaN (a NaN gradient) and gives 0 for an infinite norm, as torch does
+SGB_HD float clip_coef(float total, float max_norm) {
+  const float c = mul(div(1.f, add(total, 1e-6f)), max_norm);
+  return c > 1.f ? 1.f : c;
+}
+// g.mul_(clip_coef) folded into the optimizer's grad_scale: column gs_col of both weight-decay rows of an hp_len-wide table
+SGB_HD void clip_scale_rows(float* hp, int hp_len, int gs_col, float coef) {
+  hp[gs_col] = mul(hp[gs_col], coef);
+  hp[hp_len + gs_col] = mul(hp[hp_len + gs_col], coef);
+}
 
 }  // namespace sgb_optim

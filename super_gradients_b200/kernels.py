@@ -1133,6 +1133,14 @@ def lamb_step(p, g, m, v, update, n_decay, chunks, hp, partials):
     _timed("sgb_lamb_step", _ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(update), int(n_decay), _ptr(chunks), int(chunks.shape[0]), _ptr(hp), _ptr(partials), _stream())
 
 
+def clip_grad_norm(g, chunks, hp, gs_col, max_norm, partials, norm_coef):
+    """clip_grad_norm_(max_norm) over the live gradients g (sg_trainer.py:634-636), folded into grad_scale: two launches, the
+    float64 per-chunk sums of (g * hp[0, gs_col])^2 into partials (float64 [nchunk]), then one CTA that writes the total norm
+    and the coefficient to norm_coef (device float32 [2]) and multiplies column gs_col of both rows of hp (device float32
+    [2, hp_len]) by the coefficient.  chunks: the chunk table of lamb_grad_sqnorm (FlatState.chunks)."""
+    _timed("sgb_clip_grad_norm", _ptr(g), _ptr(chunks), int(chunks.shape[0]), _ptr(hp), int(hp.shape[-1]), int(gs_col), float(max_norm), _ptr(partials), _ptr(norm_coef), _stream())
+
+
 def ema_update(ema, p, decay_dev):
     _timed("sgb_ema_update", _ptr(ema), _ptr(p), p.numel(), _ptr(decay_dev), _stream())
 

@@ -237,13 +237,14 @@ _SIGNATURES = {
     "sgb_lion_step": (c_int, [P, P, P, _L, P, P]),
     "sgb_lamb_grad_sqnorm": (c_int, [P, P, c_int32, P, P, P]),
     "sgb_lamb_step": (c_int, [P, P, P, P, P, _L, P, c_int32, P, P, P]),
+    "sgb_clip_grad_norm": (c_int, [P, P, c_int32, P, c_int32, c_int32, _F, P, P, P]),
     "sgb_average_snapshots": (c_int, [P, c_int32, _L, P, P]),
 }
 
 _lib = None
 
 # kernels launched by one call of each entry point (default 1); LAUNCHES[0] accumulates them (bench.py: gpu_launches)
-LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_lamb_step": 2, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_conv_wgrad_halo_launches": 0, "sgb_conv_wgrad_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
+LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_lamb_step": 2, "sgb_clip_grad_norm": 2, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_conv_wgrad_halo_launches": 0, "sgb_conv_wgrad_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
 LAUNCHES = [0]
 
 

@@ -94,6 +94,17 @@ class FlatState:
                 b.data = self.buffers[off : off + k].view(b.shape)
                 off += k
         self.buffer_names = [n for n, _ in bufs]
+        self._chunks = None
+
+    @property
+    def chunks(self) -> torch.Tensor:
+        """Device int64 chunk table over the live parameters (fused_optimizers.lamb_chunk_table), built on first use: the fixed-order
+        float64 gradient norms of Lamb and of clip_grad_norm reduce over it."""
+        if self._chunks is None:
+            from .fused_optimizers import lamb_chunk_table
+
+            self._chunks = lamb_chunk_table([p.numel() for _, p in self.order]).to(self.params.device)
+        return self._chunks
 
     def zero_grad(self):
         self.grads.zero_()

@@ -102,6 +102,10 @@ def lamb_chunk_table(numels: List[int], chunk: int = LAMB_CHUNK) -> torch.Tensor
 
 HP_LEN = {"Adam": 8, "RMSprop": 8, "RMSpropTF": 8, "Lion": 7, "Lamb": 13}
 
+# the grad_scale column of every optimizer's hyper-parameter rows (SGD and AdamW: sg_trainer.TrainStep.set_hyper_params; the others:
+# hyper_param_rows), where clip_grad_norm folds its coefficient
+GRAD_SCALE_COLUMN = {"SGD": 3, "AdamW": 7, "Adam": 7, "RMSprop": 7, "RMSpropTF": 7, "Lion": 6, "Lamb": 9}
+
 
 class FlatOptimizer:
     """The state and the per-step launches of one of NAMES over a FlatState: one kernel per weight-decay range for the elementwise
@@ -114,7 +118,7 @@ class FlatOptimizer:
         self.state = state_tensors(name, op, flat.params)
         if name == "Lamb":
             dev = flat.params.device
-            self.chunks = lamb_chunk_table([p.numel() for _, p in flat.order]).to(dev)
+            self.chunks = flat.chunks
             self.partials = torch.zeros(3 * self.chunks.shape[0], dtype=torch.float64, device=dev)
             self.update = torch.zeros_like(flat.params)
 

@@ -3,8 +3,9 @@ train_loader, valid_loader) / .test() -- driving the sm_90a hot path (reference:
 
 What is kept: the per-batch order of SURVEY.md Appendix B (H2D -> forward+loss -> backward -> optimizer -> EMA -> LR
 step), named training_params of the reference recipes (max_epochs, initial_lr, lr_mode, cosine_final_lr_ratio,
-lr_warmup_steps, optimizer, optimizer_params, zero_weight_decay_on_bias_and_bn, ema, ema_params, batch_accumulate,
-loss, save_model, ...), the checkpoint dictionary keys, rank-0-only checkpointing.
+lr_warmup_steps, optimizer, optimizer_params, zero_weight_decay_on_bias_and_bn, ema, ema_params, batch_accumulate (also under
+cuda_graph), clip_grad_norm, precise_bn, precise_bn_batch_size, loss, save_model, ...), the checkpoint dictionary keys, rank-0-only
+checkpointing.
 What is different by design: one flat fp32 parameter / gradient buffer (training/flat_state.py), bf16 activations
 without a GradScaler, two optimizer launches per step, ONE flat NCCL all-reduce of live gradients per step under
 torchrun, and (optionally) the whole step captured in a CUDA graph.
@@ -12,6 +13,7 @@ Out of scope (SURVEY.md section 2): hydra recipes, dataset classes, loggers, met
 """
 import datetime
 import inspect
+import itertools
 import math
 import os
 import time
@@ -73,6 +75,9 @@ DEFAULT_TRAINING_PARAMS = {
     # sg_trainer.py:603-609, 732-739, 1645-1653).  The reference's default is True (training/params.py:28); here it is False so that
     # runs which do not ask for it write the files they always wrote.
     "average_best_models": False,
+    "clip_grad_norm": None,  # max L2 norm of the gradients of one optimisation step (sg_trainer.py:634-636); None: no clipping
+    "precise_bn": False,  # recompute the BatchNorm2d running statistics after every train epoch (sg_trainer.py:1552-1563)
+    "precise_bn_batch_size": None,  # samples precise_bn averages over (all ranks together); None: one batch per rank
 }
 
 AVERAGE_MODEL_FILENAME = "average_model.pth"
@@ -220,9 +225,11 @@ class TrainStep:
     STAGING_SLOTS = 8  # pinned host slots of the per-step hyper-parameters (how far the host may run ahead of the device)
 
     def __init__(self, model: nn.Module, criterion: Callable, optimizer: str, optimizer_params: Mapping[str, Any], zero_wd_on_bias_and_bn: bool, ema: bool = False, batch_accumulate: int = 1,
-                 keep_outputs: bool = False):  # fmt: skip
+                 keep_outputs: bool = False, clip_grad_norm: Optional[float] = None):  # fmt: skip
         """keep_outputs: expose the detached model outputs of the last step as `last_outputs` (train metrics).  Under a captured graph
-        that is the graph's static output buffer, so work enqueued after run() reads the step just replayed."""
+        that is the graph's static output buffer, so work enqueued after run() reads the step just replayed.
+        clip_grad_norm: clip the (reduced) gradients to this L2 norm before every optimizer update, on the device; `clip_norm_coef`
+        then holds the last update's {total norm, coefficient}."""
         self.model, self.criterion = model, criterion
         self.keep_outputs = keep_outputs
         self.last_outputs = None
@@ -267,6 +274,10 @@ class TrainStep:
         if self.device.type == "cuda":
             self.ctx.side_stream = torch.cuda.Stream(device=self.device)  # weight gradients overlap the dgrad / BN-backward chain
         self._nbt = [b for n, b in model.named_buffers() if n.endswith("num_batches_tracked")]
+        self.clip_grad_norm = float(clip_grad_norm) if clip_grad_norm else None
+        if self.clip_grad_norm is not None:
+            self.clip_partials = torch.zeros(f.chunks.shape[0], dtype=torch.float64, device=self.device)
+            self.clip_norm_coef = torch.zeros(2, dtype=torch.float32, device=self.device)
 
     # -------------------------------------------------------------------------------------------- host-side schedule
     def set_hyper_params(self, lr: float, ema_decay_value: Optional[float] = None):
@@ -367,6 +378,8 @@ class TrainStep:
         """Optimizer + EMA over the (already reduced) flat gradients; no collective in here."""
         f = self.flat
         nd = f.n_decay
+        if self.clip_grad_norm is not None and f.chunks.shape[0]:
+            K.clip_grad_norm(f.grads, f.chunks, self.hp, FO.GRAD_SCALE_COLUMN[self.opt_name], self.clip_grad_norm, self.clip_partials, self.clip_norm_coef)
         ranges = [(0, nd, 0), (nd, f.n_live, 1)] if self.fused is None else []
         if self.fused is not None:
             self.fused.step(f, self.hp)
@@ -395,10 +408,13 @@ class TrainStep:
         """inputs / targets: device tensors (targets may be any structure the criterion accepts).  With a captured
         graph the tensors are copied into the static buffers first."""
         if self.graph is not None:
-            if not do_optimizer_step:
-                raise RuntimeError("gradient accumulation is not supported together with cuda_graph")
+            if not do_optimizer_step and not isinstance(self.graph, _SplitReplay):
+                raise RuntimeError("gradient accumulation under cuda_graph needs a TrainStep built with batch_accumulate > 1")
             self._copy_static(self.static_in, (inputs, targets))
-            self.graph.replay()
+            if do_optimizer_step:
+                self.graph.replay()
+            else:  # inside an accumulation window: forward + backward only, the gradients add up in the flat buffer
+                self.graph.first.replay()
             loss, items = self.static_out
         else:
             loss, items = self._step_eager(inputs, targets, do_optimizer_step)
@@ -421,8 +437,9 @@ class TrainStep:
         warmup = max(warmup, 2)  # step 1 sizes the zero arena, step 2 builds the batched work tables the graph replays
         self.static_in = (clone(inputs), clone(targets))
         # The warm-up steps exist to size the arena / build the work tables, not to train: parameters, optimizer moments, EMA,
-        # BatchNorm buffers and the step counter are restored afterwards, so a captured run follows the eager trajectory.
-        live = [t for t in (self.flat.params, *self.state, getattr(self, "ema_params", None), getattr(self, "ema_buffers", None), self.flat.buffers, *self._nbt) if torch.is_tensor(t) and t.numel()]
+        # BatchNorm buffers, the hyper-parameter rows (clip_grad_norm scales their grad_scale in place) and the step counter are
+        # restored afterwards, so a captured run follows the eager trajectory.
+        live = [t for t in (self.flat.params, *self.state, getattr(self, "ema_params", None), getattr(self, "ema_buffers", None), self.flat.buffers, *self._nbt, self.hp) if torch.is_tensor(t) and t.numel()]
         saved, steps0 = [t.clone() for t in live], self.opt_steps
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
@@ -437,11 +454,12 @@ class TrainStep:
         self.opt_steps = steps0
         torch.cuda.synchronize()
         SF.bump_weight_epoch()
-        split = self.world > 1 or os.environ.get("SGB_SPLIT_GRAPH") == "1"
+        split = self.world > 1 or self.accumulate > 1 or os.environ.get("SGB_SPLIT_GRAPH") == "1"
         if split:
             # Data parallel: TWO graphs around an eagerly issued all-reduce (forward + backward | NCCL | optimizer + EMA).  Capturing
             # the collective inside the graph saves one launch but depends on NCCL's capture support and on nothing else in the
             # process touching CUDA meanwhile; the split costs ~one extra graph launch per step and is as robust as the 1-GPU capture.
+            # With batch_accumulate > 1 the micro-batches inside an accumulation window replay the first graph alone.
             g1, self.static_out = self._capture_region(lambda: self.forward_backward(*self.static_in))
             g2, _ = self._capture_region(self._apply_update, pool=g1.pool())
             self.graph = _SplitReplay(g1, (lambda: self.flat.all_reduce_grads(self.world)) if self.world > 1 else (lambda: None), g2)
@@ -499,6 +517,8 @@ class Trainer:
     # ------------------------------------------------------------------------------------------------ train
     def train(self, model: nn.Module, training_params: Mapping[str, Any], train_loader, valid_loader=None, test_loaders=None, additional_configs_to_log=None):
         tp = {**DEFAULT_TRAINING_PARAMS, **dict(training_params or {})}
+        if tp["clip_grad_norm"] is not None and tp["clip_grad_norm"] <= 0:
+            raise TypeError("Params", "Invalid clip_grad_norm")  # reference sg_trainer.py:1416-1417
         if tp["average_best_models"] and not tp["save_model"]:
             warnings.warn("'training_params.average_best_models' is enabled, but 'training_params.save_model' is disabled: model averaging "
                           "writes its snapshots next to the checkpoints, so 'average_best_models' is disabled")  # reference sg_trainer.py:1428-1434
@@ -527,7 +547,7 @@ class Trainer:
 
         train_metrics = [MetricsFactory().get(m) for m in tp["train_metrics_list"] or []]
         self.step = TrainStep(self.net, criterion, tp["optimizer"], tp["optimizer_params"], bool(tp["zero_weight_decay_on_bias_and_bn"]), ema=bool(tp["ema"]), batch_accumulate=int(tp["batch_accumulate"]),
-                              keep_outputs=bool(train_metrics))  # fmt: skip
+                              keep_outputs=bool(train_metrics), clip_grad_norm=tp["clip_grad_norm"])  # fmt: skip
         handler = CallbackHandler(_resolve_callbacks(tp["phase_callbacks"]))
         context = PhaseContext(net=self.net, criterion=criterion, device=self.device, experiment_name=self.experiment_name, ckpt_dir=self.checkpoints_dir_path,
                                train_loader=train_loader, valid_loader=valid_loader, training_params=tp, optimizer=None, context_methods=self)  # fmt: skip
@@ -567,13 +587,7 @@ class Trainer:
             for batch_idx, batch in enumerate(train_loader):
                 if batch_idx >= steps_per_epoch:
                     break
-                if hasattr(batch, "to_model_input"):  # PackedDetectionBatch / PackedPoseBatch: the GPU augmentation makes the input
-                    inputs, targets = batch.to_model_input(self.device)
-                else:
-                    inputs, targets = batch[0], batch[1]
-                inputs = inputs.to(self.device, non_blocking=True)
-                if torch.is_tensor(targets) and not (hasattr(criterion, "forward") and type(criterion).__name__ == "PPYoloELoss"):
-                    targets = targets.to(self.device, non_blocking=True)
+                inputs, targets = self._train_batch_to_device(batch)
                 gstep = epoch * steps_per_epoch + batch_idx
                 lr = self._lr_at(tp, gstep, steps_per_epoch)
                 do_step = (batch_idx + 1 + steps_per_epoch * epoch) % acc == 0
@@ -609,6 +623,17 @@ class Trainer:
             metrics.update({f"train_{k}": v for k, v in _metric_values(train_metrics).items()})  # never collides with the validation keys
             context.update_context(metrics_dict=metrics)
             handler.fire("on_train_loader_end", context)
+            if tp["precise_bn"]:  # live weights, then the EMA weights (reference sg_trainer.py:1552-1563)
+                self._precise_bn(train_loader, tp)
+                if self.step.ema_on:
+                    # the reference's EMA model is kept in eval mode (utils/ema.py:50-51): its forwards leave the statistics as they are
+                    self.step.swap_ema()
+                    self.net.eval()
+                    try:
+                        self._precise_bn(train_loader, tp)
+                    finally:
+                        self.net.train()
+                        self.step.swap_ema()
             if valid_loader is not None and (epoch + 1) % int(tp["run_validation_freq"]) == 0:
                 self.step.swap_ema()  # validate / checkpoint the EMA weights (sg_trainer.py:1566-1569)
                 handler.fire("on_validation_loader_start", context)
@@ -645,6 +670,52 @@ class Trainer:
                 self.model_weight_averaging.cleanup()
         handler.fire("on_training_end", context)
         return self.history
+
+    def _train_batch_to_device(self, batch):
+        """-> (inputs, targets) of one train-loader batch on the device, as the train step consumes them."""
+        if hasattr(batch, "to_model_input"):  # PackedDetectionBatch / PackedPoseBatch: the GPU augmentation makes the input
+            inputs, targets = batch.to_model_input(self.device)
+        else:
+            inputs, targets = batch[0], batch[1]
+        inputs = inputs.to(self.device, non_blocking=True)
+        if torch.is_tensor(targets) and not (hasattr(self.criterion, "forward") and type(self.criterion).__name__ == "PPYoloELoss"):
+            targets = targets.to(self.device, non_blocking=True)
+        return inputs, targets
+
+    @torch.no_grad()
+    def _precise_bn(self, loader, tp):
+        """compute_precise_bn_stats (reference utils/distributed_training_utils.py:98-144) on the flat BatchNorm buffer: the running
+        statistics of every nn.BatchNorm2d become the mean, over num_iter fresh batches of the train loader and over the ranks, of the
+        statistics of single batches (momentum 1.0 during the pass, restored after it).  Every forward runs in the model's current
+        mode, eagerly, outside the train step's arena and graph.  Modules that are not nn.BatchNorm2d (SyncBatchNorm under sync_bn)
+        keep what their own momentum made of the forwards, as in the reference.  The results are written into the flat buffer in
+        place, so the captured graph and the EMA keep addressing the same storage."""
+        world = torch.distributed.get_world_size() if is_distributed() else 1
+        size = tp["precise_bn_batch_size"]
+        num_iter = int(size / (loader.batch_size * world)) if size else world
+        num_iter = min(num_iter, len(loader))
+        bns = [m for m in self.net.modules() if isinstance(m, nn.BatchNorm2d)]
+        buffers = self.step.flat.buffers
+        acc = torch.zeros_like(buffers)
+        momenta = [bn.momentum for bn in bns]
+        for bn in bns:
+            bn.momentum = 1.0
+        try:
+            for batch in itertools.islice(loader, num_iter):
+                self.net(self._train_batch_to_device(batch)[0])
+                acc += buffers / num_iter  # every running statistic at once; only the BatchNorm2d ranges are kept
+        finally:
+            for bn, mom in zip(bns, momenta):
+                bn.momentum = mom
+        if world > 1:
+            torch.distributed.all_reduce(acc)
+            acc.mul_(1.0 / world)
+        keep = torch.zeros(buffers.numel(), dtype=torch.bool)
+        for bn in bns:
+            for t in (bn.running_mean, bn.running_var):
+                off = (t.data_ptr() - buffers.data_ptr()) // buffers.element_size()
+                keep[off : off + t.numel()] = True
+        buffers.copy_(torch.where(keep.to(buffers.device), acc, buffers))
 
     def _validate_final_average_model(self, valid_loader, tp, handler, context):
         """Validates average_model.pth once after the last epoch (reference sg_trainer.py:1785-1822): every rank loads it into the
