@@ -147,6 +147,13 @@ def as_nhwc(t: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def require_nhwc_out(out: torch.Tensor, shape) -> torch.Tensor:
+    """Returns `out` when it is a dense bf16 channels_last tensor of exactly `shape` (a caller-owned batch a launch writes), else raises."""
+    if tuple(out.shape) != tuple(shape) or out.dtype != torch.bfloat16 or not out.is_contiguous(memory_format=torch.channels_last):
+        raise L.SgbError(f"out must be a dense bf16 channels_last tensor of shape {tuple(shape)}, got {out.dtype} {tuple(out.shape)} strides {out.stride()}")
+    return out
+
+
 def empty_nhwc(n, c, h, w, device, c_alloc=None) -> torch.Tensor:
     """bf16 NHWC tensor with logical channels c; storage pitch is c rounded up to 8 (padding channels are zero)."""
     ca = c_alloc or ((c + 7) // 8) * 8

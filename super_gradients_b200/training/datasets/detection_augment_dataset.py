@@ -62,9 +62,15 @@ class PackedDetectionBatch:
         """Called by DataLoader(pin_memory=True) in the main process, so the copy to the device is asynchronous."""
         return PackedDetectionBatch(self.buffer.pin_memory(), self.batch, self.targets, self.input_dim, self.pad_value, self.max_value)
 
-    def to_model_input(self, device) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(images bf16 NHWC [B, 16, H, W], targets [N, 6]): one copy and one augmentation launch, no host synchronisation."""
-        return run_packed(self.buffer, self.batch, device, self.input_dim, self.pad_value, self.max_value), self.targets
+    @property
+    def input_shape(self) -> Tuple[int, int, int, int]:
+        """Shape of the model input to_model_input makes."""
+        return (self.batch, 16, *self.input_dim)
+
+    def to_model_input(self, device, out=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(images bf16 NHWC [B, 16, H, W], targets [N, 6]): one copy and one augmentation launch, no host synchronisation.  out: a
+        bf16 channels_last tensor of input_shape the images are written into instead of a new one."""
+        return run_packed(self.buffer, self.batch, device, self.input_dim, self.pad_value, self.max_value, out=out), self.targets
 
 
 @register_collate_function()

@@ -81,9 +81,15 @@ class PackedImageNetBatch:
         y2 = torch.full((x.size(0), self.num_classes), off, device=device).scatter_(1, x.flip(0), on)
         return y1 * self.lam + y2 * (1.0 - self.lam)
 
-    def to_model_input(self, device) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(images bf16 NHWC [B, 16, S, S], targets [B, num_classes]): one copy and one augmentation launch, no host synchronisation."""
-        images = run_packed(self.buffer, self.batch, self.workspace_bytes, device, self.size, self.fill, self.mean, self.std, self.mix_mode, self.lam, self.box)
+    @property
+    def input_shape(self) -> Tuple[int, int, int, int]:
+        """Shape of the model input to_model_input makes."""
+        return (self.batch, 16, self.size, self.size)
+
+    def to_model_input(self, device, out=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(images bf16 NHWC [B, 16, S, S], targets [B, num_classes]): one copy and one augmentation launch, no host synchronisation.
+        out: a bf16 channels_last tensor of input_shape the images are written into instead of a new one."""
+        images = run_packed(self.buffer, self.batch, self.workspace_bytes, device, self.size, self.fill, self.mean, self.std, self.mix_mode, self.lam, self.box, out=out)
         return images, self.targets(device)
 
 

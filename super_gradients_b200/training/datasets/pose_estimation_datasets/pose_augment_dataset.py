@@ -64,9 +64,15 @@ class PackedPoseBatch:
         """Called by DataLoader(pin_memory=True) in the main process, so the copy to the device is asynchronous."""
         return PackedPoseBatch(self.buffer.pin_memory(), self.batch, self.targets, self.output_size, self.max_value)
 
-    def to_model_input(self, device):
-        """(images bf16 NHWC [B, 16, S, S], (boxes, joints, is_crowd)): one copy and one augmentation call, no host synchronisation."""
-        return run_packed(self.buffer, self.batch, device, self.output_size, self.max_value), self.targets
+    @property
+    def input_shape(self) -> Tuple[int, int, int, int]:
+        """Shape of the model input to_model_input makes."""
+        return (self.batch, 16, self.output_size, self.output_size)
+
+    def to_model_input(self, device, out=None):
+        """(images bf16 NHWC [B, 16, S, S], (boxes, joints, is_crowd)): one copy and one augmentation call, no host synchronisation.
+        out: a bf16 channels_last tensor of input_shape the images are written into instead of a new one."""
+        return run_packed(self.buffer, self.batch, device, self.output_size, self.max_value, out=out), self.targets
 
 
 @register_collate_function()

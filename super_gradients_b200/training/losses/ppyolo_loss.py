@@ -21,13 +21,35 @@ from ... import kernels as K
 from ...common.registry import register_loss
 
 
-def pad_targets_host(targets: Tensor, batch_size: int, n_max: int) -> Tuple[Tensor, Tensor, Tensor]:
+def host_out(out, specs):
+    """numpy arrays to pad into: fresh zeros (out None), or the caller-owned CPU tensors `out`, checked against `specs` ((shape,
+    numpy dtype) per tensor) and zeroed, so the slots a batch does not fill hold no earlier batch's targets."""
+    if out is None:
+        return [np.zeros(shape, dtype) for shape, dtype in specs]
+    if len(out) != len(specs):
+        raise ValueError(f"out must hold {len(specs)} tensors, got {len(out)}")
+    arrays = []
+    for t, (shape, dtype) in zip(out, specs):
+        if t.is_cuda or not t.is_contiguous() or tuple(t.shape) != tuple(shape) or t.numpy().dtype != np.dtype(dtype):
+            raise ValueError(f"out tensors must be contiguous host tensors of the padded shapes: expected {shape} {np.dtype(dtype)}, got {tuple(t.shape)} {t.dtype}")
+        a = t.numpy()
+        a.fill(0)
+        arrays.append(a)
+    return arrays
+
+
+def max_targets_host(targets: Tensor) -> int:
+    """Largest number of targets one image of the batch holds: flat [N, 6] (img, cls, cx, cy, w, h) host targets, numpy only."""
+    img = targets.detach().float().numpy().reshape(-1, 6)[:, 0].astype(np.int64)
+    return int(np.bincount(img).max()) if img.size else 0
+
+
+def pad_targets_host(targets: Tensor, batch_size: int, n_max: int, out=None) -> Tuple[Tensor, Tensor, Tensor]:
     """flat [N, 6] (img, cls, cx, cy, w, h) -> gt_boxes [B, n_max, 4] xyxy, gt_labels [B, n_max] int32,
-    gt_valid [B, n_max] uint8  (ppyolo_loss.py:726-775).  Vectorised numpy on the host copy of the targets."""
+    gt_valid [B, n_max] uint8  (ppyolo_loss.py:726-775).  Vectorised numpy on the host copy of the targets.
+    out: caller-owned host tensors of those shapes and dtypes, written (and returned) instead of new ones."""
     t = targets.detach().float().cpu().numpy().reshape(-1, 6)
-    boxes = np.zeros((batch_size, n_max, 4), np.float32)
-    labels = np.zeros((batch_size, n_max), np.int32)
-    valid = np.zeros((batch_size, n_max), np.uint8)
+    boxes, labels, valid = host_out(out, (((batch_size, n_max, 4), np.float32), ((batch_size, n_max), np.int32), ((batch_size, n_max), np.uint8)))
     if t.shape[0]:
         img = t[:, 0].astype(np.int64)
         order = np.argsort(img, kind="stable")
@@ -40,7 +62,7 @@ def pad_targets_host(targets: Tensor, batch_size: int, n_max: int) -> Tuple[Tens
         boxes[img, slot] = xyxy
         labels[img, slot] = t[:, 1].astype(np.int32)
         valid[img, slot] = (xyxy.sum(1) > 0).astype(np.uint8)
-    return torch.from_numpy(boxes), torch.from_numpy(labels), torch.from_numpy(valid)
+    return tuple(out) if out is not None else (torch.from_numpy(boxes), torch.from_numpy(labels), torch.from_numpy(valid))
 
 
 class _FusedDetectionLoss(torch.autograd.Function):
@@ -101,6 +123,13 @@ class PPYoloELoss(nn.Module):
     @property
     def component_names(self):
         return ["loss_cls", "loss_iou", "loss_dfl", "loss"]
+
+    # The padded-target interface of the captured train step (sg_trainer.TrainStep.run_padded)
+    def max_targets(self, targets: Tensor) -> int:
+        return max_targets_host(targets)
+
+    def pad_targets(self, targets: Tensor, batch_size: int, n_max: int, out=None) -> Tuple[Tensor, Tensor, Tensor]:
+        return pad_targets_host(targets, batch_size, n_max, out)
 
     def forward(self, outputs: Union[Tuple, Tuple[Tuple[Tensor, Tensor], Tuple]], targets: Tensor) -> Tuple[Tensor, Tensor]:
         if isinstance(outputs, tuple) and len(outputs) == 2:

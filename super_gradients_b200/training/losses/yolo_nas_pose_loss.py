@@ -15,18 +15,36 @@ from torch import Tensor, nn
 
 from ... import kernels as K
 from ...common.registry import register_loss
+from .ppyolo_loss import host_out
 
 
-def pad_pose_targets_host(targets: Tuple[Tensor, Tensor, Tensor], batch_size: int, n_max: int) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+def _same_instances(img, joints, crowd):
+    # the reference selects boxes, joints and crowd flags per image by THEIR OWN image index column, in order
+    j_img, c_img = joints[:, 0, 0].astype(np.int64), crowd[:, 0].astype(np.int64)
+    if not (np.array_equal(j_img, img) and np.array_equal(c_img, img)):
+        raise ValueError("boxes, joints and crowd rows must describe the same instances in the same order")
+
+
+def max_pose_targets_host(targets: Tuple[Tensor, Tensor, Tensor]) -> int:
+    """Largest number of instances one image of the batch holds: (boxes [N, 5], joints [N, J, 4], crowd [N, 2]) host targets, each
+    with the image index first, numpy only.  Raises ValueError as pad_pose_targets_host does when the three disagree."""
+    boxes, joints, crowd = (t.detach().float().numpy() for t in targets)
+    if not boxes.shape[0]:
+        return 0
+    img = boxes[:, 0].astype(np.int64)
+    _same_instances(img, joints, crowd)
+    return int(np.bincount(img).max())
+
+
+def pad_pose_targets_host(targets: Tuple[Tensor, Tensor, Tensor], batch_size: int, n_max: int, out=None) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
     """(boxes [N, 5] = img, x1, y1, x2, y2; joints [N, J, 4] = img, x, y, visibility; crowd [N, 2] = img, is_crowd) ->
     gt_boxes [B, n_max, 4], gt_poses [B, n_max, J, 3], gt_crowd [B, n_max] uint8, gt_valid [B, n_max] uint8
-    (YoloNASPoseLoss._unpack_flat_targets, yolo_nas_pose_loss.py:343-401).  Instances keep their order within an image."""
+    (YoloNASPoseLoss._unpack_flat_targets, yolo_nas_pose_loss.py:343-401).  Instances keep their order within an image.
+    out: caller-owned host tensors of those shapes and dtypes, written (and returned) instead of new ones."""
     boxes, joints, crowd = (t.detach().float().cpu().numpy() for t in targets)
     J = joints.shape[1]
-    gt_boxes = np.zeros((batch_size, n_max, 4), np.float32)
-    gt_poses = np.zeros((batch_size, n_max, J, 3), np.float32)
-    gt_crowd = np.zeros((batch_size, n_max), np.uint8)
-    gt_valid = np.zeros((batch_size, n_max), np.uint8)
+    gt_boxes, gt_poses, gt_crowd, gt_valid = host_out(out, (((batch_size, n_max, 4), np.float32), ((batch_size, n_max, J, 3), np.float32),
+                                                            ((batch_size, n_max), np.uint8), ((batch_size, n_max), np.uint8)))  # fmt: skip
     if boxes.shape[0]:
         img = boxes[:, 0].astype(np.int64)
         order = np.argsort(img, kind="stable")
@@ -35,15 +53,12 @@ def pad_pose_targets_host(targets: Tuple[Tensor, Tensor, Tensor], batch_size: in
         slot[order] = np.arange(img.shape[0]) - first[img[order]]
         if slot.max() >= n_max:
             raise ValueError(f"an image has {slot.max() + 1} instances but n_max={n_max}")
-        # the reference selects boxes, joints and crowd flags per image by THEIR OWN image index column, in order
-        j_img, c_img = joints[:, 0, 0].astype(np.int64), crowd[:, 0].astype(np.int64)
-        if not (np.array_equal(j_img, img) and np.array_equal(c_img, img)):
-            raise ValueError("boxes, joints and crowd rows must describe the same instances in the same order")
+        _same_instances(img, joints, crowd)
         gt_boxes[img, slot] = boxes[:, 1:5]
         gt_poses[img, slot] = joints[:, :, 1:4]
         gt_crowd[img, slot] = (crowd[:, 1] != 0).astype(np.uint8)
         gt_valid[img, slot] = (boxes[:, 1:5].sum(1) > 0).astype(np.uint8)
-    return torch.from_numpy(gt_boxes), torch.from_numpy(gt_poses), torch.from_numpy(gt_crowd), torch.from_numpy(gt_valid)
+    return tuple(out) if out is not None else (torch.from_numpy(gt_boxes), torch.from_numpy(gt_poses), torch.from_numpy(gt_crowd), torch.from_numpy(gt_valid))
 
 
 class _FusedPoseLoss(torch.autograd.Function):
@@ -108,11 +123,19 @@ class YoloNASPoseLoss(nn.Module):
         self.assigner_multiply_by_pose_oks = assigner_multiply_by_pose_oks
         self.rescale_pose_loss_with_assigned_score = rescale_pose_loss_with_assigned_score
         self.average_losses_in_ddp = average_losses_in_ddp
+        self.max_targets_per_image = max_targets_per_image
         self._n_max = max_targets_per_image
 
     @property
     def component_names(self):
         return ["loss_cls", "loss_iou", "loss_dfl", "loss_pose_cls", "loss_pose_reg", "loss"]
+
+    # The padded-target interface of the captured train step (sg_trainer.TrainStep.run_padded)
+    def max_targets(self, targets) -> int:
+        return max_pose_targets_host(targets)
+
+    def pad_targets(self, targets, batch_size: int, n_max: int, out=None) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        return pad_pose_targets_host(targets, batch_size, n_max, out)
 
     def forward(self, outputs, targets) -> Tuple[Tensor, Tensor]:
         _, predictions = outputs

@@ -18,7 +18,7 @@ import math
 import os
 import time
 import warnings
-from typing import Any, Callable, Dict, Mapping, Optional
+from typing import Any, Callable, Dict, Mapping, Optional, Tuple
 
 import torch
 from torch import nn
@@ -198,12 +198,41 @@ def _update_metrics(metrics, fields: Mapping[str, Any]):
         m.update(**{k: v for k, v in fields.items() if k in accepted})
 
 
+def _host_targets(targets) -> bool:
+    """A batch's targets as a loader gives them to a padding loss: a host tensor or a tuple of host tensors."""
+    parts = targets if isinstance(targets, (tuple, list)) else (targets,)
+    return all(torch.is_tensor(t) and not t.is_cuda for t in parts)
+
+
 def _metric_values(metrics) -> Dict[str, float]:
     values = {}
     for m in metrics:
         res = m.compute()
         values.update({k: float(v) for k, v in res.items()} if isinstance(res, Mapping) else {type(m).__name__: float(res)})
     return values
+
+
+def padded_step_plan(n_max: Optional[int], graph_batch: Optional[int], floor: int, need: int, batch: int) -> Tuple[str, int]:
+    """What a captured train step fed host targets that the loss pads does with one batch (TrainStep.run_padded).  n_max / graph_batch:
+    those of the captured graph, None when there is none; floor: the loss's max_targets_per_image (or the n_max agreed after an
+    overflow); need: the batch's largest per-image target count.  -> ("capture", n_max of the new graph), ("replay", n_max), or
+    ("eager", n_max) for a batch of another size than the captured one or one that needs more than n_max."""
+    if n_max is None:
+        return "capture", max(int(floor), int(need), 1)
+    if batch != graph_batch or need > n_max:
+        return "eager", n_max
+    return "replay", n_max
+
+
+def agree_overflow(overflow_need: int, device) -> int:
+    """Epoch end of a captured padded-target step: the largest need, over every rank, of this epoch's steps that exceeded their n_max
+    (0: none did).  One all-reduce MAX under data parallelism: no rank can know without it whether another one fell back, and
+    every rank must take the same decision to capture again, because capture()'s warm-up steps issue collectives."""
+    if not is_distributed():
+        return int(overflow_need)
+    t = torch.tensor([int(overflow_need)], dtype=torch.int64, device=device)
+    torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
+    return int(t.item())
 
 
 class _SplitReplay:
@@ -267,6 +296,15 @@ class TrainStep:
         self.graph = None
         self.static_in = None
         self.static_out = None
+        self.replays = 0           # steps that replayed the captured graph
+        # run_padded: host targets padded into a pinned staging ring and copied into the graph's static target buffer
+        self.n_max = None          # n_max of the captured padded-target graph (None: no such graph)
+        self.fallbacks = 0         # run_padded steps that ran eagerly beside a captured graph
+        self._n_floor = 0          # n_max agreed at the end of an epoch with an overflow: the floor of the next capture
+        self._overflow_need = 0    # largest need this epoch of the steps that exceeded n_max
+        self._warned_overflow = False
+        self._graph_tables = None
+        self._graph_outputs = None
         self._filters_stale = False
         self.batched_plumbing = True
         self.arena = K.StepArena()   # zero-initialised scratch of one step (owned here: a captured graph replays its addresses)
@@ -406,26 +444,140 @@ class TrainStep:
 
     def run(self, inputs, targets, do_optimizer_step=True):
         """inputs / targets: device tensors (targets may be any structure the criterion accepts).  With a captured
-        graph the tensors are copied into the static buffers first."""
+        graph the tensors are copied into the static buffers first (inputs that ARE the static input are not copied)."""
         if self.graph is not None:
-            if not do_optimizer_step and not isinstance(self.graph, _SplitReplay):
-                raise RuntimeError("gradient accumulation under cuda_graph needs a TrainStep built with batch_accumulate > 1")
+            self._check_replay(do_optimizer_step)
             self._copy_static(self.static_in, (inputs, targets))
-            if do_optimizer_step:
-                self.graph.replay()
-            else:  # inside an accumulation window: forward + backward only, the gradients add up in the flat buffer
-                self.graph.first.replay()
-            loss, items = self.static_out
+            loss, items = self._replay(do_optimizer_step)
         else:
             loss, items = self._step_eager(inputs, targets, do_optimizer_step)
         if do_optimizer_step:
             self.opt_steps += 1
         return loss, items
 
+    def _check_replay(self, do_optimizer_step):
+        if not do_optimizer_step and not isinstance(self.graph, _SplitReplay):
+            raise RuntimeError("gradient accumulation under cuda_graph needs a TrainStep built with batch_accumulate > 1")
+
+    def _replay(self, do_optimizer_step):
+        if do_optimizer_step:
+            self.graph.replay()
+            # the host-side bookkeeping of _apply_update, which the replay ran on the device only: the weights moved, so the next
+            # eager forward (a fallback beside the graph, validation, precise_bn) re-prepares every filter cache
+            SF.bump_weight_epoch()
+            self._filters_stale = True
+        else:  # inside an accumulation window: forward + backward only, the gradients add up in the flat buffer
+            self.graph.first.replay()
+        self.replays += 1
+        if self.keep_outputs:  # an eager step beside the graph may have replaced them
+            self.last_outputs = self._graph_outputs
+        return self.static_out
+
+    def run_padded(self, inputs, targets, do_optimizer_step=True):
+        """The step under a CUDA graph for host targets that the criterion pads itself (it offers max_targets(targets) and
+        pad_targets(targets, batch_size, n_max, out), e.g. PPYoloELoss and YoloNASPoseLoss).  inputs: a device tensor; targets: the
+        loader's host targets.  The first call captures the step with n_max = max(criterion.max_targets_per_image, the batch's need).
+        Later batches are padded into a pinned staging slot, copied into the graph's static target buffer with one asynchronous copy
+        and replayed; a batch that needs more than n_max, or whose batch size differs from the captured one, runs eagerly (padded by
+        the loss as without a graph, with the same collectives as a replay).  end_epoch() captures again with a larger n_max after an
+        epoch with such an overflow."""
+        batch = int(inputs.shape[0])
+        need = self.criterion.max_targets(targets)
+        floor = max(int(getattr(self.criterion, "max_targets_per_image", 0) or 0), self._n_floor)
+        graph_batch = int(self.static_in[0].shape[0]) if self.n_max is not None else None
+        action, n_max = padded_step_plan(self.n_max, graph_batch, floor, need, batch)
+        if action == "capture":
+            self._target_ring(self.criterion.pad_targets(targets, batch, n_max))
+            self._stage_targets(targets, batch, n_max)
+            self._capture((inputs.clone(), self._tgt_static))
+            self.n_max = n_max
+        if action == "eager":
+            loss, items = self._fallback(inputs, targets, need, n_max, do_optimizer_step)
+        else:
+            self._check_replay(do_optimizer_step)
+            if action == "replay":
+                self._stage_targets(targets, batch, n_max)
+                self._copy_static(self.static_in[0], inputs)
+            loss, items = self._replay(do_optimizer_step)
+        if do_optimizer_step:
+            self.opt_steps += 1
+        return loss, items
+
+    def _fallback(self, inputs, targets, need, n_max, do_optimizer_step):
+        """One eager step beside the captured graph (run_padded)."""
+        self.fallbacks += 1
+        if need > n_max:
+            self._overflow_need = max(self._overflow_need, need)
+            if not self._warned_overflow:
+                warnings.warn(f"a train batch has an image with {need} targets, more than the captured step's n_max={n_max}: such steps run without "
+                              "the CUDA graph, and the step is captured again with a larger n_max at the start of the next epoch (raise the loss's "
+                              "max_targets_per_image to avoid this)")  # fmt: skip
+                self._warned_overflow = True
+        self._arena_replayed()
+        return self._step_eager(inputs, targets, do_optimizer_step)
+
+    def _arena_replayed(self):
+        """Before an eager step after replays: the replays left the scratch they used dirty without the host knowing how far (the
+        arena clears only what the last host-side step used), so the next begin_step() clears all of it."""
+        if self.arena.buf is not None:
+            self.arena.high = self.arena.buf.numel()
+
+    def _target_ring(self, padded):
+        """STAGING_SLOTS pinned host slots and one device buffer, each ONE contiguous byte buffer holding tensors shaped like the
+        padded targets `padded` as 16-byte aligned views; the device views are the graph's static targets."""
+        offsets, pos = [], 0
+        for t in padded:
+            offsets.append(pos)
+            pos += (t.numel() * t.element_size() + 15) // 16 * 16
+
+        def views(buf):
+            return tuple(buf[o : o + t.numel() * t.element_size()].view(t.dtype).view(t.shape) for o, t in zip(offsets, padded))
+
+        self._tgt_host = torch.zeros((self.STAGING_SLOTS, pos), dtype=torch.uint8, pin_memory=True)
+        self._tgt_host_views = [views(self._tgt_host[k]) for k in range(self.STAGING_SLOTS)]
+        self._tgt_dev = torch.zeros(pos, dtype=torch.uint8, device=self.device)
+        self._tgt_static = views(self._tgt_dev)
+        self._tgt_slot, self._tgt_events = 0, [None] * self.STAGING_SLOTS
+
+    def _stage_targets(self, targets, batch, n_max):
+        """Pads `targets` into the next pinned slot and enqueues ONE asynchronous copy of the slot into the static target buffer.  As
+        for the hyper-parameters, a slot is only rewritten after the copy that read it has executed, so the host never waits for the
+        device otherwise (a copy from pageable memory would block the host on every step)."""
+        k = self._tgt_slot
+        self._tgt_slot = (k + 1) % self.STAGING_SLOTS
+        if self._tgt_events[k] is not None:
+            self._tgt_events[k].synchronize()
+        self.criterion.pad_targets(targets, batch, n_max, out=self._tgt_host_views[k])
+        self._tgt_dev.copy_(self._tgt_host[k], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._tgt_events[k] = ev
+
+    def end_epoch(self):
+        """End of a train epoch under run_padded: when a step of this epoch on any rank needed more than its n_max, the graph is freed
+        and the next run_padded call captures it again with n_max at least the largest such need.  Every rank calls this at the same
+        epoch end, so every rank captures again at the same step."""
+        if self.n_max is None:
+            return
+        grown = agree_overflow(self._overflow_need, self.device)
+        self._overflow_need = 0
+        if grown > 0:
+            self._n_floor = max(self._n_floor, self.n_max, grown)
+            self.release_graph()
+
+    def release_graph(self):
+        """Frees the captured graph, its memory pool and its static buffers (once the device has finished with them)."""
+        torch.cuda.synchronize()
+        self._arena_replayed()
+        self.graph = self.static_in = self.static_out = self.last_outputs = None
+        self._graph_tables = self._graph_outputs = None
+        self.n_max = None
+
     @staticmethod
     def _copy_static(dst, src):
         if torch.is_tensor(dst):
-            dst.copy_(src, non_blocking=True)
+            if dst is not src:
+                dst.copy_(src, non_blocking=True)
         else:
             for d, s in zip(dst, src):
                 TrainStep._copy_static(d, s)
@@ -434,12 +586,17 @@ class TrainStep:
         """Captures the whole step in a CUDA graph (static shapes: pad the targets to a fixed n_max).  The LR is read
         from device memory, so set_hyper_params() keeps working between replays."""
         clone = lambda t: t.clone() if torch.is_tensor(t) else type(t)(clone(u) for u in t)  # noqa: E731
+        return self._capture((clone(inputs), clone(targets)), warmup)
+
+    def _capture(self, static_in, warmup: int = 3):
+        """capture() over the given static input / target buffers, which the graph then reads."""
         warmup = max(warmup, 2)  # step 1 sizes the zero arena, step 2 builds the batched work tables the graph replays
-        self.static_in = (clone(inputs), clone(targets))
+        self.static_in = static_in
         # The warm-up steps exist to size the arena / build the work tables, not to train: parameters, optimizer moments, EMA,
-        # BatchNorm buffers, the hyper-parameter rows (clip_grad_norm scales their grad_scale in place) and the step counter are
-        # restored afterwards, so a captured run follows the eager trajectory.
-        live = [t for t in (self.flat.params, *self.state, getattr(self, "ema_params", None), getattr(self, "ema_buffers", None), self.flat.buffers, *self._nbt, self.hp) if torch.is_tensor(t) and t.numel()]
+        # BatchNorm buffers, the hyper-parameter rows (clip_grad_norm scales their grad_scale in place), the gradients accumulated so
+        # far (a capture again inside an accumulation window) and the step counter are restored afterwards, so a captured run follows
+        # the eager trajectory.
+        live = [t for t in (self.flat.params, self.flat.grads, *self.state, getattr(self, "ema_params", None), getattr(self, "ema_buffers", None), self.flat.buffers, *self._nbt, self.hp) if torch.is_tensor(t) and t.numel()]
         saved, steps0 = [t.clone() for t in live], self.opt_steps
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
@@ -452,6 +609,9 @@ class TrainStep:
             for t, v in zip(live, saved):
                 t.copy_(v)
         self.opt_steps = steps0
+        # the outputs a warm-up step kept (keep_outputs) must not be freed inside the capture: with tuple outputs they hold blocks the
+        # side stream used, and freeing those while capturing makes the capture depend on uncaptured work
+        self.last_outputs = None
         torch.cuda.synchronize()
         SF.bump_weight_epoch()
         split = self.world > 1 or self.accumulate > 1 or os.environ.get("SGB_SPLIT_GRAPH") == "1"
@@ -465,6 +625,9 @@ class TrainStep:
             self.graph = _SplitReplay(g1, (lambda: self.flat.all_reduce_grads(self.world)) if self.world > 1 else (lambda: None), g2)
         else:
             self.graph, self.static_out = self._capture_region(lambda: self._step_eager(*self.static_in))
+        # the graph reads these work tables; an eager step beside it (run_padded) may build new ones, so they stay alive with it
+        self._graph_tables = (self.ctx.weight_table, self.ctx.wgrad_table, self.ctx.alpha_table)
+        self._graph_outputs = self.last_outputs  # the model outputs the captured forward kept: the graph's static buffers
         return self.graph
 
     def _capture_region(self, fn, pool=None):
@@ -555,6 +718,8 @@ class Trainer:
         total_steps = steps_per_epoch * int(tp["max_epochs"])
         ema_p = {**DEFAULT_TRAINING_PARAMS["ema_params"], **dict(tp["ema_params"] or {})}
         acc = int(tp["batch_accumulate"])
+        # host targets that the loss pads itself (detection, pose): under cuda_graph they go through TrainStep.run_padded
+        padded = bool(tp["cuda_graph"]) and callable(getattr(criterion, "pad_targets", None))
         best = None
         start_epoch = 0
         if ckpt is not None:
@@ -587,12 +752,13 @@ class Trainer:
             for batch_idx, batch in enumerate(train_loader):
                 if batch_idx >= steps_per_epoch:
                     break
-                inputs, targets = self._train_batch_to_device(batch)
+                inputs, targets = self._train_batch_to_device(batch, self._static_input_for(batch) if tp["cuda_graph"] else None)
+                host_padded = padded and _host_targets(targets)
                 gstep = epoch * steps_per_epoch + batch_idx
                 lr = self._lr_at(tp, gstep, steps_per_epoch)
                 do_step = (batch_idx + 1 + steps_per_epoch * epoch) % acc == 0
                 self.step.set_hyper_params(lr, ema_decay(ema_p["decay_type"], float(ema_p["decay"]), gstep + 1, total_steps, float(ema_p.get("beta", 15))) if tp["ema"] else None)
-                if tp["cuda_graph"] and self.step.graph is None:
+                if tp["cuda_graph"] and self.step.graph is None and not host_padded:
                     if torch.is_tensor(targets) and targets.is_cuda:
                         self.step.capture(inputs, targets)
                     elif not getattr(self, "_warned_no_graph", False):
@@ -603,7 +769,7 @@ class Trainer:
                 if handler.callbacks:
                     context.update_context(batch_idx=batch_idx, inputs=inputs, target=targets, lr=lr)
                     handler.fire("on_train_batch_start", context)
-                loss, _items = self.step.run(inputs, targets, do_step)
+                loss, _items = self.step.run_padded(inputs, targets, do_step) if host_padded else self.step.run(inputs, targets, do_step)
                 running = loss.clone() if running is None else running + loss  # clone: with a captured graph `loss` is the static output buffer
                 if train_metrics:  # MetricsUpdateCallback at TRAIN_BATCH_END (sg_trainer.py:1264), enqueued behind the step: no sync
                     _update_metrics(train_metrics, {"preds": self.step.last_outputs, "target": targets, "inputs": inputs, "device": self.device})
@@ -617,6 +783,8 @@ class Trainer:
                         handler.fire("on_train_batch_gradient_step_start", context)
                         handler.fire("on_train_batch_gradient_step_end", context)
                     handler.fire("on_train_batch_end", context)
+            if padded:
+                self.step.end_epoch()
             train_loss = float(running / max(nb, 1)) if running is not None else float("nan")
             self.history["train_loss"].append(train_loss)
             metrics = {"train_loss": train_loss}
@@ -671,14 +839,24 @@ class Trainer:
         handler.fire("on_training_end", context)
         return self.history
 
-    def _train_batch_to_device(self, batch):
-        """-> (inputs, targets) of one train-loader batch on the device, as the train step consumes them."""
-        if hasattr(batch, "to_model_input"):  # PackedDetectionBatch / PackedPoseBatch: the GPU augmentation makes the input
-            inputs, targets = batch.to_model_input(self.device)
+    def _static_input_for(self, batch):
+        """The captured step's static input when `batch` is a packed GPU-augmentation batch of its shape (the augmentation then writes
+        the batch there: no allocation and no device-to-device copy per step), else None."""
+        st = self.step
+        if st is None or st.graph is None or not hasattr(batch, "to_model_input"):
+            return None
+        x = st.static_in[0]
+        return x if tuple(x.shape) == tuple(batch.input_shape) else None
+
+    def _train_batch_to_device(self, batch, out=None):
+        """-> (inputs, targets) of one train-loader batch on the device, as the train step consumes them.  out: where a packed
+        batch's augmentation writes the input (see _static_input_for)."""
+        if hasattr(batch, "to_model_input"):  # PackedDetectionBatch / PackedPoseBatch / PackedImageNetBatch: the GPU augmentation makes the input
+            inputs, targets = batch.to_model_input(self.device, out=out)
         else:
             inputs, targets = batch[0], batch[1]
         inputs = inputs.to(self.device, non_blocking=True)
-        if torch.is_tensor(targets) and not (hasattr(self.criterion, "forward") and type(self.criterion).__name__ == "PPYoloELoss"):
+        if torch.is_tensor(targets) and not callable(getattr(self.criterion, "pad_targets", None)):  # losses that pad their targets take them on the host
             targets = targets.to(self.device, non_blocking=True)
         return inputs, targets
 

@@ -164,11 +164,13 @@ def pack_into(plans: Sequence[AugmentPlan], raw: np.ndarray) -> None:
     fill_table(plans, offsets, raw[:head].view(np.int64).reshape(len(plans), K.AUG_FIELDS))
 
 
-def run_packed(host: torch.Tensor, batch: int, device, input_dim: Tuple[int, int], pad_value: int = 114, max_value: float = 255.0) -> torch.Tensor:
-    """One copy of the packed uint8 buffer `host` to `device` and one augmentation launch -> bf16 NHWC [B, 16, H, W]."""
+def run_packed(host: torch.Tensor, batch: int, device, input_dim: Tuple[int, int], pad_value: int = 114, max_value: float = 255.0, out=None) -> torch.Tensor:
+    """One copy of the packed uint8 buffer `host` to `device` and one augmentation launch -> bf16 NHWC [B, 16, H, W], written into
+    `out` (e.g. a captured train step's static input) when given."""
     head = batch * K.AUG_FIELDS * 8
     dev = host.to(device, non_blocking=True)
-    out = K.empty_nhwc(batch, 16, input_dim[0], input_dim[1], device)
+    shape = (batch, 16, input_dim[0], input_dim[1])
+    out = K.empty_nhwc(*shape, device) if out is None else K.require_nhwc_out(out, shape)
     K.detection_augment(host[:head].view(torch.int64).view(batch, K.AUG_FIELDS), dev[:head].view(torch.int64).view(batch, K.AUG_FIELDS), dev[head:], out,
                         pad_value=pad_value, max_value=max_value)  # fmt: skip
     return out

@@ -213,12 +213,13 @@ def pack_into(plans: Sequence[ImageNetPlan], raw: np.ndarray, size: int) -> None
         ws += h * size * 3
 
 
-def run_packed(host: torch.Tensor, batch: int, workspace_bytes: int, device, size: int, fill, mean, std, mix_mode=0, lam=1.0, box=(0, 0, 0, 0)) -> torch.Tensor:
-    """One copy of the packed uint8 buffer `host` to `device` and one augmentation launch -> bf16 NHWC [B, 16, size, size]."""
+def run_packed(host: torch.Tensor, batch: int, workspace_bytes: int, device, size: int, fill, mean, std, mix_mode=0, lam=1.0, box=(0, 0, 0, 0), out=None) -> torch.Tensor:
+    """One copy of the packed uint8 buffer `host` to `device` and one augmentation launch -> bf16 NHWC [B, 16, size, size], written
+    into `out` (e.g. a captured train step's static input) when given."""
     head = batch * K.IN_FIELDS * 8
     dev = host.to(device, non_blocking=True)
     ws = torch.empty(max(workspace_bytes, 1), dtype=torch.uint8, device=device)
-    out = K.empty_nhwc(batch, 16, size, size, device)
+    out = K.empty_nhwc(batch, 16, size, size, device) if out is None else K.require_nhwc_out(out, (batch, 16, size, size))
     K.imagenet_augment(host[:head].view(torch.int64).view(batch, K.IN_FIELDS), dev[:head].view(torch.int64).view(batch, K.IN_FIELDS), dev[head:], ws, out, fill, mean, std,
                        mix_mode=mix_mode, lam=lam, box=box)  # fmt: skip
     return out

@@ -129,11 +129,12 @@ def pack_into(plans: Sequence[PosePlan], raw: np.ndarray) -> None:
     fill_table(plans, offsets, raw[:head].view(np.int64).reshape(len(plans), K.POSE_FIELDS))
 
 
-def run_packed(host: torch.Tensor, batch: int, device, size: int, max_value: float = 255.0) -> torch.Tensor:
-    """One copy of the packed uint8 buffer `host` to `device` and one pose augmentation call -> bf16 NHWC [B, 16, size, size]."""
+def run_packed(host: torch.Tensor, batch: int, device, size: int, max_value: float = 255.0, out=None) -> torch.Tensor:
+    """One copy of the packed uint8 buffer `host` to `device` and one pose augmentation call -> bf16 NHWC [B, 16, size, size], written
+    into `out` (e.g. a captured train step's static input) when given."""
     head = batch * K.POSE_FIELDS * 8
     dev = host.to(device, non_blocking=True)
     ws = torch.empty(max(host.numel() - head, 1), dtype=torch.uint8, device=device)
-    out = K.empty_nhwc(batch, 16, size, size, device)
+    out = K.empty_nhwc(batch, 16, size, size, device) if out is None else K.require_nhwc_out(out, (batch, 16, size, size))
     K.pose_augment(host[:head].view(torch.int64).view(batch, K.POSE_FIELDS), dev[:head].view(torch.int64).view(batch, K.POSE_FIELDS), dev[head:], ws, out, max_value)
     return out
