@@ -500,6 +500,9 @@ extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, con
                               float* assigned_box, float* assigned_score, double* sums, void* workspace,
                               int64_t workspace_bytes, void* stream) {
   if (int rc = check_loss(d)) return rc;
+  // the top-k keeps one gt's metric row of all L anchors in shared memory
+  const size_t smem = (size_t)d->L * sizeof(float);
+  SGB_REQUIRE(d->n_max == 0 || smem <= 200 * 1024, "too many anchors for the shared-memory metric row");
   SGB_REQUIRE(cls_logits && reg_distri && anchor_points && stride_tensor && assigned_label && assigned_box &&
                   assigned_score && sums && workspace,
               "null pointer");
@@ -513,13 +516,12 @@ extern "C" int sgb_tal_assign(const SgbLossDesc* d, const float* cls_logits, con
   tal_decode_kernel<<<grid, 256, 0, st>>>(*d, reg_distri, anchor_points, stride_tensor, w.pbox);
   SGB_LAUNCH_CHECK("tal_decode_kernel");
   if (d->n_max > 0) {
-    size_t smem = (size_t)d->L * sizeof(float);
-    static bool attr = false;
-    if (!attr) {
-      cudaFuncSetAttribute(tal_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      attr = true;
-    }
-    SGB_REQUIRE(smem <= 200 * 1024, "too many anchors for the shared-memory metric row");
+    // The opt-in above 48 KB counts the kernel's static shared memory too (the top-k's merge slots), so it is set
+    // whatever the row size.  It is a per-device setting: set on every call, so every device
+    // gets it, and always to the same cap, so concurrent callers never lower it under each other.
+    if (int rc = sgb_cuda_check(cudaFuncSetAttribute(tal_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024),
+                                "cudaFuncSetAttribute(tal_topk_kernel)"))
+      return rc;
     tal_topk_kernel<<<d->B * d->n_max, 256, smem, st>>>(*d, cls_logits, anchor_points, gt_boxes, gt_labels, gt_valid,
                                                         w);
     SGB_LAUNCH_CHECK("tal_topk_kernel");

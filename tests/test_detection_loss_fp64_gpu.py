@@ -139,9 +139,10 @@ def test_tal_decisions_parameter_sweep(topk, alpha, beta):
     assert _check_assignment(c, topk, alpha, beta, f"640x384 topk={topk} alpha={alpha} beta={beta}") > 0
 
 
-@pytest.mark.parametrize("B,H,W,n,topk", [(8, 640, 640, 120, 13), (8, 384, 640, 200, 64), (1, 1024, 1024, 200, 13), (8, 1024, 1024, 100, 64)])
+@pytest.mark.parametrize("B,H,W,n,topk", [(8, 640, 640, 120, 13), (8, 384, 640, 200, 64), (2, 480, 1248, 150, 13), (1, 1024, 1024, 200, 13), (8, 1024, 1024, 100, 64)])
 def test_tal_decisions_image_sizes(B, H, W, n, topk):
-    """L = 8400 (640^2), 5040 (640 x 384) and 21504 (1024^2: the top-k metric row takes 84 KB of shared memory, above 48 KB)."""
+    """L = 8400 (640^2), 5040 (640 x 384), 12285 (1248 x 480: a 49140 B row, under 48 KB alone but not with the kernel's static
+    shared memory) and 21504 (1024^2: the top-k metric row takes 84 KB of shared memory, above 48 KB)."""
     c = DC.decision_case(B, H, W, n, seed=B + H + n, n_invalid=4)
     assert _check_assignment(c, topk, 1.0, 6.0, f"B={B} {W}x{H} n={n} topk={topk}") > 0
 
