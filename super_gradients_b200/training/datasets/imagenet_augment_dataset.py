@@ -5,12 +5,17 @@ makes the draws of the ResNet-50 recipe's train chain (RandomResizedCropAndInter
 transforms/imagenet_augment.py) and returns the plan with only the crop window's bytes.  `ImageNetAugmentCollateFN` packs a batch into
 one uint8 buffer and draws the batch's mixup / cutmix parameters as the reference's CollateMixup does in batch mode
 (datasets/mixup.py:179-206, 89-100), touching no CUDA state; `PackedImageNetBatch.to_model_input(device)` then makes the bf16 NHWC
-model input with one copy and one kernel launch, and the [B, num_classes] soft targets with a few small torch ops on the device."""
+model input with one copy and one kernel launch, and the [B, num_classes] soft targets with a few small torch ops on the device.
+
+`ImageNetValidationDataset` / `ImageNetValidationCollateFN` do the same for the recipe's validation chain Resize(236) ->
+CenterCrop(224) -> ToTensor -> Normalize: the workers only pack the decoded images, and `PackedImageNetValidationBatch` makes the
+model input with one copy and one launch of the predict() resize-and-crop kernel (kernels.resample_crop_u8)."""
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
+from ... import kernels as K
 from ...common.registry import register_collate_function
 from ..transforms.imagenet_augment import ImageNetPlan, RandAugmentConfig, draw_plan, pack_into, packed_size, run_packed, workspace_size
 
@@ -154,3 +159,85 @@ class ImageNetAugmentCollateFN:
         labels = torch.tensor([p.label for p in plans], dtype=torch.int32)
         return PackedImageNetBatch(buf, len(plans), labels, workspace_size(plans, self.size), self.size, self.fill, self.img_mean, self.img_std, lam, use_cutmix, box,
                                    self.num_classes, self.label_smoothing)  # fmt: skip
+
+
+class ImageNetValidationDataset(torch.utils.data.Dataset):
+    """The recipe's validation chain torchvision Resize(resize) (Pillow bilinear, antialiased) -> CenterCrop(size) -> ToTensor ->
+    Normalize(img_mean, img_std) over any dataset returning (PIL RGB image or uint8 H x W x 3 RGB array, label).  Items are the
+    uint8 image and the label; every pixel is the kernel's."""
+
+    def __init__(self, dataset, resize: int = 236, size: int = 224, img_mean=IMAGENET_MEAN, img_std=IMAGENET_STD):
+        if int(resize) < int(size):
+            raise ValueError(f"Resize({resize}) must not be smaller than CenterCrop({size}): the GPU path does not pad")
+        self.dataset, self.resize, self.size = dataset, int(resize), int(size)
+        self.img_mean, self.img_std = tuple(float(m) for m in img_mean), tuple(float(s) for s in img_std)
+
+    def __len__(self) -> int:
+        return len(self.dataset)
+
+    def __getitem__(self, index: int) -> Tuple[np.ndarray, int]:
+        image, label = self.dataset[index]
+        return _as_rgb_array(image), int(label)
+
+
+def validation_geometry(height: int, width: int, resize: int, size: int) -> Tuple[Tuple[int, int], Tuple[int, int]]:
+    """torchvision's Resize(resize) output size (shorter side resize, longer side truncated) and CenterCrop(size)'s top-left
+    corner (rounded half to even) -> ((resized h, w), (top, left))."""
+    short, long = (width, height) if width <= height else (height, width)
+    new_long = int(resize * long / short)
+    rh, rw = (new_long, resize) if width <= height else (resize, new_long)
+    return (rh, rw), (int(round((rh - size) / 2.0)), int(round((rw - size) / 2.0)))
+
+
+class PackedImageNetValidationBatch:
+    """A collated batch: `buffer` (uint8: the int64 [B, RS_FIELDS] table, then the images) and the int64 labels."""
+
+    def __init__(self, buffer: torch.Tensor, batch: int, labels: torch.Tensor, size: int, mean, std):
+        self.buffer, self.batch, self.labels, self.size, self.mean, self.std = buffer, batch, labels, size, mean, std
+
+    def pin_memory(self) -> "PackedImageNetValidationBatch":
+        """Called by DataLoader(pin_memory=True) in the main process, so the copy to the device is asynchronous."""
+        return PackedImageNetValidationBatch(self.buffer.pin_memory(), self.batch, self.labels, self.size, self.mean, self.std)
+
+    @property
+    def input_shape(self) -> Tuple[int, int, int, int]:
+        """Shape of the model input to_model_input makes."""
+        return (self.batch, 16, self.size, self.size)
+
+    def to_model_input(self, device, out=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(images bf16 NHWC [B, 16, S, S], labels [B]): one copy and one resize-and-crop launch, no host synchronisation.  out: a
+        bf16 channels_last tensor of input_shape the images are written into instead of a new one."""
+        head = self.batch * K.RS_FIELDS * 8
+        dev = self.buffer.to(device, non_blocking=True)
+        out = K.empty_nhwc(*self.input_shape, device) if out is None else K.require_nhwc_out(out, self.input_shape)
+        table_host = self.buffer[:head].view(torch.int64).view(self.batch, K.RS_FIELDS)
+        K.resample_crop_u8(table_host, dev[:head].view(torch.int64).view(self.batch, K.RS_FIELDS), dev[head:], out, max_value=255.0, mean=self.mean, std=self.std)
+        return out, self.labels
+
+
+@register_collate_function()
+class ImageNetValidationCollateFN:
+    """Collates ImageNetValidationDataset items into a PackedImageNetValidationBatch; the labels are default_collate's."""
+
+    def __init__(self, resize: int = 236, size: int = 224, img_mean=IMAGENET_MEAN, img_std=IMAGENET_STD):
+        self.resize, self.size, self.img_mean, self.img_std = int(resize), int(size), tuple(img_mean), tuple(img_std)
+
+    @classmethod
+    def for_dataset(cls, dataset: ImageNetValidationDataset) -> "ImageNetValidationCollateFN":
+        return cls(dataset.resize, dataset.size, dataset.img_mean, dataset.img_std)
+
+    def __call__(self, data: Sequence[Tuple[np.ndarray, int]]) -> PackedImageNetValidationBatch:
+        images = [_as_rgb_array(d[0]) for d in data]
+        B = len(images)
+        head = B * K.RS_FIELDS * 8
+        offsets = np.cumsum([0] + [im.nbytes for im in images])
+        buf = torch.empty(head + int(offsets[-1]), dtype=torch.uint8)
+        raw = buf.numpy()
+        table = raw[:head].view(np.int64).reshape(B, K.RS_FIELDS)
+        for b, im in enumerate(images):
+            h, w = im.shape[:2]
+            (rh, rw), (top, left) = validation_geometry(h, w, self.resize, self.size)
+            table[b] = (offsets[b], h, w, w * 3, rh, rw, top, left)
+            raw[head + offsets[b] : head + offsets[b + 1]] = np.ascontiguousarray(im).reshape(-1)
+        labels = torch.tensor([int(d[1]) for d in data], dtype=torch.int64)
+        return PackedImageNetValidationBatch(buf, B, labels, self.size, self.img_mean, self.img_std)

@@ -6,9 +6,12 @@ AbstractPoseEstimationDataset.  In DataLoader workers it runs the host half of t
 KeypointsCompose.apply_to_sample does: sanitize, then the transforms, loading a mosaic's three extra samples with
 random.randrange and passing each through the transforms applied so far.  `PoseAugmentCollateFN` packs a batch into one uint8
 buffer (table + images) plus YoloNASPoseCollateFN's targets, touching no CUDA state; `PackedPoseBatch.to_model_input(device)`
-then makes the model input with one copy and one kernel call."""
+then makes the model input with one copy and one kernel call.  With `with_gt_samples` (the validation datasets) each item also
+carries the transformed sample's ground truth, and `YoloNASPoseAugmentCollateFN` delivers it as YoloNASPoseCollateFN does, in the
+batch's `extras` {"gt_samples": [...]}, which PoseEstimationMetrics reads."""
 import random
-from typing import List, Sequence, Tuple
+from dataclasses import dataclass
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -19,10 +22,26 @@ from ...transforms.keypoints_augment import PosePlan, pack_into, packed_size, ru
 from .yolo_nas_pose_collate_fn import flat_collate_tensors_with_batch_index
 
 
+@dataclass
+class PoseGroundTruth:
+    """One transformed sample as YoloNASPoseCollateFN leaves it in gt_samples (set_image_to_none): joints [N, J, 3], areas [N] or
+    None, bboxes_xywh [N, 4] or None, is_crowd [N] or None; no image or mask."""
+
+    joints: np.ndarray
+    areas: Optional[np.ndarray]
+    bboxes_xywh: Optional[np.ndarray]
+    is_crowd: Optional[np.ndarray]
+    image: None = None
+    mask: None = None
+    additional_samples: None = None
+
+
 class PoseAugmentDataset(torch.utils.data.Dataset):
-    def __init__(self, dataset, transforms: Sequence):
+    """with_gt_samples: items are (plan, targets, PoseGroundTruth), else (plan, targets)."""
+
+    def __init__(self, dataset, transforms: Sequence, with_gt_samples: bool = False):
         self.output_size = check_pose_pipeline(transforms)
-        self.dataset, self.transforms = dataset, list(transforms)
+        self.dataset, self.transforms, self.with_gt_samples = dataset, list(transforms), bool(with_gt_samples)
         self.max_value = float([t for t in self.transforms if isinstance(t, KeypointsImageStandardize)][0].max_value)
 
     def __len__(self) -> int:
@@ -50,19 +69,24 @@ class PoseAugmentDataset(torch.utils.data.Dataset):
         xywh = np.asarray(s.bboxes_xywh)
         xyxy = np.concatenate([xywh[..., :2], xywh[..., :2] + xywh[..., 2:4]], axis=-1)
         is_crowd = np.zeros(len(xyxy)) if s.is_crowd is None else s.is_crowd
-        return s.plan, (xyxy, s.joints, is_crowd.astype(int).reshape((-1, 1)))
+        targets = (xyxy, s.joints, is_crowd.astype(int).reshape((-1, 1)))
+        if self.with_gt_samples:
+            return s.plan, targets, PoseGroundTruth(s.joints, s.areas, s.bboxes_xywh, s.is_crowd)
+        return s.plan, targets
 
 
 class PackedPoseBatch:
-    """A collated batch: `buffer` (uint8: the int64 per-sample table, then the images) and YoloNASPoseCollateFN's targets
-    (boxes [N, 5], joints [N, J, 4], is_crowd [N, 2], each with the sample index first)."""
+    """A collated batch: `buffer` (uint8: the int64 per-sample table, then the images), YoloNASPoseCollateFN's targets
+    (boxes [N, 5], joints [N, J, 4], is_crowd [N, 2], each with the sample index first) and `extras`, the additional batch items
+    the metrics receive ({"gt_samples": [...]} from YoloNASPoseAugmentCollateFN)."""
 
-    def __init__(self, buffer: torch.Tensor, batch: int, targets, output_size: int, max_value: float):
+    def __init__(self, buffer: torch.Tensor, batch: int, targets, output_size: int, max_value: float, extras=None):
         self.buffer, self.batch, self.targets, self.output_size, self.max_value = buffer, batch, targets, output_size, max_value
+        self.extras = extras if extras is not None else {}
 
     def pin_memory(self) -> "PackedPoseBatch":
         """Called by DataLoader(pin_memory=True) in the main process, so the copy to the device is asynchronous."""
-        return PackedPoseBatch(self.buffer.pin_memory(), self.batch, self.targets, self.output_size, self.max_value)
+        return PackedPoseBatch(self.buffer.pin_memory(), self.batch, self.targets, self.output_size, self.max_value, self.extras)
 
     @property
     def input_shape(self) -> Tuple[int, int, int, int]:
@@ -92,3 +116,16 @@ class PoseAugmentCollateFN:
         pack_into(plans, buf.numpy())
         targets = tuple(flat_collate_tensors_with_batch_index([torch.from_numpy(d[1][k]) for d in data]) for k in range(3))
         return PackedPoseBatch(buf, len(plans), targets, self.output_size, self.max_value)
+
+
+@register_collate_function()
+class YoloNASPoseAugmentCollateFN(PoseAugmentCollateFN):
+    """Collates PoseAugmentDataset(with_gt_samples=True) items into a PackedPoseBatch whose extras are YoloNASPoseCollateFN's
+    {"gt_samples": [...]} (reference datasets/pose_estimation_datasets/yolo_nas_pose_collate_fn.py:28-70)."""
+
+    def __call__(self, data: List[Tuple[PosePlan, tuple, PoseGroundTruth]]) -> PackedPoseBatch:
+        if any(len(d) != 3 for d in data):
+            raise ValueError("YoloNASPoseAugmentCollateFN takes (plan, targets, ground truth) items: build the dataset with with_gt_samples=True")
+        batch = super().__call__([d[:2] for d in data])
+        batch.extras = {"gt_samples": [d[2] for d in data]}
+        return batch

@@ -943,9 +943,14 @@ class Trainer:
         for i, batch in enumerate(loader):
             if max_batches is not None and i >= int(max_batches):
                 break
-            inputs, targets = batch[0].to(self.device), batch[1]
-            if torch.is_tensor(targets) and type(self.criterion).__name__ != "PPYoloELoss":
-                targets = targets.to(self.device)
+            if hasattr(batch, "to_model_input"):  # a packed validation batch: the GPU makes the input, extras travel with the batch
+                inputs, targets = self._train_batch_to_device(batch)
+                extra = getattr(batch, "extras", {})
+            else:
+                inputs, targets = batch[0].to(self.device), batch[1]
+                if torch.is_tensor(targets) and type(self.criterion).__name__ != "PPYoloELoss":
+                    targets = targets.to(self.device)
+                extra = batch[2] if len(batch) > 2 and isinstance(batch[2], Mapping) else {}
             if handler is not None and handler.callbacks:
                 context.update_context(batch_idx=i, inputs=inputs, target=targets)
                 handler.fire(f"on_{phase}_batch_start", context)
@@ -960,7 +965,6 @@ class Trainer:
                     items_tot = out[1].detach().double().cpu() if items_tot is None else items_tot + out[1].detach().double().cpu()
             n += 1
             if valid_metrics:
-                extra = batch[2] if len(batch) > 2 and isinstance(batch[2], Mapping) else {}
                 _update_metrics(valid_metrics, {"preds": preds, "target": targets, "inputs": inputs, "device": self.device, **extra})
         values = _metric_values(valid_metrics)
         self.net.train()

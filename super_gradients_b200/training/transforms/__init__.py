@@ -15,8 +15,10 @@ from .keypoints import (
 from .transforms import (
     DetectionHorizontalFlip,
     DetectionHSV,
+    DetectionImagePermute,
     DetectionMixup,
     DetectionPaddedRescale,
+    DetectionPadToSize,
     DetectionRandomAffine,
     DetectionRGB2BGR,
     DetectionStandardize,
@@ -24,6 +26,6 @@ from .transforms import (
 )
 
 __all__ = ["AugmentPlan", "BatchAugmenter", "MixupPlan", "DetectionRandomAffine", "DetectionRGB2BGR", "DetectionHSV", "DetectionHorizontalFlip",
-           "DetectionMixup", "DetectionPaddedRescale", "DetectionStandardize", "DetectionTargetsFormatTransform", "KeypointsRandomHorizontalFlip",
+           "DetectionMixup", "DetectionPaddedRescale", "DetectionPadToSize", "DetectionStandardize", "DetectionImagePermute", "DetectionTargetsFormatTransform", "KeypointsRandomHorizontalFlip",
            "KeypointsBrightnessContrast", "KeypointsReverseImageChannels", "KeypointsHSV", "KeypointsRandomRotate90", "KeypointsRandomAffineTransform",
            "KeypointsMosaic", "KeypointsLongestMaxSize", "KeypointsPadIfNeeded", "KeypointsImageStandardize", "KeypointsRemoveSmallObjects"]  # fmt: skip

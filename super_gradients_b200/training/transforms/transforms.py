@@ -18,7 +18,9 @@ from ...common.registry import register_transform
 from .detection_augment import AugmentPlan, MixupPlan, MosaicPlan, MosaicTile
 
 RECIPE_ORDER = ("DetectionMosaic", "DetectionRandomAffine", "DetectionRGB2BGR", "DetectionHSV", "DetectionHorizontalFlip", "DetectionMixup",
-                "DetectionPaddedRescale", "DetectionStandardize", "DetectionTargetsFormatTransform")  # fmt: skip
+                "DetectionPaddedRescale", "DetectionPadToSize", "DetectionStandardize", "DetectionImagePermute", "DetectionTargetsFormatTransform")  # fmt: skip
+# DetectionPadToSize runs on the affine step of the kernel, so it only combines with the steps that commute with a pad of one grey
+PAD_TO_SIZE_EXCLUDES = ("DetectionMosaic", "DetectionRandomAffine", "DetectionHSV", "DetectionHorizontalFlip", "DetectionMixup", "DetectionPaddedRescale")
 
 
 def _tuple_of_two(v):
@@ -79,10 +81,13 @@ class HostSample:
             is_crowd = np.concatenate([is_crowd, np.ones_like(crowd[:, 4], dtype=bool)], axis=0)
         return cls(AugmentPlan(image, image.shape[:2]), image.shape[:2], boxes, labels, is_crowd)
 
-    def to_dict(self) -> dict:
-        """convert_detection_sample_to_dict(include_crowd_target=False): what a train dataset returns."""
+    def to_dict(self, include_crowd_target: bool = False) -> dict:
+        """convert_detection_sample_to_dict: what a dataset returns, `crowd_target` too when it was built with_crowd."""
         crowd = self.is_crowd > 0
-        return {"target": np.concatenate([self.bboxes_xyxy[~crowd], self.labels[~crowd][..., None]], axis=-1)}
+        out = {"target": np.concatenate([self.bboxes_xyxy[~crowd], self.labels[~crowd][..., None]], axis=-1)}
+        if include_crowd_target:
+            out["crowd_target"] = np.concatenate([self.bboxes_xyxy[crowd], self.labels[crowd][..., None]], axis=-1)
+        return out
 
 
 class _Transform:
@@ -357,6 +362,45 @@ class DetectionPaddedRescale(_Transform):
 
 
 @register_transform()
+class DetectionPadToSize(_Transform):
+    """Center padding to output_size (rows, cols) without a rescale (DetectionPadIfNeeded in "center" mode, detection_pad_if_needed.py);
+    the boxes move by the pad's top-left offsets.  The pixels are the kernel's affine step with the integer translation
+    (pad_left, pad_top), whose border is the pad value: cv2's fixed-point warp reads every output pixel from exactly one source pixel
+    there.  An image larger than output_size would make the reference's output larger than output_size, so it raises ValueError."""
+
+    def __init__(self, output_size, pad_value):
+        self.output_size = _tuple_of_two(output_size)
+        values = [pad_value] if isinstance(pad_value, Number) else list(pad_value)
+        if len(set(values)) != 1 or not float(values[0]).is_integer() or not 0 <= values[0] <= 255:
+            raise ValueError(f"pad_value must be one integer in [0, 255] (or the same one for every channel), got {pad_value}")
+        self.pad_value = int(values[0])
+
+    def apply_to_sample(self, sample: HostSample) -> HostSample:
+        (h, w), (oh, ow) = sample.shape, self.output_size
+        if h > oh or w > ow:
+            raise ValueError(f"DetectionPadToSize({self.output_size}) received a {h}x{w} image: the GPU path writes a fixed {oh}x{ow} batch")
+        top, left = (oh - h) // 2, (ow - w) // 2
+        sample.plan.affine = (np.array([[1.0, 0.0, left], [0.0, 1.0, top]]), (oh, ow), self.pad_value)
+        sample.plan.rescaled = (oh, ow)
+        boxes = sample.bboxes_xyxy[:, :4].copy()  # _shift_bboxes_xyxy (transforms/utils.py)
+        boxes[:, [0, 2]] += left
+        boxes[:, [1, 3]] += top
+        return sample.replaced(shape=(oh, ow), bboxes_xyxy=np.concatenate((boxes, sample.bboxes_xyxy[:, 4:]), 1))
+
+
+@register_transform()
+class DetectionImagePermute(_Transform):
+    """HWC -> CHW of the reference's image; the kernel writes the NHWC model input, so only the default dims (2, 0, 1) are accepted."""
+
+    def __init__(self, dims=(2, 0, 1)):
+        if tuple(dims) != (2, 0, 1):
+            raise ValueError(f"only dims (2, 0, 1) are supported on the GPU path, got {dims}")
+
+    def apply_to_sample(self, sample: HostSample) -> HostSample:
+        return sample
+
+
+@register_transform()
 class DetectionStandardize(_Transform):
     def __init__(self, max_value: float = 255.0):
         self.max_value = float(max_value)
@@ -395,5 +439,8 @@ def check_order(transforms) -> None:
     pos = [RECIPE_ORDER.index(n) for n in names]
     if pos != sorted(set(pos)):
         raise ValueError(f"the transforms must appear at most once each and in the order {RECIPE_ORDER}, got {names}")
-    if "DetectionPaddedRescale" not in names:
-        raise ValueError("DetectionPaddedRescale must be in the pipeline: it fixes the model input size")
+    if "DetectionPaddedRescale" not in names and "DetectionPadToSize" not in names:
+        raise ValueError("DetectionPaddedRescale or DetectionPadToSize must be in the pipeline: it fixes the model input size")
+    if "DetectionPadToSize" in names and any(n in PAD_TO_SIZE_EXCLUDES for n in names):
+        raise ValueError(f"DetectionPadToSize combines only with DetectionRGB2BGR, DetectionStandardize, DetectionImagePermute and "
+                         f"DetectionTargetsFormatTransform, got {names}")  # fmt: skip
