@@ -268,6 +268,24 @@ int sgb_qarep_bwd_fused(const SgbQarepDesc* d, const sgb_bf16* dout, const sgb_b
                         double* sums, const float* gamma3, const float* gamma_p, sgb_bf16* dy3, sgb_bf16* du, float* dgamma3,
                         float* dbeta3, float* dbias1a, float* dgamma_p, float* dbeta_p, void* stream);
 
+/* The passes above for the train-mode QARepVGG stem on patches (functional._QARepVGGStem), with y3 / u never stored: each pass
+ * recomputes [y3 | u] = xp @ w^T from the 32-channel patch tensor xp ([M][32] bf16, dense) and the resident filter w ([2C][32] bf16)
+ * exactly as sgb_conv_fprop would have stored them, then does what the pass of the same name above does with them.  C = 32, 48 or 64;
+ * the layouts of out / dout / dy3 / du are those of the desc (y3 / u fields: dy3 / du).  Forward: sgb_stem_qarep_moments (moments zero
+ * on entry), then sgb_stem_qarep_fwd; backward: sgb_stem_qarep_bwd_reduce (sums zero on entry), then sgb_stem_qarep_bwd_apply.
+ * sgb_stem_gemm writes [y3 | u] itself ([M][2C]), for tests.  sgb_stem_recompute_launches counts the launches of all five. */
+int sgb_stem_gemm(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, sgb_bf16* y, void* stream);
+int sgb_stem_qarep_moments(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, double* moments, void* stream);
+int sgb_stem_qarep_fwd(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, const double* moments, const float* gamma3,
+                       const float* beta3, const float* bias1_alpha, const float* gamma_p, const float* beta_p, float* rm3, float* rv3,
+                       float* rm_p, float* rv_p, sgb_bf16* out, float* coef, void* stream);
+int sgb_stem_qarep_bwd_reduce(const SgbQarepDesc* d, const sgb_bf16* dout, const sgb_bf16* xp, const sgb_bf16* w, const float* coef,
+                              double* sums, void* stream);
+int sgb_stem_qarep_bwd_apply(const SgbQarepDesc* d, const sgb_bf16* dout, const sgb_bf16* xp, const sgb_bf16* w, const float* coef,
+                             const double* sums, const float* gamma3, const float* gamma_p, sgb_bf16* dy3, sgb_bf16* du, float* dgamma3,
+                             float* dbeta3, float* dbias1a, float* dgamma_p, float* dbeta_p, void* stream);
+int64_t sgb_stem_recompute_launches(void);
+
 
 /* ---- pooling / elementwise (rows C6, C7, C8) --------------------------------------------------------------- */
 /* stride-`stride` max-pool k x k, pad k/2 (csp_darknet53.py:135-157 SPP; resnet.py maxpool 3/2/1). idx (int8,

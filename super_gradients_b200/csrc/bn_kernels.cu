@@ -11,6 +11,8 @@
 // Reference: nn.BatchNorm2d as used by modules/conv_bn_act_block.py:92-93, modules/qarepvgg_block.py:190-204,
 // training/models/classification_models/resnet.py:53-84 and its autograd backward.
 #include "common.cuh"
+#include "sm100_host.h"
+#include "sm100_ptx.cuh"
 #include "stream_ring.cuh"
 
 #include <cooperative_groups.h>
@@ -176,23 +178,32 @@ static int sgb_sm_count() {
   return sms;
 }
 
+// Grid of chan_fused_kernel<OpA, OpB> over M pixels of C channels (its dynamic shared memory in *smem), or a negative error code.  The
+// grid fixes which pixels every fp32 partial sum covers: the stem kernels that recompute the operands use it to sum in the same order.
 template <class OpA, class OpB>
-int launch_chan_fused(const OpA& a, const OpB& b, int64_t M, int C, cudaStream_t st, const char* what) {
+int chan_fused_grid(int64_t M, int C, size_t* smem, const char* what) {
   auto tail = [&](int ncoef, int nacc) { return ((size_t)ncoef * C + (size_t)(nacc * 8 + 1) * TPB) * sizeof(float); };
   const size_t ta = tail(OpA::NCOEF, OpA::NACC), tb = tail(OpB::NCOEF, OpB::NACC);
-  const size_t smem = chan_ring_bytes2<OpA, OpB>() + (ta > tb ? ta : tb);
+  *smem = chan_ring_bytes2<OpA, OpB>() + (ta > tb ? ta : tb);
   static bool attr = false;
   if (!attr) {
     cudaFuncSetAttribute(chan_fused_kernel<OpA, OpB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     attr = true;
   }
   int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chan_fused_kernel<OpA, OpB>, TPB, smem) != cudaSuccess || per_sm < 1)
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chan_fused_kernel<OpA, OpB>, TPB, *smem) != cudaSuccess || per_sm < 1)
     return sgb_cuda_check(cudaErrorCooperativeLaunchTooLarge, what);
   int64_t want = (M + 255) / 256;
   int64_t cap = (int64_t)sgb_sm_count() * per_sm;
   if (cap > sgb_chan_grid_cap()) cap = sgb_chan_grid_cap();
-  const int grid = (int)(want < 1 ? 1 : (want > cap ? cap : want));
+  return (int)(want < 1 ? 1 : (want > cap ? cap : want));
+}
+
+template <class OpA, class OpB>
+int launch_chan_fused(const OpA& a, const OpB& b, int64_t M, int C, cudaStream_t st, const char* what) {
+  size_t smem = 0;
+  const int grid = chan_fused_grid<OpA, OpB>(M, C, &smem, what);
+  if (grid < 0) return grid;
   int64_t Mv = M;
   int Cv = C;
   void* args[] = {(void*)&a, (void*)&b, (void*)&Mv, (void*)&Cv};
@@ -460,6 +471,49 @@ struct BnBwdApplyOp {
 // ============================================================================================== QARepVGG algebra
 // y3 = conv3x3(x) (raw), u = conv1x1_{alpha*K1 + I}(x) (raw);  z = s3*(y3 - mu3) + beta3 + u + alpha*b1;
 // out = act(post_bn(z)) = act(a3*y3 + au*u + c0).  See include/sgb200.h for the coefficient / moment layout.
+// The per-element arithmetic of the passes below, shared with the stem kernels that recompute y3 / u (stem_qarep_kernel): r(k) is
+// coefficient row k of the element's channel, acc[a] its running sum a.
+__device__ __forceinline__ void qarep_mom(float y3, float u, float* acc) {
+  acc[0] += y3;
+  acc[1] = fmaf(y3, y3, acc[1]);
+  acc[2] += u;
+  acc[3] = fmaf(u, u, acc[3]);
+  acc[4] = fmaf(y3, u, acc[4]);
+}
+// out = act(a3 * y3 + au * u + c0) (coefficient rows 0 a3, 1 au, 2 c0)
+template <class R>
+__device__ __forceinline__ float qarep_out(float y3, float u, R r, int act) {
+  return apply_act(fmaf(r(0), y3, fmaf(r(1), u, r(2))), act);
+}
+// T0 += dzp, T1 += dzp * zhat, T2 += dzp * y3hat (QarepBwdRedOp's coefficient rows)
+template <class R>
+__device__ __forceinline__ void qarep_bwd_sums(const SgbQarepDesc& d, float g, float y3, float u, R r, float* acc) {
+  float dz = g;
+  if (d.act == SGB_ACT_RELU) dz = fmaf(r(4), y3, fmaf(r(5), u, r(6))) > 0.f ? dz : 0.f;
+  const float y3c = y3 - r(0);
+  acc[0] += dz;
+  if (d.use_post_bn) acc[1] = fmaf(dz, (fmaf(r(7), y3c, u - r(2))) * r(3), acc[1]);
+  acc[2] = fmaf(dz, y3c * r(1), acc[2]);
+}
+// dy3, du of one element (QarepBwdApplyOp's coefficient rows)
+template <class R>
+__device__ __forceinline__ void qarep_bwd_grads(const SgbQarepDesc& d, float g, float y3, float u, R r, float& o3, float& ou) {
+  float dzp = g;
+  if (d.act == SGB_ACT_RELU) dzp = fmaf(r(4), y3, fmaf(r(5), u, r(6))) > 0.f ? dzp : 0.f;
+  const float y3c = y3 - r(0);
+  const float y3h = y3c * r(1);
+  float dz;
+  if (d.use_post_bn) {
+    const float zh = fmaf(r(7), y3c, u - r(2)) * r(3);
+    dz = r(8) * (dzp - r(9) - zh * r(10));
+    o3 = r(7) * (dz - y3h * r(11));
+  } else {
+    dz = dzp;
+    o3 = r(7) * (dz - r(9) - y3h * r(11));
+  }
+  ou = dz;
+}
+
 // the five moments of (y3, u) as a pass of the same skeleton: first half of the fused forward launch (sgb_qarep_fwd_fused)
 struct QarepMomOp {
   static constexpr int NCOEF = 0, NACC = 5;
@@ -475,11 +529,10 @@ struct QarepMomOp {
     const V8 a = unpack8(raw[0]), b = unpack8(raw[1]);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
-      acc[0][e] += a.v[e];
-      acc[1][e] = fmaf(a.v[e], a.v[e], acc[1][e]);
-      acc[2][e] += b.v[e];
-      acc[3][e] = fmaf(b.v[e], b.v[e], acc[3][e]);
-      acc[4][e] = fmaf(a.v[e], b.v[e], acc[4][e]);
+      float s[5] = {acc[0][e], acc[1][e], acc[2][e], acc[3][e], acc[4][e]};
+      qarep_mom(a.v[e], b.v[e], s);
+#pragma unroll
+      for (int k = 0; k < 5; ++k) acc[k][e] = s[k];
     }
   }
 };
@@ -565,7 +618,7 @@ struct QarepFwdOpT {
     V8 a = unpack8(raw[0]);
     const V8 b = unpack8(raw[1]);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) a.v[e] = apply_act(fmaf(r[0][e], a.v[e], fmaf(r[1][e], b.v[e], r[2][e])), d.act);
+    for (int e = 0; e < 8; ++e) a.v[e] = qarep_out(a.v[e], b.v[e], [&](int k) { return r[k][e]; }, d.act);
     if constexpr (RES) {
       // the block's own output is rounded to bf16 first, exactly as when it was stored and re-read by a separate scale_add pass:
       // the fused form is bit-identical to the two-pass form
@@ -611,12 +664,10 @@ struct QarepBwdRedOp {
     const V8 g = unpack8(raw[0]), a = unpack8(raw[1]), b = unpack8(raw[2]);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
-      float dz = g.v[e];
-      if (d.act == SGB_ACT_RELU) dz = fmaf(r[4][e], a.v[e], fmaf(r[5][e], b.v[e], r[6][e])) > 0.f ? dz : 0.f;
-      const float y3c = a.v[e] - r[0][e];
-      acc[0][e] += dz;
-      if (d.use_post_bn) acc[1][e] = fmaf(dz, (fmaf(r[7][e], y3c, b.v[e] - r[2][e])) * r[3][e], acc[1][e]);
-      acc[2][e] = fmaf(dz, y3c * r[1][e], acc[2][e]);
+      float s[3] = {acc[0][e], acc[1][e], acc[2][e]};
+      qarep_bwd_sums(d, g.v[e], a.v[e], b.v[e], [&](int k) { return r[k][e]; }, s);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) acc[k][e] = s[k];
     }
   }
 };
@@ -685,22 +736,7 @@ struct QarepBwdApplyOp {
     const V8 g = unpack8(raw[0]), a = unpack8(raw[1]), b = unpack8(raw[2]);
     V8 o3, ou;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      float dzp = g.v[e];
-      if (d.act == SGB_ACT_RELU) dzp = fmaf(r[4][e], a.v[e], fmaf(r[5][e], b.v[e], r[6][e])) > 0.f ? dzp : 0.f;
-      const float y3c = a.v[e] - r[0][e];
-      const float y3h = y3c * r[1][e];
-      float dz;
-      if (d.use_post_bn) {
-        const float zh = fmaf(r[7][e], y3c, b.v[e] - r[2][e]) * r[3][e];
-        dz = r[8][e] * (dzp - r[9][e] - zh * r[10][e]);
-        o3.v[e] = r[7][e] * (dz - y3h * r[11][e]);
-      } else {
-        dz = dzp;
-        o3.v[e] = r[7][e] * (dz - r[9][e] - y3h * r[11][e]);
-      }
-      ou.v[e] = dz;
-    }
+    for (int e = 0; e < 8; ++e) qarep_bwd_grads(d, g.v[e], a.v[e], b.v[e], [&](int k) { return r[k][e]; }, o3.v[e], ou.v[e]);
     st8(dy3 + pix * d.pitch3 + d.off3 + c0, o3);
     st8(du + pix * d.pitchu + d.offu + c0, ou);
   }
@@ -729,6 +765,287 @@ int check_qarep(const SgbQarepDesc* d) {
   SGB_REQUIRE(!d->res || (d->res_alpha && d->pitchr % 8 == 0 && d->offr % 8 == 0 && d->pitchr >= d->offr + d->C && ((uintptr_t)d->res & 15) == 0),
               "shortcut tensor layout");
   SGB_REQUIRE(!d->count || (((uintptr_t)d->count & 7) == 0 && d->param_scale > 0.f && d->param_scale <= 1.f), "cross-rank count / param_scale");
+  return SGB_OK;
+}
+
+// ============================================================================================== QARepVGG stem on patches
+// The train-mode stem (functional._QARepVGGStem) is ONE 1 x 1 GEMM over 32 gathered patch channels: [y3 | u] = xp @ W^T with
+// W = [K3 ; centre(K1)] ([2K][32] bf16).  Storing [y3 | u] costs 2K bf16 per pixel written once and read by four passes; recomputing
+// it costs two k16 wgmma steps per 128-pixel chunk against a filter that stays in shared memory.  So every pass of the block
+// recomputes y3 / u from xp instead of reading them, and computes exactly what the stored-operand pass computes:
+//   - the GEMM is conv_wgmma_kernel's for that shape (the same two k16 steps in the same order, fp32 accumulators rounded to bf16), so
+//     the recomputed values are bit-equal to the stored ones;
+//   - the values then go through shared memory to chan_body's thread mapping (a thread owns one 8-channel vector, its coefficients in
+//     registers, and every lanes-th pixel of the CTA's range) and the Ops' own per-element code;
+//   - the reductions (STEM_MOM, STEM_BRED) split the pixels into the same contiguous ranges as the fused chan launch they replace
+//     (chan_fused_grid) and sum in its order -- per thread in pixel order, then over the lanes in order, one fp64 atomic per channel
+//     and range -- so the sums, and with them the coefficients, the output and the gradients, are those of the stored-operand path.
+//     STEM_GEMM   [y3 | u] written out (a test's view of what the other modes recompute)
+//     STEM_MOM    the five moments of QarepMomOp                    (forward, phase 1)
+//     STEM_FWD    out = act(a3 y3 + au u + c0), QarepFwdOp's prologue (forward, phase 2)
+//     STEM_BRED   T0..T2 of QarepBwdRedOp from dout                  (backward, phase 1)
+//     STEM_BAPPLY dy3 | du of QarepBwdApplyOp, its prologue's parameter gradients (backward, phase 2)
+// CTA of three warpgroups, persistent over ranges of pixels walked in 128-pixel chunks: warpgroup 0 is the TMA producer (the filter
+// once, then per chunk the xp rows and, backward, the dout rows into a ring of stages); warpgroups 1-2 run the wgmma over 64 rows each,
+// park the rounded tile in shared memory, and then process it in chan_body's mapping.
+enum StemMode { STEM_GEMM, STEM_MOM, STEM_FWD, STEM_BRED, STEM_BAPPLY };
+constexpr int STEM_THREADS = 384, STEM_BM = 128, STEM_KP = 32, STEM_STAGES = 6;
+
+struct StemGemmOp {  // STEM_GEMM: [y3 | u] to y ([M][2K] bf16)
+  static constexpr int NCOEF = 0, NACC = 0;
+  bf16* y;
+  double* out = nullptr;
+  int out_stride = 0;
+  __device__ void prologue(float*) const {}
+};
+
+template <int KOUT, int MODE, class Op>
+struct StemLayout {
+  static constexpr int BN = 2 * KOUT;
+  static constexpr int YP = BN + 8;  // row pitch of the parked tile (elements): 16-byte rows, conflict-free fragment stores
+  static constexpr bool DOUT = MODE == STEM_BRED || MODE == STEM_BAPPLY;
+  static constexpr int NACC = Op::NACC;
+  static constexpr uint32_t A_BYTES = STEM_BM * STEM_KP * 2;  // 128 rows x 64 bytes, 64B swizzle
+  static constexpr uint32_t G_BYTES = DOUT ? STEM_BM * KOUT * 2 : 0;
+  static constexpr uint32_t STAGE = (A_BYTES + G_BYTES + 1023u) & ~1023u;
+  static constexpr uint32_t W_BYTES = (BN * STEM_KP * 2 + 1023u) & ~1023u;
+  static constexpr uint32_t Y_BYTES = STEM_BM * YP * 2;
+  static constexpr uint32_t CTRL = 8u * (2 * STEM_STAGES + 1);
+  static size_t smem() {
+    return 1024 + W_BYTES + STEM_STAGES * STAGE + Y_BYTES + CTRL + ((size_t)Op::NCOEF * KOUT + (size_t)(NACC * 8 + 1) * TPB) * sizeof(float);
+  }
+};
+
+__device__ __forceinline__ void stem_consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Pixels [b * per, min((b + 1) * per, M)) form range b, b = 0 .. nranges - 1; CTAs take ranges blockIdx.x, + gridDim.x, ...
+template <int KOUT, int MODE, class Op>
+__global__ void __launch_bounds__(STEM_THREADS, 1)
+stem_qarep_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_g,
+                  const Op op, const SgbQarepDesc d, const int64_t M, const int64_t per, const int nranges) {
+  using Lay = StemLayout<KOUT, MODE, Op>;
+  constexpr int BN = Lay::BN, YP = Lay::YP, NACC = Lay::NACC, NCOEF = Op::NCOEF, JB = KOUT / 8;
+  constexpr int CVB = KOUT / 8, LANES = TPB / CVB;  // chan_body's mapping for C = KOUT: one channel-vector pass
+  extern __shared__ __align__(16) unsigned char smem_raw[];  // the 64B-swizzled operands want 1024-byte alignment: rounded up here
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t s_w = base, s_stage0 = base + Lay::W_BYTES, s_y = s_stage0 + STEM_STAGES * Lay::STAGE, ctrl = s_y + Lay::Y_BYTES;
+  auto full_bar = [&](int s) { return ctrl + 8u * s; };
+  auto empty_bar = [&](int s) { return ctrl + 8u * (STEM_STAGES + s); };
+  const uint32_t w_bar = ctrl + 8u * 2 * STEM_STAGES;
+  auto gen = [&](uint32_t a) { return smem_raw + (a - smem_u32(smem_raw)); };
+  bf16* ytile = reinterpret_cast<bf16*>(gen(s_y));                  // [128][YP]: y3 in columns [0, K), u in [K, 2K)
+  float* sc = reinterpret_cast<float*>(gen(ctrl + Lay::CTRL));      // [NCOEF][KOUT] coefficients
+  float* sred = sc + NCOEF * KOUT;                                   // [TPB][NACC * 8 + 1]: chan_body's reduction scratch
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STEM_STAGES; ++s) {
+      sm100::mbar_init(full_bar(s), 1);
+      sm100::mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
+    }
+    sm100::mbar_init(w_bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  if (threadIdx.x < TPB) op.prologue(sc);  // the Op's prologue strides its channels by TPB (block 0: the side effects, once)
+  __syncthreads();
+
+  if (warp == 0) {
+    if (sm100::elect_one()) {
+      sm100::mbar_expect_tx(w_bar, BN * STEM_KP * 2);
+      sm100::tma_load_2d(s_w, &map_w, w_bar, 0, 0);
+      int stg = 0;
+      uint32_t par = 1;  // the first pass through the ring is free
+      for (int b = blockIdx.x; b < nranges; b += gridDim.x) {
+        const int64_t p0 = (int64_t)b * per, p1 = p0 + per < M ? p0 + per : M;
+        for (int64_t s0 = p0; s0 < p1; s0 += STEM_BM) {
+          sm100::mbar_wait(empty_bar(stg), par);
+          const uint32_t sa = s_stage0 + stg * Lay::STAGE;
+          sm100::mbar_expect_tx(full_bar(stg), Lay::A_BYTES + Lay::G_BYTES);  // rows past M are zero-filled and still counted
+          sm100::tma_load_2d(sa, &map_x, full_bar(stg), 0, (int)s0);
+          if constexpr (Lay::DOUT) sm100::tma_load_2d(sa + Lay::A_BYTES, &map_g, full_bar(stg), 0, (int)s0);
+          if (++stg == STEM_STAGES) {
+            stg = 0;
+            par ^= 1;
+          }
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1, wq = warp & 3;
+    const int rl0 = wg * 64 + wq * 16 + (lane >> 2);  // fragment rows rl0, rl0 + 8 of this thread
+    const int t = threadIdx.x - 128, pl = t / CVB, cvi = t % CVB, c0 = cvi * 8;
+    const bool active = pl < LANES;
+    float r[NCOEF > 0 ? NCOEF : 1][8];  // chan_body: the thread's coefficients, in registers for the whole kernel
+#pragma unroll
+    for (int k = 0; k < NCOEF; ++k)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) r[k][e] = sc[k * KOUT + c0 + e];
+    float acc[BN / 2];
+    float sums[NACC > 0 ? NACC : 1][8];
+    sm100::mbar_wait(w_bar, 0);
+    int stg = 0;
+    uint32_t par = 0;
+    for (int b = blockIdx.x; b < nranges; b += gridDim.x) {
+      const int64_t p0 = (int64_t)b * per, p1 = p0 + per < M ? p0 + per : M;
+#pragma unroll
+      for (int a = 0; a < (NACC > 0 ? NACC : 1); ++a)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) sums[a][e] = 0.f;
+      for (int64_t s0 = p0; s0 < p1; s0 += STEM_BM) {
+        const int rows = (int)(p1 - s0 < STEM_BM ? p1 - s0 : STEM_BM);
+        sm100::mbar_wait(full_bar(stg), par);
+        const uint32_t sa = s_stage0 + stg * Lay::STAGE;
+        // conv_wgmma_kernel's k-sequence for a 32-channel 1 x 1 GEMM: one 64B-swizzled stage, two k16 steps, the first overwriting D
+        sm100::wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const uint64_t da = sm100::smem_desc(sa + (uint32_t)wg * 64u * 64u + 32u * j, 64, 16u, 512u);
+          const uint64_t db = sm100::smem_desc(s_w + 32u * j, 64, 16u, 512u);
+          sm100::mma_kk<BN>(acc, da, db, j);
+        }
+        sm100::wgmma_commit();
+        sm100::wgmma_wait<0>();
+        sm100::fence_regs(acc);
+        // park the tile as conv_wgmma_kernel stores it: bf16 pairs rounded to nearest
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 2 * JB; ++j)
+            *reinterpret_cast<__nv_bfloat162*>(ytile + (rl0 + 8 * h) * YP + 8 * j + 2 * (lane & 3)) =
+                __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        stem_consumer_sync();
+        if (active) {
+          const bf16* g_tile = reinterpret_cast<const bf16*>(gen(sa + Lay::A_BYTES));  // [128][KOUT] dout rows
+          const int off = (int)((s0 - p0) % LANES);
+          for (int rl = (pl - off + LANES) % LANES; rl < rows; rl += LANES) {  // pixels p0 + pl, + LANES, ... in order
+            const int64_t m = s0 + rl;
+            const V8 a = unpack8(*reinterpret_cast<const uint4*>(ytile + rl * YP + c0));
+            const V8 bu = unpack8(*reinterpret_cast<const uint4*>(ytile + rl * YP + KOUT + c0));
+            if constexpr (MODE == STEM_GEMM) {
+              *reinterpret_cast<uint4*>(op.y + m * BN + c0) = *reinterpret_cast<const uint4*>(ytile + rl * YP + c0);
+              *reinterpret_cast<uint4*>(op.y + m * BN + KOUT + c0) = *reinterpret_cast<const uint4*>(ytile + rl * YP + KOUT + c0);
+            } else if constexpr (MODE == STEM_MOM) {
+#pragma unroll
+              for (int e = 0; e < 8; ++e) {
+                float s[5] = {sums[0][e], sums[1][e], sums[2][e], sums[3][e], sums[4][e]};
+                qarep_mom(a.v[e], bu.v[e], s);
+#pragma unroll
+                for (int k = 0; k < 5; ++k) sums[k][e] = s[k];
+              }
+            } else if constexpr (MODE == STEM_FWD) {
+              V8 o;
+#pragma unroll
+              for (int e = 0; e < 8; ++e) o.v[e] = qarep_out(a.v[e], bu.v[e], [&](int k) { return r[k][e]; }, d.act);
+              st8(op.outp + m * d.pitcho + d.offo + c0, o);
+            } else {
+              const V8 g = unpack8(*reinterpret_cast<const uint4*>(g_tile + rl * KOUT + c0));
+              if constexpr (MODE == STEM_BRED) {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                  float s[3] = {sums[0][e], sums[1][e], sums[2][e]};
+                  qarep_bwd_sums(d, g.v[e], a.v[e], bu.v[e], [&](int k) { return r[k][e]; }, s);
+#pragma unroll
+                  for (int k = 0; k < 3; ++k) sums[k][e] = s[k];
+                }
+              } else {
+                V8 o3, ou;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) qarep_bwd_grads(d, g.v[e], a.v[e], bu.v[e], [&](int k) { return r[k][e]; }, o3.v[e], ou.v[e]);
+                st8(op.dy3 + m * d.pitch3 + d.off3 + c0, o3);
+                st8(op.du + m * d.pitchu + d.offu + c0, ou);
+              }
+            }
+          }
+        }
+        stem_consumer_sync();  // the parked tile and the stage's dout rows are consumed
+        if (lane == 0) sm100::mbar_arrive(empty_bar(stg));
+        if (++stg == STEM_STAGES) {
+          stg = 0;
+          par ^= 1;
+        }
+      }
+      if constexpr (NACC > 0) {
+        // chan_body's combine: thread (pl, cvi) parks its sums, output (ci, a, e) adds them over pl in order, one fp64 atomic per range
+        if (active) {
+#pragma unroll
+          for (int a = 0; a < NACC; ++a)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) sred[(pl * CVB + cvi) * (NACC * 8 + 1) + a * 8 + e] = sums[a][e];
+        }
+        stem_consumer_sync();
+        for (int j = t; j < CVB * NACC * 8; j += TPB) {
+          float sum = 0.f;
+          const int ci = j / (NACC * 8), a = (j / 8) % NACC, e = j % 8;
+          for (int q = 0; q < LANES; ++q) sum += sred[(q * CVB + ci) * (NACC * 8 + 1) + a * 8 + e];
+          atomicAdd(&op.out[(int64_t)a * op.out_stride + ci * 8 + e], (double)sum);
+        }
+        stem_consumer_sync();
+      }
+    }
+  }
+}
+
+long long g_stem_launches = 0;
+
+// xp: [M][32] bf16 patches (dense), w: [2K][32] bf16, dout: [M] rows of K bf16 at pitch `gpitch` (backward modes only).  nranges:
+// the reductions' pixel ranges (the grid of the fused chan launch they replace); the other modes take one 128-pixel chunk per range.
+template <int KOUT, int MODE, class Op>
+int launch_stem_k(const Op& op, const SgbQarepDesc& d, const void* xp, const void* w, const void* dout, int gpitch, int nranges, cudaStream_t st) {
+  using Lay = StemLayout<KOUT, MODE, Op>;
+  if (int rc = sm100::init_driver()) return rc;
+  const size_t smem = Lay::smem();
+  static bool attr = false;
+  if (!attr) {
+    if (int rc = sgb_cuda_check(cudaFuncSetAttribute(stem_qarep_kernel<KOUT, MODE, Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "stem_qarep_kernel"))
+      return rc;
+    attr = true;
+  }
+  alignas(64) CUtensorMap map_x, map_w, map_g;
+  auto encode = [&](CUtensorMap* map, const void* p, uint64_t cols, uint64_t rows, uint64_t pitch, uint32_t bc, uint32_t br, CUtensorMapSwizzle sw) {
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {pitch * 2};
+    cuuint32_t box[2] = {bc, br};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = sm100::g_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      sgb_set_error("cuTensorMapEncodeTiled(stem) failed with %d (cols=%llu rows=%llu pitch=%llu)", (int)r, (unsigned long long)cols, (unsigned long long)rows,
+                    (unsigned long long)pitch);
+      return SGB_E_CUDA;
+    }
+    return SGB_OK;
+  };
+  if (int rc = encode(&map_x, xp, STEM_KP, d.M, STEM_KP, STEM_KP, STEM_BM, CU_TENSOR_MAP_SWIZZLE_64B)) return rc;
+  if (int rc = encode(&map_w, w, STEM_KP, 2 * KOUT, STEM_KP, STEM_KP, 2 * KOUT, CU_TENSOR_MAP_SWIZZLE_64B)) return rc;
+  map_g = map_x;
+  if (Lay::DOUT)
+    if (int rc = encode(&map_g, dout, KOUT, d.M, gpitch, KOUT, STEM_BM, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+  const int64_t per = nranges > 0 ? (d.M + nranges - 1) / nranges : STEM_BM;
+  const int64_t ranges = (d.M + per - 1) / per;
+  const int grid = (int)(ranges < sgb_sm_count() ? ranges : sgb_sm_count());
+  stem_qarep_kernel<KOUT, MODE, Op><<<grid, STEM_THREADS, smem, st>>>(map_x, map_w, map_g, op, d, d.M, per, (int)ranges);
+  ++g_stem_launches;
+  return sgb_cuda_check(cudaGetLastError(), "stem_qarep_kernel");
+}
+
+// The stem widths of the YOLO-NAS and YOLO-NAS-POSE recipes: 32, 48 and 64 output channels.
+template <int MODE, class Op>
+int launch_stem(const Op& op, const SgbQarepDesc& d, const void* xp, const void* w, const void* dout, int gpitch, int nranges, cudaStream_t st) {
+  switch (d.C) {
+    case 32: return launch_stem_k<32, MODE>(op, d, xp, w, dout, gpitch, nranges, st);
+    case 48: return launch_stem_k<48, MODE>(op, d, xp, w, dout, gpitch, nranges, st);
+    case 64: return launch_stem_k<64, MODE>(op, d, xp, w, dout, gpitch, nranges, st);
+  }
+  sgb_set_error("stem_qarep: %d output channels (32, 48 or 64 are served)", d.C);
+  return SGB_E_UNSUPPORTED;
+}
+
+int check_stem(const SgbQarepDesc* d, const void* xp, const void* w) {
+  SGB_REQUIRE(d && xp && w, "null pointer");
+  SGB_REQUIRE(d->C == 32 || d->C == 48 || d->C == 64, "stem_qarep: 32, 48 or 64 output channels");
+  SGB_REQUIRE(d->M > 0 && d->M < (1ll << 31) - STEM_BM, "stem_qarep: pixel count");
+  SGB_REQUIRE((((uintptr_t)xp | (uintptr_t)w) & 15) == 0, "stem_qarep: xp / w must be 16-byte aligned");
   return SGB_OK;
 }
 
@@ -864,4 +1181,62 @@ extern "C" int sgb_qarep_bwd_fused(const SgbQarepDesc* d, const sgb_bf16* dout, 
   QarepBwdRedOp ra{*d, (const bf16*)dout, (const bf16*)y3, (const bf16*)u, coef, sums, d->C};
   QarepBwdApplyOp ap{*d, (const bf16*)dout, (const bf16*)y3, (const bf16*)u, coef, sums, gamma3, gamma_p, (bf16*)dy3, (bf16*)du, dgamma3, dbeta3, dbias1a, dgamma_p, dbeta_p};
   return launch_chan_fused(ra, ap, d->M, d->C, (cudaStream_t)stream, "qarep_bwd_fused");
+}
+
+// ---------------------------------------------------------------------------------------------- QARepVGG stem on patches
+extern "C" int64_t sgb_stem_recompute_launches(void) { return (int64_t)g_stem_launches; }
+
+extern "C" int sgb_stem_gemm(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, sgb_bf16* y, void* stream) {
+  if (int rc = check_stem(d, xp, w)) return rc;
+  SGB_REQUIRE(y && ((uintptr_t)y & 15) == 0, "null or misaligned y");
+  StemGemmOp op{(bf16*)y};
+  return launch_stem<STEM_GEMM>(op, *d, xp, w, nullptr, 0, 0, (cudaStream_t)stream);
+}
+
+extern "C" int sgb_stem_qarep_moments(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, double* moments, void* stream) {
+  if (int rc = check_stem(d, xp, w)) return rc;
+  SGB_REQUIRE(moments, "null pointer");
+  QarepMomOp op{*d, nullptr, nullptr, moments, d->C};
+  size_t smem = 0;  // the moments half of sgb_qarep_fwd_fused: its pixel ranges, its summation order
+  const int nranges = chan_fused_grid<QarepMomOp, QarepFwdOp>(d->M, d->C, &smem, "stem_qarep_moments");
+  if (nranges < 0) return nranges;
+  return launch_stem<STEM_MOM>(op, *d, xp, w, nullptr, 0, nranges, (cudaStream_t)stream);
+}
+
+extern "C" int sgb_stem_qarep_fwd(const SgbQarepDesc* d, const sgb_bf16* xp, const sgb_bf16* w, const double* moments, const float* gamma3,
+                                  const float* beta3, const float* bias1_alpha, const float* gamma_p, const float* beta_p, float* rm3, float* rv3,
+                                  float* rm_p, float* rv_p, sgb_bf16* out, float* coef, void* stream) {
+  if (int rc = check_qarep(d)) return rc;
+  if (int rc = check_stem(d, xp, w)) return rc;
+  SGB_REQUIRE(!d->res, "stem_qarep_fwd: no shortcut");
+  SGB_REQUIRE(moments && gamma3 && beta3 && out && coef && ((uintptr_t)out & 15) == 0 && d->pitcho % 8 == 0, "null or misaligned pointer");
+  SGB_REQUIRE(!d->use_post_bn || (gamma_p && beta_p), "post_bn parameters missing");
+  QarepFwdOp op{*d, nullptr, nullptr, (bf16*)out, moments, gamma3, beta3, bias1_alpha, gamma_p, beta_p, rm3, rv3, rm_p, rv_p, coef};
+  return launch_stem<STEM_FWD>(op, *d, xp, w, nullptr, 0, 0, (cudaStream_t)stream);
+}
+
+extern "C" int sgb_stem_qarep_bwd_reduce(const SgbQarepDesc* d, const sgb_bf16* dout, const sgb_bf16* xp, const sgb_bf16* w, const float* coef,
+                                         double* sums, void* stream) {
+  if (int rc = check_qarep(d)) return rc;
+  if (int rc = check_stem(d, xp, w)) return rc;
+  SGB_REQUIRE(dout && coef && sums && ((uintptr_t)dout & 15) == 0, "null or misaligned pointer");
+  QarepBwdRedOp op{*d, nullptr, nullptr, nullptr, coef, sums, d->C};
+  size_t smem = 0;  // the reduction half of sgb_qarep_bwd_fused: its pixel ranges, its summation order
+  const int nranges = chan_fused_grid<QarepBwdRedOp, QarepBwdApplyOp>(d->M, d->C, &smem, "stem_qarep_bwd_reduce");
+  if (nranges < 0) return nranges;
+  return launch_stem<STEM_BRED>(op, *d, xp, w, (const bf16*)dout + (d->pitchd ? d->offd : d->offo), d->pitchd ? d->pitchd : d->pitcho, nranges,
+                                (cudaStream_t)stream);
+}
+
+extern "C" int sgb_stem_qarep_bwd_apply(const SgbQarepDesc* d, const sgb_bf16* dout, const sgb_bf16* xp, const sgb_bf16* w, const float* coef,
+                                        const double* sums, const float* gamma3, const float* gamma_p, sgb_bf16* dy3, sgb_bf16* du, float* dgamma3,
+                                        float* dbeta3, float* dbias1a, float* dgamma_p, float* dbeta_p, void* stream) {
+  if (int rc = check_qarep(d)) return rc;
+  if (int rc = check_stem(d, xp, w)) return rc;
+  SGB_REQUIRE(dout && coef && sums && gamma3 && dy3 && du && ((uintptr_t)dout & 15) == 0 && (((uintptr_t)dy3 | (uintptr_t)du) & 15) == 0,
+              "null or misaligned pointer");
+  SGB_REQUIRE(!d->use_post_bn || gamma_p, "gamma_p missing");
+  QarepBwdApplyOp op{*d, nullptr, nullptr, nullptr, coef, sums, gamma3, gamma_p, (bf16*)dy3, (bf16*)du, dgamma3, dbeta3, dbias1a, dgamma_p, dbeta_p};
+  return launch_stem<STEM_BAPPLY>(op, *d, xp, w, (const bf16*)dout + (d->pitchd ? d->offd : d->offo), d->pitchd ? d->pitchd : d->pitcho, 0,
+                                  (cudaStream_t)stream);
 }

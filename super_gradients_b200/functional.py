@@ -909,6 +909,7 @@ def qarepvgg_block(x, w3, g3, b3, w1, bias1, alpha, gp, bp, cfg):
 
 # ------------------------------------------------------------------------------------------------------------ QARepVGG stem on patches
 STEM_PATCHES = [True]  # False: the direct convolution, which test_patch_stem_is_the_same_block compares against
+STEM_RECOMPUTE = [True]  # False: [y3 | u] stored by the patch GEMM and read by the passes, which test_stem_recompute_gpu.py compares against
 
 
 def stem_patch_channels(cin: int, r: int) -> int:
@@ -945,25 +946,39 @@ class _QARepVGGStem(torch.autograd.Function):
             st[kout:, ctr : ctr + cin].copy_(w1.detach()[:, :, 0, 0])
 
         kf, _ = cfg.cache_stem.get((w3, w1), [(2 * kout, c_out, 1, 1)], c_out, fill)
-        ycat = K.conv_fprop(xp, kf, 2 * kout, 1, 1, 1, 0)
-        y3, u = ycat[:, :kout], ycat[:, kout:]
-        out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True, **_kw(sync=cfg.sync))
+        # the recompute kernels have no stand-in in the tests' CPU backend, which runs this Function on host tensors
+        recompute = STEM_RECOMPUTE[0] and xp.is_cuda and c_out == 32 and kout in (32, 48, 64)
+        if recompute:  # [y3 | u] is never stored: the four passes recompute it from xp
+            out, coef = K.stem_qarep_fwd(xp, kf, kout, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.momentum, cfg.act, **_kw(sync=cfg.sync))
+            saved = (xp, kf, coef, g3, gp)
+        else:
+            ycat = K.conv_fprop(xp, kf, 2 * kout, 1, 1, 1, 0)
+            y3, u = ycat[:, :kout], ycat[:, kout:]
+            out, coef = K.qarep_fwd(y3, u, g3, b3, bias1, gp, bp, cfg.rm3, cfg.rv3, cfg.rmp, cfg.rvp, cfg.eps, cfg.eps, cfg.momentum, cfg.act, True, **_kw(sync=cfg.sync))
+            saved = (xp, y3, u, out, coef, g3, gp)
         _bump_batches_tracked(*cfg.nbt)
-        ctx.save_for_backward(xp, y3, u, out, coef, g3, gp)
-        ctx.cfg, ctx.geom, ctx.has_bias = cfg, (kout, cin, r, s), bias1 is not None
+        ctx.save_for_backward(*saved)
+        ctx.cfg, ctx.geom, ctx.has_bias, ctx.recompute = cfg, (kout, cin, r, s), bias1 is not None, recompute
         ctx.slots = (_mg(w3), _mg(g3), _mg(b3), _mg(w1), _mg(bias1), _mg(gp), _mg(bp))
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        xp, y3, u, out, coef, g3, gp = ctx.saved_tensors
         cfg = ctx.cfg
         kout, cin, r, s = ctx.geom
         sw3, sg3, sb3, sw1, sbias, sgp, sbp = ctx.slots
-        n, _, h, w = y3.shape
-        dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
-        _dy3, _du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(dout, out, y3, u, coef, g3, gp, cfg.eps, cfg.eps, cfg.act, True, acc=(sg3, sb3, sbias, sgp, sbp),
-                                                         out_grads=(dcat[:, :kout], dcat[:, kout:]), **_kw(sync=cfg.sync))  # fmt: skip
+        acc = (sg3, sb3, sbias, sgp, sbp)
+        if ctx.recompute:
+            xp, kf, coef, g3, gp = ctx.saved_tensors
+            n, _, h, w = xp.shape
+            dcat = K.empty_nhwc(n, 2 * kout, h, w, xp.device)
+            dg3, db3, dab, dgp, dbp = K.stem_qarep_bwd(dout, xp, kf, kout, coef, g3, gp, cfg.eps, cfg.act, dcat, acc=acc, **_kw(sync=cfg.sync))
+        else:
+            xp, y3, u, out, coef, g3, gp = ctx.saved_tensors
+            n, _, h, w = y3.shape
+            dcat = K.empty_nhwc(n, 2 * kout, h, w, y3.device)
+            _dy3, _du, dg3, db3, dab, dgp, dbp = K.qarep_bwd(dout, out, y3, u, coef, g3, gp, cfg.eps, cfg.eps, cfg.act, True, acc=acc,
+                                                             out_grads=(dcat[:, :kout], dcat[:, kout:]), **_kw(sync=cfg.sync))  # fmt: skip
         ((dw3, dw1),) = _wgrad(xp, dcat, 1, 1, 1, 0, cin, ("stem", (kout, r, s), (sw3, sw1)))
         return None, dw3, _unless_slot(sg3, dg3), _unless_slot(sb3, db3), dw1, (_unless_slot(sbias, dab) if ctx.has_bias else None), _unless_slot(sgp, dgp), _unless_slot(sbp, dbp), None
 

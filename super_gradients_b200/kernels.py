@@ -844,6 +844,70 @@ def qarep_bwd(dout, out, y3, u, coef, gamma3, gamma_p, eps3, eps_post, act, use_
     return dy3, du, dg3, db3, dab, dgp, dbp
 
 
+def _stem_desc(xp, w, kout, eps, momentum, act, use_post_bn=True) -> L.QarepDesc:
+    """Desc of the stem passes that recompute [y3 | u] = xp @ w^T: xp a dense [N, 32, H, W] patch tensor, w the [2 kout, 32] bf16 filter."""
+    n, c, h, wd = xp.shape
+    if c != 32 or nhwc_pitch(xp) != 32 or xp.dtype != torch.bfloat16 or w.dtype != torch.bfloat16 or w.numel() != 2 * kout * 32 or not w.is_contiguous():
+        raise L.SgbError("stem_qarep: xp must be a dense 32-channel bf16 patch tensor and w a contiguous [2K, 32] bf16 filter")
+    d = L.QarepDesc()
+    d.M, d.C = n * h * wd, kout
+    d.eps3, d.eps_post, d.momentum = eps, eps, momentum
+    d.act = act_code(act)
+    d.use_post_bn = 1 if use_post_bn else 0
+    return d
+
+
+def stem_gemm(xp, w, kout):
+    """[y3 | u] exactly as the stem passes recompute it (and as conv_fprop(xp, w, 2 kout, 1, 1, 1, 0) stores it): for tests."""
+    n, _, h, wd = xp.shape
+    y = empty_nhwc(n, 2 * kout, h, wd, xp.device)
+    d = _stem_desc(xp, w, kout, 0.0, 0.0, ACT_NONE)
+    _timed("sgb_stem_gemm", ctypes.byref(d), _ptr(xp), _ptr(w), _ptr(y), _stream())
+    return y
+
+
+def stem_qarep_fwd(xp, w, kout, gamma3, beta3, bias1a, gamma_p, beta_p, rm3, rv3, rmp, rvp, eps, momentum, act, sync=None):
+    """qarep_fwd of the QARepVGG stem on patches without [y3 | u] in memory: the moments pass and the apply pass each recompute it from
+    xp and w.  Returns (out, coef).  sync: as qarep_fwd's, the moments and the local count are all-reduced between the two passes."""
+    n, _, h, wd = xp.shape
+    out = empty_nhwc(n, kout, h, wd, xp.device)
+    d = _stem_desc(xp, w, kout, eps, momentum, act)
+    d.pitcho, d.offo = nhwc_pitch(out), 0
+    coef = torch.empty((9, kout), dtype=torch.float32, device=xp.device)
+    buf = new_sync_sums(5 * kout, d.M, xp.device) if sync is not None else None
+    mom = buf[:-1].view(5, kout) if buf is not None else zeros((5, kout), torch.float64, xp.device)
+    _timed("sgb_stem_qarep_moments", ctypes.byref(d), _ptr(xp), _ptr(w), _ptr(mom), _stream())
+    if sync is not None:
+        sync(buf)
+        sync.count = buf[-1:]
+        d.count, d.param_scale = sync.count.data_ptr(), sync.param_scale
+    _timed("sgb_stem_qarep_fwd", ctypes.byref(d), _ptr(xp), _ptr(w), _ptr(mom), _ptr(gamma3), _ptr(beta3), _ptr(bias1a), _ptr(gamma_p), _ptr(beta_p), _ptr(rm3), _ptr(rv3), _ptr(rmp), _ptr(rvp), _ptr(out), _ptr(coef), _stream())
+    return out, coef
+
+
+def stem_qarep_bwd(dout, xp, w, kout, coef, gamma3, gamma_p, eps, act, dcat, acc=None, sync=None):
+    """qarep_bwd of the QARepVGG stem on patches: both passes recompute [y3 | u] from xp and w.  Writes [dy3 | du] into dcat (a dense
+    [N, 2 kout, H, W] tensor) and returns dgamma3, dbeta3, dbias1a, dgamma_p, dbeta_p (accumulated into `acc`'s tensors where given).
+    sync: the forward's functional.BnSync -- the three sums are all-reduced by sync(sums) between the two passes."""
+    if act_code(act) not in (ACT_NONE, ACT_RELU):
+        raise L.SgbError("stem_qarep_bwd: only identity / ReLU activations have a backward pass in super_gradients_b200")
+    dout = as_nhwc(dout)
+    d = _stem_desc(xp, w, kout, eps, 0.0, act)
+    d.pitcho, d.offo = nhwc_pitch(dout), 0
+    if tuple(dcat.shape) != (xp.shape[0], 2 * kout, xp.shape[2], xp.shape[3]) or nhwc_pitch(dcat) != 2 * kout:
+        raise L.SgbError("stem_qarep_bwd: dcat must be a dense [N, 2K, H, W] NHWC tensor")
+    d.pitch3, d.pitchu = 2 * kout, 2 * kout
+    sums = zeros((3, kout), torch.float64, xp.device)
+    _timed("sgb_stem_qarep_bwd_reduce", ctypes.byref(d), _ptr(dout), _ptr(xp), _ptr(w), _ptr(coef), _ptr(sums), _stream())
+    if sync is not None:
+        sync(sums)
+        d.count, d.param_scale = sync.count.data_ptr(), sync.param_scale
+    z = lambda: zeros((kout,), torch.float32, xp.device)  # noqa: E731
+    dg3, db3, dab, dgp, dbp = [a if a is not None else z() for a in (acc or (None,) * 5)]
+    _timed("sgb_stem_qarep_bwd_apply", ctypes.byref(d), _ptr(dout), _ptr(xp), _ptr(w), _ptr(coef), _ptr(sums), _ptr(gamma3), _ptr(gamma_p), _ptr(dcat), _ptr(dcat[:, kout:]), _ptr(dg3), _ptr(db3), _ptr(dab), _ptr(dgp), _ptr(dbp), _stream())
+    return dg3, db3, dab, dgp, dbp
+
+
 # ------------------------------------------------------------------------------------------------ pooling / misc
 def maxpool_fwd(x, k, stride, pad, want_idx=True, out=None):
     n, c, h, w = x.shape

@@ -190,6 +190,12 @@ _SIGNATURES = {
     "sgb_qarep_bwd_reduce": (c_int, [POINTER(QarepDesc), P, P, P, P, P, P, P]),
     "sgb_qarep_bwd_apply": (c_int, [POINTER(QarepDesc)] + [P] * 16),
     "sgb_qarep_bwd_fused": (c_int, [POINTER(QarepDesc)] + [P] * 15),
+    "sgb_stem_gemm": (c_int, [POINTER(QarepDesc), P, P, P, P]),
+    "sgb_stem_qarep_moments": (c_int, [POINTER(QarepDesc), P, P, P, P]),
+    "sgb_stem_qarep_fwd": (c_int, [POINTER(QarepDesc)] + [P] * 15),
+    "sgb_stem_qarep_bwd_reduce": (c_int, [POINTER(QarepDesc)] + [P] * 6),
+    "sgb_stem_qarep_bwd_apply": (c_int, [POINTER(QarepDesc)] + [P] * 15),
+    "sgb_stem_recompute_launches": (c_int64, []),
     "sgb_maxpool_fwd": (c_int, [P, _I, _I, _I, _I, _I, _I, _I, _I, _I, P, _I, _I, _I, _I, P, P]),
     "sgb_maxpool_bwd": (c_int, [P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, P, P, P]),
     "sgb_maxpool_bwd_bf16": (c_int, [P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, P, P, _I, P]),
@@ -244,7 +250,7 @@ _SIGNATURES = {
 _lib = None
 
 # kernels launched by one call of each entry point (default 1); LAUNCHES[0] accumulates them (bench.py: gpu_launches)
-LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_lamb_step": 2, "sgb_clip_grad_norm": 2, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_conv_wgrad_halo_launches": 0, "sgb_conv_wgrad_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
+LAUNCH_COUNT = {"sgb_tal_assign": 4, "sgb_lamb_step": 2, "sgb_clip_grad_norm": 2, "sgb_atss_assign": 3, "sgb_pose_tal_assign": 4, "sgb_sm100_launches": 0, "sgb_stem_recompute_launches": 0, "sgb_conv_halo_launches": 0, "sgb_conv_force_im2col": 0, "sgb_conv_wgrad_halo_launches": 0, "sgb_conv_wgrad_force_im2col": 0, "sgb_sliding_window_merge_workspace_bytes": 0, "sgb_sliding_window_merge_launches": 0, "sgb_last_error": 0, "sgb_version": 0, "sgb_check_device": 0}
 LAUNCHES = [0]
 
 
