@@ -747,9 +747,10 @@ int sgb_classify_rows(const void* logits, int64_t N, int32_t C, int64_t row_stri
                       int32_t* label, float* confidence, void* stream);
 
 /* ---- optimizer over the flat parameter buffer (sg_trainer.py:634-644) --------------------------------------- */
-/* Hyper-parameters live in DEVICE memory (so a CUDA-graph-captured step follows the host-side LR schedule):
- *   sgd   hp[5] = {lr, momentum, weight_decay, grad_scale, nesterov}
- *   adamw hp[8] = {lr, beta1, beta2, eps, weight_decay, 1-beta1^t, 1-beta2^t, grad_scale}   (torch.optim semantics) */
+/* Hyper-parameters live in DEVICE memory (so a CUDA-graph-captured step follows the host-side LR schedule).  hp is ONE device
+ * float32 row in the layout of csrc/optim_math.cuh, grad_scale included:
+ *   sgd   SGD_*     torch.optim.SGD
+ *   adamw ADAMW_*   torch.optim.AdamW */
 int sgb_sgd_step(float* p, const float* g, float* mom, int64_t n, const float* hp, void* stream);
 int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream);
 /* The other optimizers of the reference's registry (common/object_names.py:143-152), one launch per weight-decay range.  hp is ONE
@@ -781,7 +782,7 @@ int sgb_lamb_step(float* p, const float* g, float* m, float* v, float* update, i
 /* clip_grad_norm (sg_trainer.py:634-636; the value is refused when <= 0, :1416-1417): torch.nn.utils.clip_grad_norm_ with norm
  * type 2 over every live gradient, run once per optimisation step after the all-reduce and before the optimizer.  The gradients
  * are not rewritten: the coefficient is folded into the optimizer's grad_scale, column gs_col of both hp rows (hp is the
- * optimizer's device table of two hp_len-wide rows: sgd 3, adamw 7, ADAM_GS / RMS_GS / RTF_GS / LION_GS / LAMB_GS of
+ * optimizer's device table of two hp_len-wide rows: SGD_GS / ADAMW_GS / ADAM_GS / RMS_GS / RTF_GS / LION_GS / LAMB_GS of
  * csrc/optim_math.cuh).  chunks / nchunk: the chunk table of sgb_lamb_step; partials: device float64 [nchunk].
  *   launch 1  partials[c] = sum over chunk c of (g * hp[gs_col])^2                       (the kernel of sgb_lamb_grad_sqnorm)
  *   launch 2  one CTA: total = (float)sqrt(sum of partials, float64, fixed order);

@@ -1,8 +1,8 @@
 // Memory-bound companions of the convolution GEMMs: weight layout/cast, NCHW<->NHWC, train/infer BatchNorm with
-// fused residual + activation (forward and both backward passes), the QARepVGG branch algebra, pooling, axpby and
-// the flat-buffer optimizers.  All tensors are NHWC bf16 with channel pitch/offset; every kernel moves 16-byte
-// vectors (8 channels) per thread with consecutive threads on consecutive channel vectors (coalesced), per-channel
-// reductions go registers -> shared atomics -> one fp64 global atomic per channel per CTA.
+// fused residual + activation (forward and both backward passes), the QARepVGG branch algebra, pooling and axpby.
+// All tensors are NHWC bf16 with channel pitch/offset; every kernel moves 16-byte vectors (8 channels) per thread with
+// consecutive threads on consecutive channel vectors (coalesced), per-channel reductions go registers -> shared
+// atomics -> one fp64 global atomic per channel per CTA.
 #include "common.cuh"
 #include "stream_ring.cuh"
 
@@ -795,43 +795,6 @@ __global__ void avgpool_bwd_kernel(const bf16* __restrict__ dy, int N, int HW, i
   }
 }
 
-// ---------------------------------------------------------------------------------------------- optimizers
-// Hyper-parameters are read from DEVICE memory so that a CUDA-graph-captured step follows the host's LR schedule.
-// sgd   hp: [lr, momentum, weight_decay, grad_scale, nesterov]
-// adamw hp: [lr, beta1, beta2, eps, weight_decay, 1-beta1^t, 1-beta2^t, grad_scale]
-__global__ void sgd_kernel(float* p, const float* g, float* mom, int64_t n, const float* hp) {
-  const float lr = hp[0], mu = hp[1], wd = hp[2], gs = hp[3];
-  const bool nesterov = hp[4] != 0.f;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    float gr = g[i] * gs + wd * p[i];
-    float d = gr;
-    if (mu != 0.f) {
-      float b = mu * mom[i] + gr;
-      mom[i] = b;
-      d = nesterov ? gr + mu * b : b;
-    }
-    p[i] -= lr * d;
-  }
-}
-__global__ void adamw_kernel(float* p, const float* g, float* m, float* v, int64_t n, const float* hp) {
-  const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4], bc1 = hp[5], bc2 = hp[6], gs = hp[7];
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    float gr = g[i] * gs;
-    float pi = p[i] * (1.f - lr * wd);
-    float mi = b1 * m[i] + (1.f - b1) * gr;
-    float vi = b2 * v[i] + (1.f - b2) * gr * gr;
-    m[i] = mi;
-    v[i] = vi;
-    float denom = sqrtf(vi) / sqrtf(bc2) + eps;
-    p[i] = pi - (lr / bc1) * mi / denom;
-  }
-}
-__global__ void ema_kernel(float* e, const float* p, int64_t n, const float* decay) {
-  const float d = *decay;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    e[i] = e[i] * d + (1.f - d) * p[i];
-}
-
 }  // namespace
 
 // ================================================================================================== C ABI
@@ -1026,24 +989,5 @@ extern "C" int sgb_avgpool_bwd(const sgb_bf16* dy, int N, int HW, int C, sgb_bf1
   avgpool_bwd_kernel<<<grid_for((int64_t)N * HW * C), TPB, 0, (cudaStream_t)stream>>>((const bf16*)dy, N, HW, C,
                                                                                      (bf16*)dx);
   SGB_LAUNCH_CHECK("avgpool_bwd_kernel");
-  return SGB_OK;
-}
-
-extern "C" int sgb_sgd_step(float* p, const float* g, float* mom, int64_t n, const float* hp, void* stream) {
-  SGB_REQUIRE(p && g && mom && hp, "null pointer");
-  sgd_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, mom, n, hp);
-  SGB_LAUNCH_CHECK("sgd_kernel");
-  return SGB_OK;
-}
-extern "C" int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream) {
-  SGB_REQUIRE(p && g && m && v && hp, "null pointer");
-  adamw_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, m, v, n, hp);
-  SGB_LAUNCH_CHECK("adamw_kernel");
-  return SGB_OK;
-}
-extern "C" int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream) {
-  SGB_REQUIRE(ema && p && decay, "null pointer");
-  ema_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(ema, p, n, decay);
-  SGB_LAUNCH_CHECK("ema_kernel");
   return SGB_OK;
 }

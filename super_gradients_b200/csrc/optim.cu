@@ -1,6 +1,8 @@
-// Adam, RMSprop, RMSpropTF, Lion and Lamb over the flat fp32 parameter / gradient buffers (training/flat_state.py).  The
-// per-element arithmetic is optim_math.cuh; hyper-parameters are read from DEVICE memory so a CUDA-graph-captured step follows
-// the host's schedule.  The elementwise optimizers are one grid-stride pass per weight-decay range, like adamw_kernel.
+// SGD, AdamW, Adam, RMSprop, RMSpropTF, Lion and Lamb over the flat fp32 parameter / gradient buffers (training/flat_state.py),
+// and the EMA update.  Hyper-parameters are read from DEVICE memory, one row per weight-decay range in the layouts of
+// optim_math.cuh, so a CUDA-graph-captured step follows the host's schedule.  The per-element arithmetic of Adam, RMSprop,
+// RMSpropTF, Lion and Lamb is optim_math.cuh's; sgd_kernel, adamw_kernel and ema_kernel spell theirs with plain operators, which
+// nvcc contracts into FMAs (g * gs + wd * p is one).  The elementwise optimizers are one grid-stride pass per weight-decay range.
 //
 // Lamb needs a global gradient norm and per-tensor norms of p and of the update.  Every reduction runs over a chunk table
 // (fused_optimizers.lamb_chunk_table: {start, len, first chunk of its tensor, chunks of its tensor}; a chunk lies inside one
@@ -26,6 +28,40 @@ inline int grid_for(int64_t work, int per_cta = TPB * 4, int max_ctas = 132 * 8)
   if (g > max_ctas) g = max_ctas;
   if (g < 1) g = 1;
   return (int)g;
+}
+
+__global__ void sgd_kernel(float* p, const float* g, float* mom, int64_t n, const float* hp) {
+  const float lr = hp[SGD_LR], mu = hp[SGD_MOMENTUM], wd = hp[SGD_WD], gs = hp[SGD_GS];
+  const bool nesterov = hp[SGD_NESTEROV] != 0.f;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float gr = g[i] * gs + wd * p[i];
+    float d = gr;
+    if (mu != 0.f) {
+      float b = mu * mom[i] + gr;
+      mom[i] = b;
+      d = nesterov ? gr + mu * b : b;
+    }
+    p[i] -= lr * d;
+  }
+}
+__global__ void adamw_kernel(float* p, const float* g, float* m, float* v, int64_t n, const float* hp) {
+  const float lr = hp[ADAMW_LR], b1 = hp[ADAMW_B1], b2 = hp[ADAMW_B2], eps = hp[ADAMW_EPS], wd = hp[ADAMW_WD], bc1 = hp[ADAMW_BC1], bc2 = hp[ADAMW_BC2],
+              gs = hp[ADAMW_GS];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float gr = g[i] * gs;
+    float pi = p[i] * (1.f - lr * wd);
+    float mi = b1 * m[i] + (1.f - b1) * gr;
+    float vi = b2 * v[i] + (1.f - b2) * gr * gr;
+    m[i] = mi;
+    v[i] = vi;
+    float denom = sqrtf(vi) / sqrtf(bc2) + eps;
+    p[i] = pi - (lr / bc1) * mi / denom;
+  }
+}
+__global__ void ema_kernel(float* e, const float* p, int64_t n, const float* decay) {
+  const float d = *decay;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    e[i] = e[i] * d + (1.f - d) * p[i];
 }
 
 __global__ void __launch_bounds__(TPB) adam_kernel(float* p, const float* g, float* m, float* v, int64_t n, const float* hp) {
@@ -173,6 +209,25 @@ __global__ void __launch_bounds__(TPB) lamb_apply_kernel(float* __restrict__ p, 
 }  // namespace
 
 // ================================================================================================== C ABI
+extern "C" int sgb_sgd_step(float* p, const float* g, float* mom, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && mom && hp, "null pointer");
+  sgd_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, mom, n, hp);
+  SGB_LAUNCH_CHECK("sgd_kernel");
+  return SGB_OK;
+}
+extern "C" int sgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream) {
+  SGB_REQUIRE(p && g && m && v && hp, "null pointer");
+  adamw_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(p, g, m, v, n, hp);
+  SGB_LAUNCH_CHECK("adamw_kernel");
+  return SGB_OK;
+}
+extern "C" int sgb_ema_update(float* ema, const float* p, int64_t n, const float* decay, void* stream) {
+  SGB_REQUIRE(ema && p && decay, "null pointer");
+  ema_kernel<<<grid_for(n, TPB * 4), TPB, 0, (cudaStream_t)stream>>>(ema, p, n, decay);
+  SGB_LAUNCH_CHECK("ema_kernel");
+  return SGB_OK;
+}
+
 extern "C" int sgb_adam_step(float* p, const float* g, float* m, float* v, int64_t n, const float* hp, void* stream) {
   SGB_REQUIRE(p && g && m && v && hp, "null pointer");
   SGB_REQUIRE(n >= 0, "n must be >= 0");

@@ -1,6 +1,7 @@
-// Per-element arithmetic of the flat-buffer optimizers Adam, RMSprop, RMSpropTF, Lion and Lamb, and of clip_grad_norm's
-// coefficient, host+device: the CUDA kernels in optim.cu run it per element, and the CPU suite compiles this header with g++
-// (-ffp-contract=off) behind serial drivers (tests/host_kernels/optim_host.cpp, clip_host.cpp).
+// The hyper-parameter rows of all seven flat-buffer optimizers, and the per-element arithmetic of Adam, RMSprop, RMSpropTF, Lion
+// and Lamb and of clip_grad_norm's coefficient, host+device: the CUDA kernels in optim.cu run it per element, and the CPU suite
+// compiles this header with g++ (-ffp-contract=off) behind serial drivers (tests/host_kernels/optim_host.cpp, clip_host.cpp).
+// SGD and AdamW keep their arithmetic in their kernels in optim.cu, written with plain operators that nvcc contracts into FMAs.
 //
 // Each function restates, op for op, the reference's single-tensor CPU step in float32 (torch.optim.Adam / RMSprop, and the
 // RMSpropTF, Lion and Lamb classes of training/utils/optimizers/).  torch's CPU kernels round as follows, and so does this header:
@@ -27,6 +28,10 @@
 namespace sgb_optim {
 
 // ---- hyper-parameter rows (float32, one row per weight-decay group; row 1 is the zero-decay group)
+// sgd:        torch.optim.SGD; nesterov is 0 or 1
+enum { SGD_LR, SGD_MOMENTUM, SGD_WD, SGD_GS, SGD_NESTEROV, SGD_HP };
+// adamw:      torch.optim.AdamW; bc1 = 1 - beta1^t, bc2 = 1 - beta2^t
+enum { ADAMW_LR, ADAMW_B1, ADAMW_B2, ADAMW_EPS, ADAMW_WD, ADAMW_BC1, ADAMW_BC2, ADAMW_GS, ADAMW_HP };
 // adam:       torch.optim.Adam, L2-coupled decay
 enum { ADAM_WD, ADAM_W1, ADAM_B2, ADAM_1MB2, ADAM_NEG_STEP, ADAM_BC2_SQRT, ADAM_EPS, ADAM_GS, ADAM_HP };
 // rmsprop:    torch.optim.RMSprop (zero-initialised square_avg, eps outside the sqrt)

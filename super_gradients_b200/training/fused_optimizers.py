@@ -1,18 +1,20 @@
-"""Adam, RMSprop, RMSpropTF, Lion and Lamb on the flat parameter buffer: their constructor arguments, state tensors and the
-per-step hyper-parameter rows of the csrc/optim.cu kernels (arithmetic: csrc/optim_math.cuh).
+"""SGD, AdamW, Adam, RMSprop, RMSpropTF, Lion and Lamb on the flat parameter buffer: their constructor arguments, state tensors and
+the per-step hyper-parameter rows of the csrc/optim.cu kernels (row layouts and most of the arithmetic: csrc/optim_math.cuh).
 
 The reference builds these with build_optimizer (training/utils/optimizer_utils.py:88-141): the registry defaults of
 training/params.py:88-94 are merged under the user's optimizer_params, and with zero_weight_decay_on_bias_and_bn the decay group
 gets `optimizer_params.get("weight_decay", 0.0)` -- not the class default -- while the other group gets 0.  Every scalar the
-kernels read is derived here in double (Python floats, as torch.optim computes them) and rounded to float32 once.
+kernels read is derived here in double (Python floats, as torch.optim computes them) and rounded to float32 once.  SGD and AdamW
+take the merged optimizer_params as they are: unknown keys are ignored, and the decay group gets the merged weight_decay.
 """
 import math
 from typing import Any, List, Mapping
 
 import torch
 
-# registry defaults merged under the user's optimizer_params (training/params.py:90-94, optimizer_utils.py:24-29)
-REGISTRY_DEFAULTS = {"Adam": {"weight_decay": 1e-4}, "RMSprop": {"weight_decay": 1e-4, "momentum": 0.9}, "RMSpropTF": {"weight_decay": 1e-4, "momentum": 0.9}}
+# registry defaults merged under the user's optimizer_params (training/params.py:84-94, optimizer_utils.py:24-29)
+REGISTRY_DEFAULTS = {"SGD": {"weight_decay": 1e-4, "momentum": 0.9}, "AdamW": {"weight_decay": 1e-2}, "Adam": {"weight_decay": 1e-4},
+                     "RMSprop": {"weight_decay": 1e-4, "momentum": 0.9}, "RMSpropTF": {"weight_decay": 1e-4, "momentum": 0.9}}
 
 # constructor defaults: torch.optim.Adam / RMSprop, and training/utils/optimizers/{rmsprop_tf,lion,lamb}.py
 CLASS_DEFAULTS = {
@@ -26,7 +28,9 @@ CLASS_DEFAULTS = {
              "trust_clip": False, "always_adapt": False},
 }  # fmt: skip
 
+# the optimizers whose constructor arguments are checked against CLASS_DEFAULTS
 NAMES = tuple(CLASS_DEFAULTS)
+ALL_NAMES = ("SGD", "AdamW") + NAMES
 
 # elements per Lamb reduction chunk (a chunk never spans two parameter tensors)
 LAMB_CHUNK = 16384
@@ -34,8 +38,12 @@ LAMB_CHUNK = 16384
 
 def resolve(name: str, optimizer_params: Mapping[str, Any], zero_wd_on_bias_and_bn: bool):
     """-> (merged constructor arguments, weight decay of the decay group).  Refuses what the constructor would refuse, and the
-    arguments that change torch's arithmetic beyond what the kernels implement."""
+    arguments that change torch's arithmetic beyond what the kernels implement (NAMES only)."""
+    if name not in ALL_NAMES:
+        raise NotImplementedError(f"optimizer {name} has no fused kernel ({', '.join(ALL_NAMES)} are implemented)")
     explicit = {**REGISTRY_DEFAULTS.get(name, {}), **dict(optimizer_params)}
+    if name in ("SGD", "AdamW"):
+        return explicit, float(explicit.get("weight_decay", 0.0))
     unknown = sorted(set(explicit) - set(CLASS_DEFAULTS[name]))
     if unknown:
         raise TypeError(f"{name}.__init__() got an unexpected keyword argument '{unknown[0]}'")
@@ -48,12 +56,13 @@ def resolve(name: str, optimizer_params: Mapping[str, Any], zero_wd_on_bias_and_
 
 
 def state_tensors(name: str, op: Mapping[str, Any], like: torch.Tensor) -> List[torch.Tensor]:
-    """The persistent per-element state, in checkpoint order: Adam / Lamb [exp_avg, exp_avg_sq]; RMSprop / RMSpropTF [square_avg,
-    momentum_buffer if momentum > 0, grad_avg if centered] (RMSpropTF's square_avg starts at ones); Lion [exp_avg]."""
+    """The persistent per-element state, in checkpoint order: SGD [momentum_buffer] (also with momentum 0); AdamW / Adam / Lamb
+    [exp_avg, exp_avg_sq]; RMSprop / RMSpropTF [square_avg, momentum_buffer if momentum > 0, grad_avg if centered] (RMSpropTF's
+    square_avg starts at ones); Lion [exp_avg]."""
     z = lambda: torch.zeros_like(like)  # noqa: E731
-    if name in ("Adam", "Lamb"):
+    if name in ("AdamW", "Adam", "Lamb"):
         return [z(), z()]
-    if name == "Lion":
+    if name in ("SGD", "Lion"):
         return [z()]
     sq = torch.ones_like(like) if name == "RMSpropTF" else z()
     return [sq] + ([z()] if float(op["momentum"]) > 0 else []) + ([z()] if op["centered"] else [])
@@ -64,7 +73,12 @@ def hyper_param_rows(name: str, op: Mapping[str, Any], wd: float, lr: float, ste
     lr, t, gs = float(lr), int(step), float(grad_scale)
     rows = []
     for w in (wd, 0.0):
-        if name == "Adam":
+        if name == "SGD":
+            rows.append([lr, float(op.get("momentum", 0.0)), w, gs, float(bool(op.get("nesterov", False)))])
+        elif name == "AdamW":
+            b1, b2 = op.get("betas", (0.9, 0.999))
+            rows.append([lr, b1, b2, float(op.get("eps", 1e-8)), w, 1 - b1**t, 1 - b2**t, gs])
+        elif name == "Adam":
             b1, b2 = (float(b) for b in op["betas"])
             rows.append([w, 1 - b1, b2, 1 - b2, -(lr / (1 - b1**t)), (1 - b2**t) ** 0.5, float(op["eps"]), gs])
         elif name == "RMSprop":
@@ -100,15 +114,15 @@ def lamb_chunk_table(numels: List[int], chunk: int = LAMB_CHUNK) -> torch.Tensor
     return torch.tensor(rows, dtype=torch.int64).reshape(-1, 4)
 
 
-HP_LEN = {"Adam": 8, "RMSprop": 8, "RMSpropTF": 8, "Lion": 7, "Lamb": 13}
+HP_LEN = {"SGD": 5, "AdamW": 8, "Adam": 8, "RMSprop": 8, "RMSpropTF": 8, "Lion": 7, "Lamb": 13}
 
-# the grad_scale column of every optimizer's hyper-parameter rows (SGD and AdamW: sg_trainer.TrainStep.set_hyper_params; the others:
-# hyper_param_rows), where clip_grad_norm folds its coefficient
+# the grad_scale column of every optimizer's hyper-parameter rows (SGD_GS, ADAMW_GS, ADAM_GS, ... of csrc/optim_math.cuh), where
+# clip_grad_norm folds its coefficient
 GRAD_SCALE_COLUMN = {"SGD": 3, "AdamW": 7, "Adam": 7, "RMSprop": 7, "RMSpropTF": 7, "Lion": 6, "Lamb": 9}
 
 
 class FlatOptimizer:
-    """The state and the per-step launches of one of NAMES over a FlatState: one kernel per weight-decay range for the elementwise
+    """The state and the per-step launches of one of ALL_NAMES over a FlatState: one kernel per weight-decay range for the elementwise
     optimizers; for Lamb three launches over both ranges at once (gradient sum of squares, m / v update with per-tensor sums,
     apply), reducing in a fixed order through a device-resident chunk table, with no host synchronisation."""
 
@@ -141,7 +155,11 @@ class FlatOptimizer:
             if b <= a:
                 continue
             p, g, st = flat.params[a:b], flat.grads[a:b], [t[a:b] for t in s]
-            if self.name == "Adam":
+            if self.name == "SGD":
+                K.sgd_step(p, g, st[0], hp[row])
+            elif self.name == "AdamW":
+                K.adamw_step(p, g, st[0], st[1], hp[row])
+            elif self.name == "Adam":
                 K.adam_step(p, g, st[0], st[1], hp[row])
             elif self.name == "Lion":
                 K.lion_step(p, g, st[0], hp[row])

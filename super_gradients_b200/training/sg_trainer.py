@@ -82,9 +82,6 @@ DEFAULT_TRAINING_PARAMS = {
 
 AVERAGE_MODEL_FILENAME = "average_model.pth"
 
-# defaults merged under user optimizer_params (reference: training/params.py:84-94)
-OPTIMIZER_DEFAULTS = {"SGD": {"weight_decay": 1e-4, "momentum": 0.9}, "AdamW": {"weight_decay": 1e-2}, **FO.REGISTRY_DEFAULTS}
-
 
 def _match_metric_name(wanted: str, available: list) -> str:
     """metric_to_watch resolution (reference: sg_trainer.py:588-601, fuzzy_idx_in_list): exact name, else the unique name that
@@ -265,23 +262,11 @@ class TrainStep:
         self.flat = FlatState(model, zero_wd_on_bias_and_bn)
         self.device = self.flat.params.device
         self.opt_name = optimizer
-        op = {**OPTIMIZER_DEFAULTS.get(optimizer, {}), **dict(optimizer_params)}
-        self.op = op
+        self.op, wd = FO.resolve(optimizer, optimizer_params, zero_wd_on_bias_and_bn)
         f = self.flat
-        self.fused = None  # Adam, RMSprop, RMSpropTF, Lion, Lamb (training/fused_optimizers.py)
-        if optimizer == "SGD":
-            self.state = [torch.zeros_like(f.params)]
-            self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, 5), dtype=torch.float32).pin_memory()
-        elif optimizer == "AdamW":
-            self.state = [torch.zeros_like(f.params), torch.zeros_like(f.params)]
-            self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, 8), dtype=torch.float32).pin_memory()
-        elif optimizer in FO.NAMES:
-            self.op, wd = FO.resolve(optimizer, optimizer_params, zero_wd_on_bias_and_bn)
-            self.fused = FO.FlatOptimizer(optimizer, self.op, wd, f)
-            self.state = self.fused.state
-            self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, self.fused.hp_len), dtype=torch.float32).pin_memory()
-        else:
-            raise NotImplementedError(f"optimizer {optimizer} has no fused kernel (SGD, Adam, AdamW, RMSprop, RMSpropTF, Lamb, Lion are implemented)")
+        self.fused = FO.FlatOptimizer(optimizer, self.op, wd, f)
+        self.state = self.fused.state
+        self.hp_host = torch.zeros((self.STAGING_SLOTS, 2, self.fused.hp_len), dtype=torch.float32).pin_memory()
         self.hp = torch.zeros_like(self.hp_host[0], device=self.device)
         self._slot, self._slot_events = 0, [None] * self.STAGING_SLOTS
         self.ema_on = ema
@@ -324,7 +309,6 @@ class TrainStep:
         # the reference's _backward_step (sg_trainer.py:611-644) calls loss.backward() on every micro-batch without dividing
         # by batch_accumulate: accumulated gradients are SUMMED; only the data-parallel average (DDP) divides
         gs = 1.0 / self.world
-        wd = float(self.op.get("weight_decay", 0.0))
         # The host may run many steps ahead of the device (graph replays are enqueued without a sync): every call stages its
         # values in its own pinned slot, and a slot is only rewritten after the copy that read it has executed.
         k = self._slot
@@ -332,19 +316,7 @@ class TrainStep:
         if self._slot_events[k] is not None:
             self._slot_events[k].synchronize()
         hp_host = self.hp_host[k]
-        if self.opt_name == "SGD":
-            mu, nes = float(self.op.get("momentum", 0.0)), float(bool(self.op.get("nesterov", False)))
-            hp_host[0] = torch.tensor([lr, mu, wd, gs, nes])
-            hp_host[1] = torch.tensor([lr, mu, 0.0, gs, nes])
-        elif self.fused is not None:
-            hp_host.copy_(torch.tensor(self.fused.rows(lr, t, gs), dtype=torch.float32))
-        else:
-            b1, b2 = self.op.get("betas", (0.9, 0.999))
-            eps = float(self.op.get("eps", 1e-8))
-            row = [lr, b1, b2, eps, wd, 1 - b1**t, 1 - b2**t, gs]
-            hp_host[0] = torch.tensor(row)
-            row[4] = 0.0
-            hp_host[1] = torch.tensor(row)
+        hp_host.copy_(torch.tensor(self.fused.rows(lr, t, gs), dtype=torch.float32))
         self.hp.copy_(hp_host, non_blocking=True)
         if self.ema_on and ema_decay_value is not None:
             self.ema_decay_host[k, 0] = ema_decay_value
@@ -415,19 +387,9 @@ class TrainStep:
     def _apply_update(self):
         """Optimizer + EMA over the (already reduced) flat gradients; no collective in here."""
         f = self.flat
-        nd = f.n_decay
         if self.clip_grad_norm is not None and f.chunks.shape[0]:
             K.clip_grad_norm(f.grads, f.chunks, self.hp, FO.GRAD_SCALE_COLUMN[self.opt_name], self.clip_grad_norm, self.clip_partials, self.clip_norm_coef)
-        ranges = [(0, nd, 0), (nd, f.n_live, 1)] if self.fused is None else []
-        if self.fused is not None:
-            self.fused.step(f, self.hp)
-        for a, b, row in ranges:
-            if b <= a:
-                continue
-            if self.opt_name == "SGD":
-                K.sgd_step(f.params[a:b], f.grads[a:b], self.state[0][a:b], self.hp[row])
-            else:
-                K.adamw_step(f.params[a:b], f.grads[a:b], self.state[0][a:b], self.state[1][a:b], self.hp[row])
+        self.fused.step(f, self.hp)
         if self.ema_on:
             K.ema_update(self.ema_params, f.params, self.ema_decay)
             if f.n_buf:

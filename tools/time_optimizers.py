@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Times one optimizer update over the live float32 parameters of YOLO-NAS-S and YOLO-NAS-L (the flat buffers of
-training/flat_state.py with zero_weight_decay_on_bias_and_bn, so two weight-decay ranges): SGD and AdamW for comparison, then Adam,
-RMSprop, RMSpropTF, Lion and Lamb.  CUDA events around the launches of one step, median of --iters steps.  Reports the bytes each
-update must move (every state and parameter read and written once, the gradient read once) over that time, against the H100 SXM
+training/flat_state.py with zero_weight_decay_on_bias_and_bn, so two weight-decay ranges) with each of SGD, AdamW, Adam, RMSprop,
+RMSpropTF, Lion and Lamb through FlatOptimizer.  CUDA events around the launches of one step, median of --iters steps.  Reports the
+bytes each update must move (every state and parameter read and written once, the gradient read once) over that time, against the H100 SXM
 data-sheet HBM3 bandwidth (3.35 TB/s).  Lamb's first launch (the global gradient sum of squares) is also timed on its own.
 
 Prints the card's name and power limit with the numbers.  Usage: python tools/time_optimizers.py [--iters 20]"""
@@ -58,30 +58,19 @@ def main():
         model = models.get(name, num_classes=80).cuda()
         flat = FlatState(model, True)
         flat.grads.normal_()
-        n, nd = flat.n_live, flat.n_decay
+        n = flat.n_live
         for opt, params in OPTIMIZERS:
+            op, wd = FO.resolve(opt, params, True)
+            fo = FO.FlatOptimizer(opt, op, wd, flat)
+            hp = torch.tensor(fo.rows(1e-4, 10, 1.0), dtype=torch.float32, device="cuda")
+
+            def step():
+                fo.step(flat, hp)
+
+            launches = 3 if opt == "Lamb" else 2
             extra = ""
-            if opt in ("SGD", "AdamW"):
-                state = [torch.zeros_like(flat.params) for _ in range(1 if opt == "SGD" else 2)]
-                hp = torch.tensor([[1e-4, 0.9, 1e-4, 1.0, 0.0]] * 2 if opt == "SGD" else [[1e-4, 0.9, 0.999, 1e-8, 1e-2, 0.1, 1e-3, 1.0]] * 2, device="cuda")
-                fn = K.sgd_step if opt == "SGD" else K.adamw_step
-
-                def step():
-                    for a, b, row in ((0, nd, 0), (nd, n, 1)):
-                        fn(flat.params[a:b], flat.grads[a:b], *[s[a:b] for s in state], hp[row])
-
-                launches = 2
-            else:
-                op, wd = FO.resolve(opt, params, True)
-                fo = FO.FlatOptimizer(opt, op, wd, flat)
-                hp = torch.tensor(fo.rows(1e-4, 10, 1.0), dtype=torch.float32, device="cuda")
-
-                def step():
-                    fo.step(flat, hp)
-
-                launches = 3 if opt == "Lamb" else 2
-                if opt == "Lamb":
-                    extra = f"{median_ms(lambda: K.lamb_grad_sqnorm(flat.grads, fo.chunks, hp, fo.partials), args.iters) * 1e3:.1f}"
+            if opt == "Lamb":
+                extra = f"{median_ms(lambda: K.lamb_grad_sqnorm(flat.grads, fo.chunks, hp, fo.partials), args.iters) * 1e3:.1f}"
             ms = median_ms(step, args.iters)
             moved = BYTES[opt] * n
             gbps = moved / ms / 1e6
