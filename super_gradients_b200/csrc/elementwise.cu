@@ -525,10 +525,13 @@ __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, int N, int H, int
     int q = t % Q; t /= Q;
     int p = t % P;
     int n = t / P;
+    // torch's selection (aten max_pool2d): the first maximum in row-major order, the last NaN if there is one, and the first in-bounds
+    // tap of a window that holds nothing above -inf.  Every recorded tap is therefore inside the image, which the backward kernels rely on.
+    const int r0 = max(0, pad - p * stride), s0 = max(0, pad - q * stride);
     float best[8];
     int bi[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = 0; }
+    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = r0 * k + s0; }
     for (int r = 0; r < k; ++r) {
       int h = p * stride - pad + r;
       if ((unsigned)h >= (unsigned)H) continue;
@@ -538,7 +541,7 @@ __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, int N, int H, int
         V8 a = ld8(x + (((int64_t)n * H + h) * W + w) * xp + xo + cv * 8);
 #pragma unroll
         for (int e = 0; e < 8; ++e)
-          if (a.v[e] > best[e]) { best[e] = a.v[e]; bi[e] = r * k + s; }
+          if (a.v[e] > best[e] || a.v[e] != a.v[e]) { best[e] = a.v[e]; bi[e] = r * k + s; }
       }
     }
     V8 o;
@@ -558,8 +561,10 @@ __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, int N, int H, int
 // Stride-1 max-pool (the SPP pools, k = 5 / 9 / 13 over 20 x 20 maps) as two separable passes through shared memory: one CTA owns
 // the H x W plane of one image and one 8-channel vector.  Pass 1: per (row, output column) the maximum over the window's columns and
 // the FIRST column offset that attains it; pass 2: per output pixel the first window row whose row-maximum is the window maximum.
-// That is the same element as the direct scan's (row-major order, strict >: the first maximum), which the backward routes to, at
-// 2k instead of k^2 comparisons per output and with the plane read from HBM once (the direct kernel ran at 73 GB/s).
+// Both passes take a NaN over anything and a later NaN over an earlier one, and start from the first in-bounds column / row.  The
+// composition is the same element as the direct scan's (row-major order: the first maximum, else the last NaN, else the first
+// in-bounds tap), which the backward routes to, at 2k instead of k^2 comparisons per output and with the plane read from HBM once
+// (the direct kernel ran at 73 GB/s).
 __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __restrict__ x, int H, int W, int C, int xp, int xo, int k, int pad, bf16* y,
                                                               int P, int Q, int yp, int yo, uint8_t* idx) {
   extern __shared__ __align__(16) unsigned char smem_mp[];
@@ -572,10 +577,11 @@ __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __rest
   __syncthreads();
   for (int i = threadIdx.x; i < H * Q; i += blockDim.x) {
     const int h = i / Q, q = i - h * Q;
+    const int s0 = max(0, pad - q);
     float best[8];
     int bi[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = 0; }
+    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = s0; }
     for (int s2 = 0; s2 < k; ++s2) {
       const int w = q - pad + s2;
       if ((unsigned)w >= (unsigned)W) continue;
@@ -584,8 +590,8 @@ __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __rest
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const float lo = __uint_as_float(ww[e] << 16), hi = __uint_as_float(ww[e] & 0xffff0000u);
-        if (lo > best[2 * e]) { best[2 * e] = lo; bi[2 * e] = s2; }
-        if (hi > best[2 * e + 1]) { best[2 * e + 1] = hi; bi[2 * e + 1] = s2; }
+        if (lo > best[2 * e] || lo != lo) { best[2 * e] = lo; bi[2 * e] = s2; }
+        if (hi > best[2 * e + 1] || hi != hi) { best[2 * e + 1] = hi; bi[2 * e + 1] = s2; }
       }
     }
 #pragma unroll
@@ -597,17 +603,19 @@ __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __rest
   __syncthreads();
   for (int i = threadIdx.x; i < P * Q; i += blockDim.x) {
     const int p = i / Q, q = i - p * Q;
+    const int r0 = max(0, pad - p);
+    const size_t o0 = ((size_t)(p - pad + r0) * Q + q) * 8;
     float best[8];
     int bi[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = 0; }
+    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = r0 * k + rarg[o0 + e]; }
     for (int r = 0; r < k; ++r) {
       const int h = p - pad + r;
       if ((unsigned)h >= (unsigned)H) continue;
       const size_t o = ((size_t)h * Q + q) * 8;
 #pragma unroll
       for (int e = 0; e < 8; ++e)
-        if (rmax[o + e] > best[e]) { best[e] = rmax[o + e]; bi[e] = r * k + rarg[o + e]; }
+        if (rmax[o + e] > best[e] || rmax[o + e] != rmax[o + e]) { best[e] = rmax[o + e]; bi[e] = r * k + rarg[o + e]; }
     }
     V8 ov;
 #pragma unroll
@@ -623,6 +631,7 @@ __global__ void __launch_bounds__(256) maxpool_s1_smem_kernel(const bf16* __rest
   }
 }
 
+// Both backward kernels take the recorded tap as it is: the forward kernels only record taps inside the image (see above).
 __global__ void maxpool_bwd_kernel(const bf16* __restrict__ dy, int N, int H, int W, int C, int k, int stride, int pad,
                                    int P, int Q, int dyp, int dyo, const uint8_t* idx, float* dx) {
   const int64_t total = (int64_t)N * P * Q * C;
