@@ -1002,25 +1002,14 @@ int launch_stem_k(const Op& op, const SgbQarepDesc& d, const void* xp, const voi
     attr = true;
   }
   alignas(64) CUtensorMap map_x, map_w, map_g;
-  auto encode = [&](CUtensorMap* map, const void* p, uint64_t cols, uint64_t rows, uint64_t pitch, uint32_t bc, uint32_t br, CUtensorMapSwizzle sw) {
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {pitch * 2};
-    cuuint32_t box[2] = {bc, br};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = sm100::g_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeTiled(stem) failed with %d (cols=%llu rows=%llu pitch=%llu)", (int)r, (unsigned long long)cols, (unsigned long long)rows,
-                    (unsigned long long)pitch);
-      return SGB_E_CUDA;
-    }
-    return SGB_OK;
-  };
-  if (int rc = encode(&map_x, xp, STEM_KP, d.M, STEM_KP, STEM_KP, STEM_BM, CU_TENSOR_MAP_SWIZZLE_64B)) return rc;
-  if (int rc = encode(&map_w, w, STEM_KP, 2 * KOUT, STEM_KP, STEM_KP, 2 * KOUT, CU_TENSOR_MAP_SWIZZLE_64B)) return rc;
+  const cuuint64_t x_dims[2] = {STEM_KP, (cuuint64_t)d.M}, w_dims[2] = {STEM_KP, 2 * KOUT}, g_dims[2] = {KOUT, (cuuint64_t)d.M};
+  const cuuint64_t row_bytes[1] = {STEM_KP * 2}, g_row_bytes[1] = {(cuuint64_t)gpitch * 2};
+  const cuuint32_t x_box[2] = {STEM_KP, STEM_BM}, w_box[2] = {STEM_KP, 2 * KOUT}, g_box[2] = {KOUT, STEM_BM};
+  if (int rc = sm100::encode_tiled(&map_x, xp, 2, x_dims, row_bytes, x_box, CU_TENSOR_MAP_SWIZZLE_64B, "stem patches")) return rc;
+  if (int rc = sm100::encode_tiled(&map_w, w, 2, w_dims, row_bytes, w_box, CU_TENSOR_MAP_SWIZZLE_64B, "stem filter")) return rc;
   map_g = map_x;
   if (Lay::DOUT)
-    if (int rc = encode(&map_g, dout, KOUT, d.M, gpitch, KOUT, STEM_BM, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+    if (int rc = sm100::encode_tiled(&map_g, dout, 2, g_dims, g_row_bytes, g_box, CU_TENSOR_MAP_SWIZZLE_NONE, "stem dout")) return rc;
   const int64_t per = nranges > 0 ? (d.M + nranges - 1) / nranges : STEM_BM;
   const int64_t ranges = (d.M + per - 1) / per;
   const int grid = (int)(ranges < sgb_sm_count() ? ranges : sgb_sm_count());

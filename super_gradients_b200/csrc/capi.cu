@@ -4,7 +4,6 @@
 
 #include "common.cuh"
 #include "conv_sm100.h"
-#include "sm100_host.h"
 
 static thread_local char g_err[512] = "";
 

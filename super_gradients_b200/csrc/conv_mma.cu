@@ -1,16 +1,17 @@
 // Generic implicit-GEMM convolution kernels (fprop / dgrad / wgrad) for NHWC bf16 tensors, fp32 accumulation.
 //
-// This is the shape-agnostic path of libsgb200: any filter size, stride, padding, channel pitch/offset, plus the
-// ConvTranspose2d(2,2) scatter store.  It runs on the legacy warp-level tensor-core path (mma.sync m16n8k16) fed
-// by a 4-stage cp.async gather pipeline, and serves the shapes the tcgen05/TMA kernels (conv_sm100.cu) do not
-// take (3-channel stems, 7x7, strided dgrad, ragged channel counts).  One kernel covers fprop and dgrad: dgrad of
-// a stride-s convolution is decomposed into s*s output-parity classes, each an exact (zero-waste) stride-1 gather.
+// This is the shape-agnostic engine of libsgb200: any filter size, stride, padding, channel pitch/offset, plus the
+// ConvTranspose2d(2,2) scatter store.  It runs on the warp-level tensor-core path (mma.sync m16n8k16) fed by a 4-stage
+// cp.async gather pipeline, and serves the calls the wgmma / TMA kernels of conv_sm100.cu decline (conv.cu routes them):
+// 3-channel stems that are not padded to 16 channels, 7x7, ragged channel counts, fp32 outputs, and the strided dgrads other
+// than 3x3 and 1x1 stride 2.  One kernel covers fprop and dgrad: dgrad of a stride-s convolution is decomposed into s*s
+// output-parity classes, each an exact (zero-waste) stride-1 gather.
 //
 // Reference arithmetic being replaced: nn.Conv2d forward/backward as called from
 //   src/super_gradients/modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,
 //   training/models/classification_models/resnet.py:26-84 (see include/sgb200.h).
 #include "common.cuh"
-#include "conv_sm100.h"
+#include "conv_mma.h"
 
 namespace {
 
@@ -455,92 +456,42 @@ int dispatch_igemm(const IGemmParams& p, int ncls, int maxM, cudaStream_t st) {
   return launch_igemm<32, 4, 2>(p, ncls, maxM, st);
 }
 
-int check_desc(const SgbConvDesc* d) {
-  SGB_REQUIRE(d != nullptr, "desc is null");
-  SGB_REQUIRE(d->N > 0 && d->H > 0 && d->W > 0 && d->C > 0 && d->K > 0 && d->R > 0 && d->S > 0, "positive dims");
-  SGB_REQUIRE(d->stride >= 1 && d->pad >= 0, "stride/pad");
-  SGB_REQUIRE(d->P == (d->H + 2 * d->pad - d->R) / d->stride + 1, "P inconsistent");
-  SGB_REQUIRE(d->Q == (d->W + 2 * d->pad - d->S) / d->stride + 1, "Q inconsistent");
-  SGB_REQUIRE(d->C % 8 == 0, "C must be a multiple of 8 (pad the channels)");
-  SGB_REQUIRE(d->x_pitch % 8 == 0 && d->x_off % 8 == 0, "x pitch/offset must be multiples of 8");
-  SGB_REQUIRE(d->x_pitch >= d->x_off + d->C, "x slice exceeds pitch");
-  SGB_REQUIRE(d->y_pitch >= d->y_off + d->K, "y slice exceeds pitch");
-  SGB_REQUIRE(d->centre_from == 0 || (d->R == 3 && d->S == 3 && d->stride == 1 && d->pad == 1 && d->centre_from > 0 &&
-                                      d->centre_from < d->K && d->centre_from % 16 == 0),
-              "centre_from needs a 3x3 / stride-1 / pad-1 convolution and 0 < centre_from < K, a multiple of 16");
-  return SGB_OK;
+// A gather of `A` (inH x inW pixels per image, Cg channels per tap at offset in_off of in_pitch) against filter rows of b_pitch
+// elements into Ngemm channels of the outH x outW image Y (at out_pitch, out_off): unit strides, taps ascending, no epilogue.
+IGemmParams igemm_params(const sgb_bf16* A, int inH, int inW, int in_pitch, int in_off, int Cg, const sgb_bf16* B, int b_pitch,
+                         int Ngemm, void* Y, int outH, int outW, int out_pitch, int out_off) {
+  IGemmParams p{};
+  p.A = reinterpret_cast<const bf16*>(A);
+  p.B = reinterpret_cast<const bf16*>(B);
+  p.Y = Y;
+  p.Ngemm = Ngemm;
+  p.Cg = Cg;
+  p.row_mul = 1;
+  p.tap_sgn = 1;
+  p.inH = inH;
+  p.inW = inW;
+  p.in_pitch = in_pitch;
+  p.in_off = in_off;
+  p.b_pitch = b_pitch;
+  p.rstep = 1;
+  p.S_filt = 1;
+  p.outH = outH;
+  p.outW = outW;
+  p.o_mul = 1;
+  p.out_pitch = out_pitch;
+  p.out_off = out_off;
+  p.stats_repl = 1;
+  return p;
 }
-
 }  // namespace
 
-extern "C" int sgb_conv_fprop(const SgbConvDesc* d, const sgb_bf16* x, const sgb_bf16* w, void* y,
-                              const SgbEpilogue* ep, void* stream) {
-  if (int rc = check_desc(d)) return rc;
-  SGB_REQUIRE(x && w && y, "null pointer");
-  if (!(ep && ep->out_f32)) {
-    sm100::Problem q{};
-    q.a = x + d->x_off; q.N = d->N; q.H = d->H; q.W = d->W; q.C = d->C; q.a_pitch = d->x_pitch;
-    q.b = w; q.b_rows = d->K; q.b_cols = d->R * d->S * d->C; q.b_cols_per_tap = d->C;
-    q.R = d->R; q.S = d->S; q.stride = d->stride; q.pad = d->pad; q.P = d->P; q.Q = d->Q; q.flip = 0;
-    q.y = y; q.y_pitch = d->y_pitch; q.y_off = d->y_off;
-    q.centre_from = d->centre_from;
-    if (ep) {
-      q.scale = ep->scale; q.shift = ep->shift; q.residual = ep->residual; q.stats = ep->stats;
-      q.stats_repl = ep->stats_repl > 0 ? ep->stats_repl : 1; q.act = ep->act;
-    } else {
-      q.stats_repl = 1;
-    }
-    if (d->pad == d->R / 2 && sm100::supported(q)) return sm100::launch(q, (cudaStream_t)stream);
-    // 2 x 2 / stride 2 / no padding over a dense tensor (the backward of ConvTranspose2d(2, 2), modules/sampling.py:72-73): the
-    // patches do not overlap, so the tensor viewed as an image [N * H/2][2][W/2][2C] -- row pair, row parity, column pair, (column
-    // parity, channel) -- turns the layer into a 2-tap (rows 0 and 1), stride-1 valid convolution with 2C channels per tap whose
-    // B columns are the filter's own (dh, dw, c) order: the im2col tcgen05 kernel serves it through its explicit tap table.
-    if (d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
-        d->W % 2 == 0 && d->P == d->H / 2 && d->Q == d->W / 2 && (2 * d->C) % 16 == 0 && d->K % 8 == 0 && d->y_pitch % 8 == 0 && d->y_off % 8 == 0 &&
-        (long long)d->N * (d->H / 2) < (1ll << 31)) {
-      q.N = d->N * (d->H / 2); q.H = 2; q.W = d->W / 2; q.C = 2 * d->C; q.a_pitch = 2 * d->C;
-      q.b_cols_per_tap = 2 * d->C;
-      q.centre_from = 0;  // a 2 x 2 filter: check_desc refused a non-zero field
-      q.R = 1; q.S = 1; q.stride = 1; q.pad = 0; q.P = 1; q.Q = d->W / 2;
-      q.ntaps = 2;
-      q.tap_dh[0] = 0; q.tap_dw[0] = 0; q.tap_b[0] = 0;
-      q.tap_dh[1] = 1; q.tap_dw[1] = 0; q.tap_b[1] = 1;
-      if (sm100::supported(q)) return sm100::launch(q, (cudaStream_t)stream);
-      return SGB_E_UNSUPPORTED;
-    }
-  }
-  IGemmParams p{};
-  p.A = reinterpret_cast<const bf16*>(x);
-  p.B = reinterpret_cast<const bf16*>(w);
-  p.Y = y;
-  GatherClass& g = p.cls[0];
-  g.M = d->N * d->P * d->Q;
-  g.Hc = d->P;
-  g.Wc = d->Q;
-  g.nr = d->R;
-  g.ns = d->S;
-  g.Kg = d->R * d->S * d->C;
-  g.hb_add = -d->pad;
-  g.wb_add = -d->pad;
-  g.r0 = g.s0 = 0;
-  g.oh_add = g.ow_add = 0;
-  p.Ngemm = d->K;
-  p.Cg = d->C;
-  p.row_mul = d->stride;
-  p.tap_sgn = 1;
-  p.inH = d->H;
-  p.inW = d->W;
-  p.in_pitch = d->x_pitch;
-  p.in_off = d->x_off;
-  p.b_pitch = d->R * d->S * d->C;
-  p.rstep = 1;
-  p.S_filt = d->S;
-  p.outH = d->P;
-  p.outW = d->Q;
-  p.o_mul = 1;
-  p.out_pitch = d->y_pitch;
-  p.out_off = d->y_off;
-  p.up2_cout = 0;
+namespace igemm {
+
+int conv_fprop(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* w, void* y, const SgbEpilogue* ep, cudaStream_t st) {
+  IGemmParams p = igemm_params(x, d.H, d.W, d.x_pitch, d.x_off, d.C, w, d.R * d.S * d.C, d.K, y, d.P, d.Q, d.y_pitch, d.y_off);
+  p.cls[0] = {d.N * d.P * d.Q, d.P, d.Q, d.R, d.S, d.R * d.S * d.C, -d.pad, -d.pad};
+  p.row_mul = d.stride;
+  p.S_filt = d.S;
   if (ep) {
     p.scale = ep->scale;
     p.shift = ep->shift;
@@ -550,225 +501,65 @@ extern "C" int sgb_conv_fprop(const SgbConvDesc* d, const sgb_bf16* x, const sgb
     SGB_REQUIRE((p.stats_repl & (p.stats_repl - 1)) == 0, "stats_repl must be a power of two");
     p.act = ep->act;
     p.out_f32 = ep->out_f32;
-  } else {
-    p.stats_repl = 1;
   }
-  return dispatch_igemm(p, 1, g.M, (cudaStream_t)stream);
+  return dispatch_igemm(p, 1, p.cls[0].M, st);
 }
 
-extern "C" int sgb_convt2x2_fprop(const SgbConvDesc* d, const sgb_bf16* x_small, const sgb_bf16* w_up,
-                                  const float* bias, sgb_bf16* y_up, void* stream) {
-  // d: equivalent conv (N,H,W,C)=upsampled -> (N,P,Q,K)=small with R=S=2, stride 2, pad 0
-  if (int rc = check_desc(d)) return rc;
-  SGB_REQUIRE(d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0, "convt2x2 needs R=S=2, stride 2, pad 0");
-  SGB_REQUIRE(d->K % 8 == 0 && d->y_pitch % 8 == 0 && d->y_off % 8 == 0, "small-side channels must be multiples of 8");
-  if (d->K % 16 == 0 && d->C % 16 == 0) {
-    // tcgen05 path: the transposed convolution is four 1x1 GEMMs, one per output parity (dh, dw), each writing the output pixels
-    // (2h + dh, 2w + dw) through the strided-row epilogue the stride-2 input gradients use.  w_up rows are ordered (dh, dw, co).
-    bool all_ok = true;
-    for (int cls = 0; cls < 4 && all_ok; ++cls) {
-      sm100::Problem q{};
-      q.a = x_small + d->y_off; q.N = d->N; q.H = d->P; q.W = d->Q; q.C = d->K; q.a_pitch = d->y_pitch;
-      q.b = w_up + (size_t)cls * d->C * d->K; q.b_rows = d->C; q.b_cols = d->K; q.b_cols_per_tap = d->K;
-      q.R = 1; q.S = 1; q.stride = 1; q.pad = 0; q.P = d->P; q.Q = d->Q; q.flip = 0;
-      q.y = y_up; q.y_pitch = d->x_pitch; q.y_off = d->x_off;
-      q.shift = bias;
-      q.stats_repl = 1;
-      q.out_mode = 1; q.o_mul = 2; q.oh_add = cls >> 1; q.ow_add = cls & 1; q.outH = d->H; q.outW = d->W;
-      q.ntaps = 1; q.tap_dh[0] = 0; q.tap_dw[0] = 0; q.tap_b[0] = 0;
-      if (!sm100::supported(q)) { all_ok = false; break; }  // identical for the four classes: fails before any launch
-      if (int rc = sm100::launch(q, (cudaStream_t)stream)) return rc;
-    }
-    if (all_ok) return SGB_OK;
-  }
-  IGemmParams p{};
-  p.A = reinterpret_cast<const bf16*>(x_small);
-  p.B = reinterpret_cast<const bf16*>(w_up);
-  p.Y = y_up;
-  GatherClass& g = p.cls[0];
-  g.M = d->N * d->P * d->Q;
-  g.Hc = d->P;
-  g.Wc = d->Q;
-  g.nr = g.ns = 1;
-  g.Kg = d->K;
-  p.Ngemm = 4 * d->C;
-  p.Cg = d->K;
-  p.row_mul = 1;
-  p.tap_sgn = 1;
-  p.inH = d->P;
-  p.inW = d->Q;
-  p.in_pitch = d->y_pitch;
-  p.in_off = d->y_off;
-  p.b_pitch = d->K;
-  p.rstep = 1;
-  p.S_filt = 1;
-  p.outH = d->H;
-  p.outW = d->W;
+// The transposed convolution as one 1x1 GEMM of 4C columns ordered (dh, dw, co), scattered to the 2 x 2 output pixels.
+int convt2x2_fprop(const SgbConvDesc& d, const sgb_bf16* x_small, const sgb_bf16* w_up, const float* bias, sgb_bf16* y_up,
+                   cudaStream_t st) {
+  IGemmParams p = igemm_params(x_small, d.P, d.Q, d.y_pitch, d.y_off, d.K, w_up, d.K, 4 * d.C, y_up, d.H, d.W, d.x_pitch, d.x_off);
+  p.cls[0] = {d.N * d.P * d.Q, d.P, d.Q, 1, 1, d.K};
   p.o_mul = 2;
-  p.out_pitch = d->x_pitch;
-  p.out_off = d->x_off;
-  p.up2_cout = d->C;
+  p.up2_cout = d.C;
   p.shift = bias;
-  p.stats_repl = 1;
-  return dispatch_igemm(p, 1, g.M, (cudaStream_t)stream);
+  return dispatch_igemm(p, 1, p.cls[0].M, st);
 }
 
-extern "C" int sgb_conv_dgrad(const SgbConvDesc* d, const sgb_bf16* dy, const sgb_bf16* w_crsk, sgb_bf16* dx,
-                              int accumulate, void* stream) {
-  if (int rc = check_desc(d)) return rc;
-  SGB_REQUIRE(dy && w_crsk && dx, "null pointer");
-  SGB_REQUIRE(d->K % 8 == 0 || d->y_pitch - d->y_off >= ((d->K + 7) / 8) * 8, "dy channels must be padded to 8");
-  SGB_REQUIRE(d->y_pitch % 8 == 0 && d->y_off % 8 == 0, "dy pitch/offset must be multiples of 8");
-  const int s = d->stride;
-  SGB_REQUIRE(s == 1 || s == 2, "dgrad supports stride 1 or 2");
-  const int Kp = ((d->K + 7) / 8) * 8;  // channels gathered per tap (w_crsk rows are padded with zeros to Kp)
-  if (s == 1 && d->pad == d->R / 2 && d->K % 16 == 0) {
-    // dgrad of a stride-1 "same" convolution == convolution of dy with the spatially flipped CRSK filter
-    sm100::Problem q{};
-    q.a = dy + d->y_off; q.N = d->N; q.H = d->P; q.W = d->Q; q.C = d->K; q.a_pitch = d->y_pitch;
-    q.b = w_crsk; q.b_rows = d->C; q.b_cols = d->R * d->S * Kp; q.b_cols_per_tap = Kp;
-    q.R = d->R; q.S = d->S; q.stride = 1; q.pad = d->R - 1 - d->pad; q.P = d->H; q.Q = d->W; q.flip = 1;
-    q.y = dx; q.y_pitch = d->x_pitch; q.y_off = d->x_off;
-    q.residual = accumulate ? dx : nullptr;
-    q.stats_repl = 1;
-    q.centre_from = d->centre_from;
-    if (sm100::supported(q)) return sm100::launch(q, (cudaStream_t)stream);
-  }
-  if (s == 2 && d->K % 16 == 0 && d->R == 3 && d->S == 3 && d->pad == 1 && d->C % 8 == 0 && d->H % 2 == 0 &&
-      d->W % 2 == 0 && d->H == 2 * d->P && d->W == 2 * d->Q) {
-    // stride-2 dgrad = 4 output-parity classes, each an exact stride-1 gather of dy with a subset of the taps
-    bool all_ok = true;
-    for (int cls = 0; cls < 4 && all_ok; ++cls) {
-      const int ph = cls >> 1, pw = cls & 1;
-      sm100::Problem q{};
-      q.a = dy + d->y_off; q.N = d->N; q.H = d->P; q.W = d->Q; q.C = d->K; q.a_pitch = d->y_pitch;
-      q.b = w_crsk; q.b_rows = d->C; q.b_cols = d->R * d->S * Kp; q.b_cols_per_tap = Kp;
-      q.R = d->R; q.S = d->S; q.stride = 1; q.pad = 0; q.P = d->P; q.Q = d->Q; q.flip = 0;
-      q.y = dx; q.y_pitch = d->x_pitch; q.y_off = d->x_off;
-      q.residual = accumulate ? dx : nullptr;
-      q.stats_repl = 1;
-      q.out_mode = 1; q.o_mul = 2; q.oh_add = ph; q.ow_add = pw; q.outH = d->H; q.outW = d->W;
-      // taps r with (h + pad - r) even, h = 2j + ph:  ho = j + (ph + pad - r) / 2
-      int nt = 0;
-      for (int r = 0; r < d->R; ++r) {
-        if (((ph + d->pad - r) & 1) != 0) continue;
-        for (int sx = 0; sx < d->S; ++sx) {
-          if (((pw + d->pad - sx) & 1) != 0) continue;
-          q.tap_dh[nt] = (ph + d->pad - r) / 2;
-          q.tap_dw[nt] = (pw + d->pad - sx) / 2;
-          q.tap_b[nt] = r * d->S + sx;
-          ++nt;
-        }
-      }
-      q.ntaps = nt;
-      if (!sm100::supported(q)) { all_ok = false; break; }  // identical for the 4 classes: fails before any launch
-      if (int rc = sm100::launch(q, (cudaStream_t)stream)) return rc;
-    }
-    if (all_ok) return SGB_OK;
-  }
-  if (s == 2 && d->K % 16 == 0 && d->R == 1 && d->S == 1 && d->pad == 0 && d->C % 8 == 0 && d->H == 2 * d->P &&
-      d->W == 2 * d->Q) {
-    // 1x1 stride-2 dgrad: only the even/even input pixels receive a gradient.  With accumulate the other three parity
-    // classes are untouched; otherwise they are zero-filled first.
-    sm100::Problem q{};
-    q.a = dy + d->y_off; q.N = d->N; q.H = d->P; q.W = d->Q; q.C = d->K; q.a_pitch = d->y_pitch;
-    q.b = w_crsk; q.b_rows = d->C; q.b_cols = Kp; q.b_cols_per_tap = Kp;
-    q.R = 1; q.S = 1; q.stride = 1; q.pad = 0; q.P = d->P; q.Q = d->Q; q.flip = 0;
-    q.y = dx; q.y_pitch = d->x_pitch; q.y_off = d->x_off;
-    q.residual = accumulate ? dx : nullptr;
-    q.stats_repl = 1;
-    q.out_mode = 1; q.o_mul = 2; q.oh_add = 0; q.ow_add = 0; q.outH = d->H; q.outW = d->W;
-    q.ntaps = 1; q.tap_dh[0] = 0; q.tap_dw[0] = 0; q.tap_b[0] = 0;
-    if (sm100::supported(q)) {
-      if (!accumulate) {
-        if (d->x_pitch == d->C && d->x_off == 0) {
-          cudaMemsetAsync(dx, 0, (size_t)d->N * d->H * d->W * d->C * sizeof(sgb_bf16), (cudaStream_t)stream);
-          return sm100::launch(q, (cudaStream_t)stream);
-        }
-      } else {
-        return sm100::launch(q, (cudaStream_t)stream);
-      }
-    }
-  }
-  IGemmParams p{};
-  p.A = reinterpret_cast<const bf16*>(dy);
-  p.B = reinterpret_cast<const bf16*>(w_crsk);
-  p.Y = dx;
-  p.Ngemm = d->C;
-  p.Cg = Kp;
-  p.row_mul = 1;
+int conv_dgrad(const SgbConvDesc& d, const sgb_bf16* dy, const sgb_bf16* w_crsk, sgb_bf16* dx, int accumulate, cudaStream_t st) {
+  const int s = d.stride;
+  const int Kp = ((d.K + 7) / 8) * 8;  // channels gathered per tap (w_crsk rows are padded with zeros to Kp)
+  IGemmParams p = igemm_params(dy, d.P, d.Q, d.y_pitch, d.y_off, Kp, w_crsk, d.R * d.S * Kp, d.C, dx, d.H, d.W, d.x_pitch, d.x_off);
   p.tap_sgn = -1;
-  p.inH = d->P;
-  p.inW = d->Q;
-  p.in_pitch = d->y_pitch;
-  p.in_off = d->y_off;
-  p.b_pitch = d->R * d->S * Kp;
   p.rstep = s;
-  p.S_filt = d->S;
-  p.outH = d->H;
-  p.outW = d->W;
+  p.S_filt = d.S;
   p.o_mul = s;
-  p.out_pitch = d->x_pitch;
-  p.out_off = d->x_off;
-  p.stats_repl = 1;
   if (accumulate) p.residual = reinterpret_cast<const bf16*>(dx);
   int ncls = 0, maxM = 0;
   for (int ph = 0; ph < s; ++ph)
     for (int pw = 0; pw < s; ++pw) {
       GatherClass& g = p.cls[ncls++];
-      g.Hc = (d->H - ph + s - 1) / s;
-      g.Wc = (d->W - pw + s - 1) / s;
-      g.M = d->N * g.Hc * g.Wc;
-      g.r0 = (ph + d->pad) % s;
-      g.s0 = (pw + d->pad) % s;
-      g.nr = g.r0 < d->R ? (d->R - g.r0 + s - 1) / s : 0;
-      g.ns = g.s0 < d->S ? (d->S - g.s0 + s - 1) / s : 0;
+      g.Hc = (d.H - ph + s - 1) / s;
+      g.Wc = (d.W - pw + s - 1) / s;
+      g.M = d.N * g.Hc * g.Wc;
+      g.r0 = (ph + d.pad) % s;
+      g.s0 = (pw + d.pad) % s;
+      g.nr = g.r0 < d.R ? (d.R - g.r0 + s - 1) / s : 0;
+      g.ns = g.s0 < d.S ? (d.S - g.s0 + s - 1) / s : 0;
       g.Kg = g.nr * g.ns * Kp;
       if (g.ns == 0) g.ns = 1;  // avoid div by zero; Kg == 0 so nothing is gathered
-      g.hb_add = (ph + d->pad - g.r0) / s;
-      g.wb_add = (pw + d->pad - g.s0) / s;
+      g.hb_add = (ph + d.pad - g.r0) / s;
+      g.wb_add = (pw + d.pad - g.s0) / s;
       g.oh_add = ph;
       g.ow_add = pw;
       if (g.M > maxM) maxM = g.M;
     }
-  return dispatch_igemm(p, ncls, maxM, (cudaStream_t)stream);
+  return dispatch_igemm(p, ncls, maxM, st);
 }
 
-extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb_bf16* dy, float* dw, void* stream) {
-  if (int rc = check_desc(d)) return rc;
-  SGB_REQUIRE(x && dy && dw, "null pointer");
-  SGB_REQUIRE(d->y_pitch % 8 == 0 && d->y_off % 8 == 0, "dy pitch/offset must be multiples of 8");
-  SGB_REQUIRE(d->K % 8 == 0 || d->y_pitch - d->y_off >= ((d->K + 7) / 8) * 8, "dy channels must be padded to 8");
-  {
-    sm100::WgradProblem q{};
-    q.x = x + d->x_off; q.dy = dy + d->y_off;
-    q.N = d->N; q.H = d->H; q.W = d->W; q.C = d->C; q.x_pitch = d->x_pitch;
-    q.K = d->K; q.y_pitch = d->y_pitch;
-    q.R = d->R; q.S = d->S; q.stride = d->stride; q.pad = d->pad; q.P = d->P; q.Q = d->Q;
-    q.dw = dw;
-    q.centre_from = d->centre_from;
-    if (sm100::wgrad_supported(q)) return sm100::wgrad_launch(q, (cudaStream_t)stream);
-    // 2 x 2 / stride 2 / no padding over a dense x: the same re-description as in sgb_conv_fprop -- a (2 x 1)-tap stride-1 valid
-    // convolution over the image [N * H/2][2][W/2][2C]; dW rows [K][dh][(dw, c)] are the KRSC rows of the 2 x 2 filter.
-    if (d->R == 2 && d->S == 2 && d->stride == 2 && d->pad == 0 && d->x_pitch == d->C && d->x_off == 0 && d->H % 2 == 0 &&
-        d->W % 2 == 0 && d->P == d->H / 2 && d->Q == d->W / 2 && (2 * d->C) % 16 == 0 && d->K % 8 == 0 && (long long)d->N * (d->H / 2) < (1ll << 31)) {
-      q.N = d->N * (d->H / 2); q.H = 2; q.W = d->W / 2; q.C = 2 * d->C; q.x_pitch = 2 * d->C;
-      q.R = 2; q.S = 1; q.stride = 1; q.pad = 0; q.P = 1; q.Q = d->W / 2;
-      return sm100::wgrad_launch(q, (cudaStream_t)stream);
-    }
-  }
+int conv_wgrad(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* dy, float* dw, cudaStream_t st) {
   WgradParams p{};
   p.X = reinterpret_cast<const bf16*>(x);
   p.DY = reinterpret_cast<const bf16*>(dy);
   p.DW = dw;
-  p.N = d->N; p.H = d->H; p.W = d->W; p.C = d->C; p.K = d->K; p.R = d->R; p.S = d->S; p.P = d->P; p.Q = d->Q;
-  p.stride = d->stride; p.pad = d->pad;
-  p.x_pitch = d->x_pitch; p.x_off = d->x_off; p.y_pitch = d->y_pitch; p.y_off = d->y_off;
-  p.npix = d->N * d->P * d->Q;
-  p.ncols = d->R * d->S * d->C;
-  int bmw = d->K <= 32 ? 32 : (d->K <= 64 ? 64 : 128);
-  if (d->K > 64 && d->K <= 96) bmw = 32;  // 3 x 32 wastes nothing
-  int mt = ceil_div(d->K, bmw), nt = ceil_div(p.ncols, 64);
+  p.N = d.N; p.H = d.H; p.W = d.W; p.C = d.C; p.K = d.K; p.R = d.R; p.S = d.S; p.P = d.P; p.Q = d.Q;
+  p.stride = d.stride; p.pad = d.pad;
+  p.x_pitch = d.x_pitch; p.x_off = d.x_off; p.y_pitch = d.y_pitch; p.y_off = d.y_off;
+  p.npix = d.N * d.P * d.Q;
+  p.ncols = d.R * d.S * d.C;
+  int bmw = d.K <= 32 ? 32 : (d.K <= 64 ? 64 : 128);
+  if (d.K > 64 && d.K <= 96) bmw = 32;  // 3 x 32 wastes nothing
+  int mt = ceil_div(d.K, bmw), nt = ceil_div(p.ncols, 64);
   int total_slices = ceil_div(p.npix, BK);
   int target = 132 * 4;
   int splits = target / (mt * nt);
@@ -779,7 +570,6 @@ extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb
   p.slices_per_z = ceil_div(total_slices, splits);
   splits = ceil_div(total_slices, p.slices_per_z);
   dim3 grid(nt, mt, splits);
-  cudaStream_t st = (cudaStream_t)stream;
   size_t smem = (size_t)STAGES * (BK * bmw + BK * 64) * sizeof(bf16);
   if (bmw == 128) {
     wgrad_kernel<128, 4, 2><<<grid, THREADS, smem, st>>>(p);
@@ -791,3 +581,5 @@ extern "C" int sgb_conv_wgrad(const SgbConvDesc* d, const sgb_bf16* x, const sgb
   SGB_LAUNCH_CHECK("wgrad_kernel");
   return SGB_OK;
 }
+
+}  // namespace igemm

@@ -9,14 +9,16 @@
 //
 // Serves every 1x1 and 3x3 convolution with C % 16 == 0 (fprop; stride-1 dgrad over the flipped CRSK filter; stride-2 dgrad as
 // s^2 output-parity classes through the explicit tap table) and their weight gradients (wgrad_wgmma_kernel, MN-major
-// operands; wgrad3x3_halo_kernel for the 3x3 stride-1 ones).  3-channel stems that are not padded to 16 channels, 7x7, ragged
-// channel counts and fp32 outputs stay on the mma.sync kernels of conv_mma.cu.
+// operands; wgrad3x3_halo_kernel for the 3x3 stride-1 ones).  conv_fprop / conv_dgrad / conv_wgrad / convt2x2_fprop at the end of
+// the file re-describe each C-ABI call as these GEMMs, or decline it: 3-channel stems that are not padded to 16 channels, 7x7,
+// ragged channel counts and fp32 outputs stay on the mma.sync kernels of conv_mma.cu.
 //
 // Reference arithmetic replaced: nn.Conv2d forward / input-gradient / weight-gradient as used by
 // modules/qarepvgg_block.py:184-204, modules/conv_bn_act_block.py:92-93,
 // training/models/classification_models/resnet.py:53-84.
 #include <cuda.h>
 
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 
@@ -758,6 +760,12 @@ wgrad3x3_halo_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_co
 }
 
 // ------------------------------------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_tiled = nullptr;
 EncodeIm2colFn g_im2col = nullptr;
 int g_num_sms = 0;
@@ -793,9 +801,79 @@ int init_driver() {
   return SGB_OK;
 }
 
+int encode_tiled(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* byte_strides,
+                 const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* what) {
+  const cuuint32_t elem_strides[5] = {1, 1, 1, 1, 1};
+  const CUresult r = g_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, byte_strides, box,
+                             elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS) return SGB_OK;
+  char shape[256] = "";
+  for (int i = 0, n = 0; i < rank && n < (int)sizeof(shape); ++i)
+    n += snprintf(shape + n, sizeof(shape) - n, "%s%llu (box %u, stride %llu)", i ? ", " : "", (unsigned long long)dims[i],
+                  (unsigned)box[i], i ? (unsigned long long)byte_strides[i - 1] : 2ull);
+  sgb_set_error("cuTensorMapEncodeTiled(%s) failed with %d: dims %s", what, (int)r, shape);
+  return SGB_E_CUDA;
+}
+
+namespace {
+
+// 64 / 32 / 16 bf16 channels per row -> 128B / 64B / 32B swizzle
 CUtensorMapSwizzle swizzle_for(int kc) {
   return kc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (kc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
+
+// The im2col map of an NHWC bf16 tensor (N x H x W x C, `pitch` elements per pixel) traversed at `stride`: each box is `pixels`
+// consecutive output pixels x `channels` channels of one tap; lower / upper are the corners of the filter window ({w, h}).
+int encode_im2col(CUtensorMap* map, const void* ptr, int N, int H, int W, int C, int pitch, int stride, const int (&lower)[2],
+                  const int (&upper)[2], int channels, int pixels, const char* what) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
+  const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  const CUresult r = g_im2col(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper,
+                              (cuuint32_t)channels, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(channels),
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS) return SGB_OK;
+  sgb_set_error("cuTensorMapEncodeIm2col(%s) failed with %d (C=%d W=%d H=%d N=%d pitch=%d lower=%d,%d upper=%d,%d stride=%d box=%d)", what,
+                (int)r, C, W, H, N, pitch, lower[0], lower[1], upper[0], upper[1], stride, channels);
+  return SGB_E_CUDA;
+}
+
+// The input-halo map of the halo kernels: an NHWC bf16 tensor of `pitch` elements per pixel, read as {8 channels, 10, 10, 1}
+// boxes, no swizzle; boxes reaching past the image or past C are zero-filled.
+int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, int pitch) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
+  const cuuint32_t box[4] = {8, HALO_W, HALO_H, 1};
+  return encode_tiled(map, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, "halo");
+}
+
+// One implicit GEMM of the im2col / halo kernels: the R x S filter b (b_rows K-major rows of b_cols columns, b_cols_per_tap per
+// tap) over the NHWC slice a at (stride, pad) onto a P x Q grid, the rows written to y.
+struct Problem {
+  // gathered tensor (NHWC bf16, channel slice): N x H x W x C with channel pitch a_pitch (elements)
+  const void* a;
+  int N, H, W, C, a_pitch;
+  // B matrix: b_rows = GEMM N (output channels of this GEMM), b_cols = taps * b_cols_per_tap, K-major bf16
+  const void* b;
+  int b_rows, b_cols, b_cols_per_tap;
+  int R, S, stride, pad, P, Q, flip;
+  // optional explicit tap table (ntaps > 0): im2col offsets (dh, dw) and B column block of each tap
+  int ntaps;
+  int tap_dh[9], tap_dw[9], tap_b[9];
+  // strided output rows (Params::out_mode)
+  int out_mode, o_mul, oh_add, ow_add, outH, outW;
+  void* y;
+  int y_pitch, y_off;
+  const float* scale;
+  const float* shift;
+  const void* residual;
+  double* stats;
+  int stats_repl, act;
+  // 0, or SgbConvDesc::centre_from: fprop (flip 0) -- output channels from here on have zero off-centre taps; dgrad (flip 1) --
+  // gathered channels from here on meet zero off-centre taps.  Only with R = S = 3, stride 1, pad 1 and no tap table.
+  int centre_from;
+};
 
 bool supported(const Problem& q) {
   if (q.C % 16 != 0 || q.b_rows % 8 != 0) return false;
@@ -808,45 +886,46 @@ bool supported(const Problem& q) {
   return true;
 }
 
-namespace {
-
 // kernel variant of one N tile width + its register footprint (decides how many CTAs can share an SM)
 template <class Fn>
 struct Variant {
   int bn;
   Fn fn;
-  int regs;
-  bool ready;
+  int regs = 0;
+  bool ready = false;
 };
 typedef void (*ConvFn)(const CUtensorMap, const CUtensorMap, const Params);
 typedef void (*WgradFn)(const CUtensorMap, const CUtensorMap, const WParams);
-Variant<ConvFn> g_conv[] = {{16, conv_wgmma_kernel<16, false>, 0, false},   {32, conv_wgmma_kernel<32, false>, 0, false},
-                            {48, conv_wgmma_kernel<48, false>, 0, false},   {64, conv_wgmma_kernel<64, false>, 0, false},
-                            {96, conv_wgmma_kernel<96, false>, 0, false},   {128, conv_wgmma_kernel<128, false>, 0, false}};
-Variant<ConvFn> g_conv_skip[] = {{16, conv_wgmma_kernel<16, true>, 0, false},   {32, conv_wgmma_kernel<32, true>, 0, false},
-                                 {48, conv_wgmma_kernel<48, true>, 0, false},   {64, conv_wgmma_kernel<64, true>, 0, false},
-                                 {96, conv_wgmma_kernel<96, true>, 0, false},   {128, conv_wgmma_kernel<128, true>, 0, false}};
-Variant<ConvFn> g_halo[] = {{16, conv3x3_halo_kernel<16, false>, 0, false},   {32, conv3x3_halo_kernel<32, false>, 0, false},
-                            {48, conv3x3_halo_kernel<48, false>, 0, false},   {64, conv3x3_halo_kernel<64, false>, 0, false},
-                            {96, conv3x3_halo_kernel<96, false>, 0, false},   {128, conv3x3_halo_kernel<128, false>, 0, false}};
-Variant<ConvFn> g_halo_skip[] = {{16, conv3x3_halo_kernel<16, true>, 0, false},   {32, conv3x3_halo_kernel<32, true>, 0, false},
-                                 {48, conv3x3_halo_kernel<48, true>, 0, false},   {64, conv3x3_halo_kernel<64, true>, 0, false},
-                                 {96, conv3x3_halo_kernel<96, true>, 0, false},   {128, conv3x3_halo_kernel<128, true>, 0, false}};
-Variant<WgradFn> g_wgrad[] = {{16, wgrad_wgmma_kernel<16>, 0, false}, {32, wgrad_wgmma_kernel<32>, 0, false},
-                              {48, wgrad_wgmma_kernel<48>, 0, false}, {64, wgrad_wgmma_kernel<64>, 0, false},
-                              {96, wgrad_wgmma_kernel<96>, 0, false}, {128, wgrad_wgmma_kernel<128>, 0, false}};
-Variant<WgradFn> g_wgrad_halo[] = {{16, wgrad3x3_halo_kernel<16>, 0, false}, {32, wgrad3x3_halo_kernel<32>, 0, false},
-                                   {48, wgrad3x3_halo_kernel<48>, 0, false}};
+template <bool SKIP>
+Variant<ConvFn> g_conv[6] = {{16, conv_wgmma_kernel<16, SKIP>}, {32, conv_wgmma_kernel<32, SKIP>},
+                             {48, conv_wgmma_kernel<48, SKIP>}, {64, conv_wgmma_kernel<64, SKIP>},
+                             {96, conv_wgmma_kernel<96, SKIP>}, {128, conv_wgmma_kernel<128, SKIP>}};
+template <bool SKIP>
+Variant<ConvFn> g_halo[6] = {{16, conv3x3_halo_kernel<16, SKIP>}, {32, conv3x3_halo_kernel<32, SKIP>},
+                             {48, conv3x3_halo_kernel<48, SKIP>}, {64, conv3x3_halo_kernel<64, SKIP>},
+                             {96, conv3x3_halo_kernel<96, SKIP>}, {128, conv3x3_halo_kernel<128, SKIP>}};
+Variant<WgradFn> g_wgrad[6] = {{16, wgrad_wgmma_kernel<16>}, {32, wgrad_wgmma_kernel<32>}, {48, wgrad_wgmma_kernel<48>},
+                               {64, wgrad_wgmma_kernel<64>}, {96, wgrad_wgmma_kernel<96>}, {128, wgrad_wgmma_kernel<128>}};
+Variant<WgradFn> g_wgrad_halo[3] = {{16, wgrad3x3_halo_kernel<16>}, {32, wgrad3x3_halo_kernel<32>}, {48, wgrad3x3_halo_kernel<48>}};
 
-template <class Fn>
-int prepare(Variant<Fn>& v, const char* what) {
-  if (v.ready) return SGB_OK;
-  if (int rc = sgb_cuda_check(cudaFuncSetAttribute(v.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), what)) return rc;
+// The variant of tile width bn in `table`; its shared-memory limit is raised and its register count read on first use.
+template <class Fn, int N>
+int prepare(Variant<Fn> (&table)[N], int bn, const char* what, Variant<Fn>*& var) {
+  for (auto& v : table)
+    if (v.bn == bn) var = &v;
+  if (var->ready) return SGB_OK;
+  if (int rc = sgb_cuda_check(cudaFuncSetAttribute(var->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), what)) return rc;
   cudaFuncAttributes fa{};
-  if (int rc = sgb_cuda_check(cudaFuncGetAttributes(&fa, v.fn), what)) return rc;
-  v.regs = fa.numRegs;
-  v.ready = true;
+  if (int rc = sgb_cuda_check(cudaFuncGetAttributes(&fa, var->fn), what)) return rc;
+  var->regs = fa.numRegs;
+  var->ready = true;
   return SGB_OK;
+}
+
+// CTAs of NUM_THREADS threads of `regs` registers each that one SM's 64K registers hold, at most two
+int max_ctas_per_sm(int regs) {
+  const int ctas = 65536 / (((regs + 7) / 8) * 8 * NUM_THREADS);
+  return ctas > 2 ? 2 : (ctas < 1 ? 1 : ctas);
 }
 
 // N tile: the narrowest variant that holds N in one tile, else the widest of 128 / 96 / 64 with the least padding
@@ -893,22 +972,6 @@ int halo_bn(const Problem& q) {
   return 0;
 }
 
-// The input-halo map of the halo kernels: an NHWC bf16 tensor of `pitch` elements per pixel, read as {8 channels, 10, 10, 1}
-// boxes, no swizzle; boxes reaching past the image or past C are zero-filled.
-int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, int pitch) {
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
-  cuuint32_t box[4] = {8, HALO_W, HALO_H, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    sgb_set_error("cuTensorMapEncodeTiled(halo) failed with %d (C=%d W=%d H=%d N=%d pitch=%d)", (int)r, C, W, H, N, pitch);
-    return SGB_E_CUDA;
-  }
-  return SGB_OK;
-}
-
 int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   Params p = p0;
   p.n_tiles = (p.N + bn - 1) / bn;
@@ -920,13 +983,8 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   // idle -- skipping measured 1-4 % slower there (tools/time_zero_taps.py).
   p.centre_n = 0;
   Variant<ConvFn>* var = nullptr;
-  for (auto& v : p.centre_c > 0 ? g_halo_skip : g_halo)
-    if (v.bn == bn) var = &v;
-  if (int rc = prepare(*var, "conv3x3_halo_kernel")) return rc;
-  const int regs_alloc = ((var->regs + 7) / 8) * 8 * NUM_THREADS;
-  int ctas_per_sm = 65536 / regs_alloc;
-  if (ctas_per_sm > 2) ctas_per_sm = 2;
-  if (ctas_per_sm < 1) ctas_per_sm = 1;
+  if (int rc = prepare(p.centre_c > 0 ? g_halo<true> : g_halo<false>, bn, "conv3x3_halo_kernel", var)) return rc;
+  int ctas_per_sm = max_ctas_per_sm(var->regs);
   int stages = 0;
   for (;; --ctas_per_sm) {
     const size_t budget = (ctas_per_sm == 1 ? 227u : 227u / ctas_per_sm - 1u) * 1024u;
@@ -940,19 +998,9 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
 
   alignas(64) CUtensorMap map_a, map_b;
   if (int rc = encode_halo_map(&map_a, q.a, q.N, q.H, q.W, q.C, q.a_pitch)) return rc;
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows};
-    cuuint64_t strides[1] = {(cuuint64_t)q.b_cols * 2};
-    cuuint32_t box[2] = {16, (cuuint32_t)bn};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_tiled(&map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(q.b), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeTiled(halo B) failed with %d (cols=%d rows=%d BN=%d)", (int)r, q.b_cols, q.b_rows, bn);
-      return SGB_E_CUDA;
-    }
-  }
+  const cuuint64_t b_dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows}, b_strides[1] = {(cuuint64_t)q.b_cols * 2};
+  const cuuint32_t b_box[2] = {16, (cuuint32_t)bn};
+  if (int rc = encode_tiled(&map_b, q.b, 2, b_dims, b_strides, b_box, CU_TENSOR_MAP_SWIZZLE_32B, "halo B")) return rc;
   // every CTA serves one N tile: the grid is a multiple of n_tiles
   int per_nt = g_num_sms * ctas_per_sm / p.n_tiles;
   if (per_nt > p.M) per_nt = p.M;
@@ -962,8 +1010,6 @@ int launch_halo(const Problem& q, const Params& p0, int bn, cudaStream_t st) {
   ++g_halo_launches;
   return sgb_cuda_check(cudaGetLastError(), "conv3x3_halo_kernel");
 }
-
-}  // namespace
 
 int launch(const Problem& q, cudaStream_t st) {
   if (int rc = init_driver()) return rc;
@@ -1006,18 +1052,13 @@ int launch(const Problem& q, cudaStream_t st) {
   if (!g_force_im2col)
     if (const int hbn = halo_bn(q)) return launch_halo(q, p, hbn, st);
   Variant<ConvFn>* var = nullptr;
-  for (auto& v : p.centre_n > 0 || p.centre_c > 0 ? g_conv_skip : g_conv)
-    if (v.bn == bn) var = &v;
-  if (int rc = prepare(*var, "conv_wgmma_kernel")) return rc;
+  if (int rc = prepare(p.centre_n > 0 || p.centre_c > 0 ? g_conv<true> : g_conv<false>, bn, "conv_wgmma_kernel", var)) return rc;
   // Small tiles leave the pipeline latency-bound: co-resident CTAs overlap each other's loads, MMAs and epilogues.
   // Limits: registers (64K per SM) and shared memory (228 KB per SM, 227 KB per CTA).
   const uint32_t a_bytes = BLOCK_M * p.KC * 2, b_bytes = ((uint32_t)(bn * p.KC * 2) + 1023u) & ~1023u;
   const uint32_t stage_bytes = a_bytes + b_bytes;
   const uint32_t ctrl_bytes = CTRL_BAR_BYTES + (p.stats ? (uint32_t)(8 * 2 * bn + 2 * p.N) * 4u : 0u);
-  const int regs_alloc = ((var->regs + 7) / 8) * 8 * NUM_THREADS;
-  int ctas_per_sm = 65536 / regs_alloc;
-  if (ctas_per_sm > 2) ctas_per_sm = 2;
-  if (ctas_per_sm < 1) ctas_per_sm = 1;
+  int ctas_per_sm = max_ctas_per_sm(var->regs);
   int stages = 0;
   for (;; --ctas_per_sm) {
     const uint32_t budget = (ctas_per_sm == 1 ? 226u : 227u / ctas_per_sm - 1u) * 1024u;
@@ -1030,39 +1071,16 @@ int launch(const Problem& q, cudaStream_t st) {
   const size_t smem = 1024 + (size_t)stages * stage_bytes + ctrl_bytes;
 
   alignas(64) CUtensorMap map_a, map_b;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)q.C, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
-    cuuint64_t strides[3] = {(cuuint64_t)q.a_pitch * 2, (cuuint64_t)q.W * q.a_pitch * 2, (cuuint64_t)q.H * q.W * q.a_pitch * 2};
-    int lower[2] = {-q.pad, -q.pad};
-    int upper[2] = {q.pad - (q.S - 1), q.pad - (q.R - 1)};
-    if (q.ntaps > 0) {  // explicit tap table (stride-2 dgrad class): base pixel = output-class pixel, no padding
-      lower[0] = lower[1] = 0;
-      upper[0] = q.Q - q.W;
-      upper[1] = q.P - q.H;
-    }
-    cuuint32_t estr[4] = {1, (cuuint32_t)q.stride, (cuuint32_t)q.stride, 1};
-    CUresult r = g_im2col(&map_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.a), dims, strides, lower, upper,
-                          (cuuint32_t)p.KC, (cuuint32_t)BLOCK_M, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(p.KC),
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeIm2col failed with %d (C=%d W=%d H=%d N=%d pitch=%d pad=%d upper=%d,%d stride=%d KC=%d)", (int)r,
-                    q.C, q.W, q.H, q.N, q.a_pitch, q.pad, upper[0], upper[1], q.stride, p.KC);
-      return SGB_E_CUDA;
-    }
+  int lower[2] = {-q.pad, -q.pad}, upper[2] = {q.pad - (q.S - 1), q.pad - (q.R - 1)};
+  if (q.ntaps > 0) {  // explicit tap table: base pixel = output-class pixel, no padding
+    lower[0] = lower[1] = 0;
+    upper[0] = q.Q - q.W;
+    upper[1] = q.P - q.H;
   }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows};
-    cuuint64_t strides[1] = {(cuuint64_t)q.b_cols * 2};
-    cuuint32_t box[2] = {(cuuint32_t)p.KC, (cuuint32_t)bn};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_tiled(&map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(q.b), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(p.KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeTiled(B) failed with %d (cols=%d rows=%d KC=%d BN=%d)", (int)r, q.b_cols, q.b_rows, p.KC, bn);
-      return SGB_E_CUDA;
-    }
-  }
+  if (int rc = encode_im2col(&map_a, q.a, q.N, q.H, q.W, q.C, q.a_pitch, q.stride, lower, upper, p.KC, BLOCK_M, "A")) return rc;
+  const cuuint64_t b_dims[2] = {(cuuint64_t)q.b_cols, (cuuint64_t)q.b_rows}, b_strides[1] = {(cuuint64_t)q.b_cols * 2};
+  const cuuint32_t b_box[2] = {(cuuint32_t)p.KC, (cuuint32_t)bn};
+  if (int rc = encode_tiled(&map_b, q.b, 2, b_dims, b_strides, b_box, swizzle_for(p.KC), "B")) return rc;
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   int grid = m_tiles * p.n_tiles;
   if (grid > g_num_sms * ctas_per_sm) grid = g_num_sms * ctas_per_sm;
@@ -1070,6 +1088,18 @@ int launch(const Problem& q, cudaStream_t st) {
   ++g_launches;
   return sgb_cuda_check(cudaGetLastError(), "conv_wgmma_kernel");
 }
+
+// One weight gradient of the wgrad kernels: dW [K][R][S][C] (fp32, accumulated into) of the R x S filter at (stride, pad) that
+// maps the NHWC slice x onto the P x Q slice dy.
+struct WgradProblem {
+  const void* x;   // NHWC bf16 slice, N x H x W x C
+  const void* dy;  // NHWC bf16 slice, N x P x Q x K
+  int N, H, W, C, x_pitch;
+  int K, y_pitch;
+  int R, S, stride, pad, P, Q;
+  float* dw;       // fp32 [K][R][S][C], accumulated into
+  int centre_from; // 0, or (3x3 only) rows from here on need only their centre tap: their off-centre dw entries are not written
+};
 
 bool wgrad_supported(const WgradProblem& q) {
   if (q.C % 16 != 0 || q.K % 8 != 0) return false;
@@ -1080,8 +1110,6 @@ bool wgrad_supported(const WgradProblem& q) {
   if ((long long)q.N * q.P * q.Q >= (1ll << 31)) return false;
   return true;
 }
-
-namespace {
 
 // Shape rule of wgrad3x3_halo_kernel, from the per-shape timings of tools/time_conv_halo.py: the 3x3 / stride-1 / pad-1 "same"
 // convolutions whose 8 x 8 tiles cover the map with little waste (halo_tiles_fit), where it measured 1.13-5.5x faster than
@@ -1101,10 +1129,8 @@ int launch_wgrad_halo(const WgradProblem& q, const WParams& p0, int nb, cudaStre
   p.halo_thw = p.halo_tw * ((q.P + HALO_TILE - 1) / HALO_TILE);
   p.tiles = q.N * p.halo_thw;
   Variant<WgradFn>* var = nullptr;
-  for (auto& v : g_wgrad_halo)
-    if (v.bn == nb) var = &v;
-  if (int rc = prepare(*var, "wgrad3x3_halo_kernel")) return rc;
-  const int ctas_per_sm = ((var->regs + 7) / 8) * 8 * NUM_THREADS * 2 <= 65536 ? 2 : 1;
+  if (int rc = prepare(g_wgrad_halo, nb, "wgrad3x3_halo_kernel", var)) return rc;
+  const int ctas_per_sm = max_ctas_per_sm(var->regs);
   const uint32_t stage_bytes = wgrad_halo_stage_bytes(nb);
   const uint32_t budget = (ctas_per_sm == 1 ? 227u : 113u) * 1024u - 1024u - CTRL_BAR_BYTES;
   p.stages = (int)(budget / stage_bytes);
@@ -1118,27 +1144,16 @@ int launch_wgrad_halo(const WgradProblem& q, const WParams& p0, int nb, cudaStre
   splits = (p.tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
 
   alignas(64) CUtensorMap map_dy, map_x;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)q.K, (cuuint64_t)q.Q, (cuuint64_t)q.P, (cuuint64_t)q.N};
-    cuuint64_t strides[3] = {(cuuint64_t)q.y_pitch * 2, (cuuint64_t)q.Q * q.y_pitch * 2, (cuuint64_t)q.P * q.Q * q.y_pitch * 2};
-    cuuint32_t box[4] = {64, HALO_TILE, HALO_TILE, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = g_tiled(&map_dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.dy), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      sgb_set_error("cuTensorMapEncodeTiled(dy tile) failed with %d (K=%d Q=%d P=%d N=%d pitch=%d)", (int)r, q.K, q.Q, q.P, q.N, q.y_pitch);
-      return SGB_E_CUDA;
-    }
-  }
+  const cuuint64_t dy_dims[4] = {(cuuint64_t)q.K, (cuuint64_t)q.Q, (cuuint64_t)q.P, (cuuint64_t)q.N};
+  const cuuint64_t dy_strides[3] = {(cuuint64_t)q.y_pitch * 2, (cuuint64_t)q.Q * q.y_pitch * 2, (cuuint64_t)q.P * q.Q * q.y_pitch * 2};
+  const cuuint32_t dy_box[4] = {64, HALO_TILE, HALO_TILE, 1};
+  if (int rc = encode_tiled(&map_dy, q.dy, 4, dy_dims, dy_strides, dy_box, CU_TENSOR_MAP_SWIZZLE_128B, "dy tile")) return rc;
   if (int rc = encode_halo_map(&map_x, q.x, q.N, q.H, q.W, q.C, q.x_pitch)) return rc;
   var->fn<<<splits * items, NUM_THREADS, smem, st>>>(map_dy, map_x, p);
   ++g_launches;
   ++g_wgrad_halo_launches;
   return sgb_cuda_check(cudaGetLastError(), "wgrad3x3_halo_kernel");
 }
-
-}  // namespace
 
 int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   if (int rc = init_driver()) return rc;
@@ -1164,9 +1179,7 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   if (!g_wgrad_force_im2col)
     if (const int nb = wgrad_halo_nb(q)) return launch_wgrad_halo(q, p, nb, st);
   Variant<WgradFn>* var = nullptr;
-  for (auto& v : g_wgrad)
-    if (v.bn == nb) var = &v;
-  if (int rc = prepare(*var, "wgrad_wgmma_kernel")) return rc;
+  if (int rc = prepare(g_wgrad, nb, "wgrad_wgmma_kernel", var)) return rc;
   const uint32_t stage_bytes = 2 * WPIX * 128 + (uint32_t)(nb / p.CB) * WPIX * p.CB * 2;
   int stages = (int)((200 * 1024 - CTRL_BAR_BYTES - 1024) / stage_bytes);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
@@ -1188,32 +1201,167 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   splits = (p.npix + p.pix_per_cta - 1) / p.pix_per_cta;
 
   alignas(64) CUtensorMap map_dy, map_x;
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)q.K, (cuuint64_t)p.npix};
-    cuuint64_t strides[1] = {(cuuint64_t)q.y_pitch * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)WPIX};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_tiled(&map_dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(q.dy), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { sgb_set_error("cuTensorMapEncodeTiled(dy) failed with %d", (int)r); return SGB_E_CUDA; }
-  }
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)q.C, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
-    cuuint64_t strides[3] = {(cuuint64_t)q.x_pitch * 2, (cuuint64_t)q.W * q.x_pitch * 2, (cuuint64_t)q.H * q.W * q.x_pitch * 2};
-    int lower[2] = {-q.pad, -q.pad};
-    int upper[2] = {q.pad - (q.S - 1), q.pad - (q.R - 1)};
-    cuuint32_t estr[4] = {1, (cuuint32_t)q.stride, (cuuint32_t)q.stride, 1};
-    CUresult r = g_im2col(&map_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(q.x), dims, strides, lower, upper,
-                          (cuuint32_t)p.CB, (cuuint32_t)WPIX, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          swizzle_for(p.CB), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { sgb_set_error("cuTensorMapEncodeIm2col(x, wgrad) failed with %d", (int)r); return SGB_E_CUDA; }
-  }
+  const cuuint64_t dy_dims[2] = {(cuuint64_t)q.K, (cuuint64_t)p.npix}, dy_strides[1] = {(cuuint64_t)q.y_pitch * 2};
+  const cuuint32_t dy_box[2] = {64, (cuuint32_t)WPIX};
+  if (int rc = encode_tiled(&map_dy, q.dy, 2, dy_dims, dy_strides, dy_box, CU_TENSOR_MAP_SWIZZLE_128B, "dy")) return rc;
+  const int lower[2] = {-q.pad, -q.pad}, upper[2] = {q.pad - (q.S - 1), q.pad - (q.R - 1)};
+  if (int rc = encode_im2col(&map_x, q.x, q.N, q.H, q.W, q.C, q.x_pitch, q.stride, lower, upper, p.CB, WPIX, "x, wgrad")) return rc;
   const int grid = base_ctas * splits;
   var->fn<<<grid, NUM_THREADS, smem, st>>>(map_dy, map_x, p);
   ++g_launches;
   return sgb_cuda_check(cudaGetLastError(), "wgrad_wgmma_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------ the ABI's calls as GEMMs
+Problem gemm(const sgb_bf16* a, int N, int H, int W, int C, int a_pitch, const sgb_bf16* b, int b_rows, int b_cols_per_tap, int R,
+             int S, int stride, int pad, int P, int Q, void* y, int y_pitch, int y_off) {
+  Problem q{};
+  q.a = a; q.N = N; q.H = H; q.W = W; q.C = C; q.a_pitch = a_pitch;
+  q.b = b; q.b_rows = b_rows; q.b_cols = R * S * b_cols_per_tap; q.b_cols_per_tap = b_cols_per_tap;
+  q.R = R; q.S = S; q.stride = stride; q.pad = pad; q.P = P; q.Q = Q;
+  q.y = y; q.y_pitch = y_pitch; q.y_off = y_off;
+  q.stats_repl = 1;
+  return q;
+}
+
+// The GEMM's P x Q rows are output parity class (ph, pw) of an outH x outW image: row (n, j, i) is pixel (2 j + ph, 2 i + pw).
+void parity_output(Problem& q, int ph, int pw, int outH, int outW) {
+  q.out_mode = 1; q.o_mul = 2; q.oh_add = ph; q.ow_add = pw; q.outH = outH; q.outW = outW;
+}
+
+// The taps of a stride-2 convolution's filter that reach input-gradient parity class (ph, pw): tap r meets row h = 2 j + ph of
+// the input when h + pad - r is even, through dy row j + (ph + pad - r) / 2 (columns alike).
+void stride2_taps(Problem& q, int ph, int pw, int pad) {
+  q.ntaps = 0;
+  for (int r = 0; r < q.R; ++r) {
+    if (((ph + pad - r) & 1) != 0) continue;
+    for (int s = 0; s < q.S; ++s) {
+      if (((pw + pad - s) & 1) != 0) continue;
+      q.tap_dh[q.ntaps] = (ph + pad - r) / 2;
+      q.tap_dw[q.ntaps] = (pw + pad - s) / 2;
+      q.tap_b[q.ntaps] = r * q.S + s;
+      ++q.ntaps;
+    }
+  }
+}
+
+// 2 x 2 / stride 2 / no padding over a dense x (the backward of ConvTranspose2d(2, 2), modules/sampling.py:72-73): the patches
+// do not overlap, so x viewed as the image [N * H/2][2][W/2][2C] -- row pair, row parity, column pair, (column parity, channel)
+// -- turns the layer into a 2 x 1 filter at stride 1 without padding, 2C channels per tap, whose KRSC rows [K][dh][(dw, c)] are
+// those of the 2 x 2 filter.  Returns false when d is not such a call.
+bool row_pairs(const SgbConvDesc& d, SgbConvDesc* pairs) {
+  if (!(d.R == 2 && d.S == 2 && d.stride == 2 && d.pad == 0 && d.x_pitch == d.C && d.x_off == 0 && d.H % 2 == 0 && d.W % 2 == 0 &&
+        d.P == d.H / 2 && d.Q == d.W / 2 && (2 * d.C) % 16 == 0 && d.K % 8 == 0 && d.y_pitch % 8 == 0 && d.y_off % 8 == 0 &&
+        (long long)d.N * (d.H / 2) < (1ll << 31)))
+    return false;
+  *pairs = d;
+  pairs->N = d.N * (d.H / 2); pairs->H = 2; pairs->W = d.W / 2; pairs->C = 2 * d.C; pairs->x_pitch = 2 * d.C;
+  pairs->S = 1; pairs->stride = 1; pairs->P = 1; pairs->Q = d.W / 2;
+  return true;
+}
+
+Problem fprop_problem(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* w, void* y, const SgbEpilogue* ep) {
+  Problem q = gemm(x + d.x_off, d.N, d.H, d.W, d.C, d.x_pitch, w, d.K, d.C, d.R, d.S, d.stride, d.pad, d.P, d.Q, y, d.y_pitch, d.y_off);
+  q.centre_from = d.centre_from;
+  if (ep) {
+    q.scale = ep->scale; q.shift = ep->shift; q.residual = ep->residual; q.stats = ep->stats;
+    q.stats_repl = ep->stats_repl > 0 ? ep->stats_repl : 1; q.act = ep->act;
+  }
+  return q;
+}
+
+WgradProblem wgrad_problem(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* dy, float* dw) {
+  WgradProblem q{};
+  q.x = x + d.x_off; q.dy = dy + d.y_off;
+  q.N = d.N; q.H = d.H; q.W = d.W; q.C = d.C; q.x_pitch = d.x_pitch;
+  q.K = d.K; q.y_pitch = d.y_pitch;
+  q.R = d.R; q.S = d.S; q.stride = d.stride; q.pad = d.pad; q.P = d.P; q.Q = d.Q;
+  q.dw = dw;
+  q.centre_from = d.centre_from;
+  return q;
+}
+
+}  // namespace
+
+int conv_fprop(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* w, void* y, const SgbEpilogue* ep, cudaStream_t st) {
+  if (ep && ep->out_f32) return DECLINED;
+  if (d.pad == d.R / 2) {
+    const Problem q = fprop_problem(d, x, w, y, ep);
+    if (supported(q)) return launch(q, st);
+  }
+  SgbConvDesc pairs;
+  if (!row_pairs(d, &pairs)) return DECLINED;
+  // the 2 x 1 filter as two explicit taps of a 1 x 1 one: rows 0 and 1 of the pair, B column blocks 0 and 1
+  Problem q = fprop_problem(pairs, x, w, y, ep);
+  q.R = 1;
+  q.ntaps = 2;
+  q.tap_dh[1] = 1;
+  q.tap_b[1] = 1;
+  return supported(q) ? launch(q, st) : SGB_E_UNSUPPORTED;
+}
+
+// The transposed convolution as four 1 x 1 GEMMs, one per output parity (dh, dw), each writing the output pixels
+// (2h + dh, 2w + dw) through the strided-row epilogue the stride-2 input gradients use.  w_up rows are ordered (dh, dw, co).
+int convt2x2_fprop(const SgbConvDesc& d, const sgb_bf16* x_small, const sgb_bf16* w_up, const float* bias, sgb_bf16* y_up,
+                   cudaStream_t st) {
+  if (d.K % 16 != 0 || d.C % 16 != 0) return DECLINED;
+  for (int cls = 0; cls < 4; ++cls) {
+    Problem q = gemm(x_small + d.y_off, d.N, d.P, d.Q, d.K, d.y_pitch, w_up + (size_t)cls * d.C * d.K, d.C, d.K, 1, 1, 1, 0, d.P,
+                     d.Q, y_up, d.x_pitch, d.x_off);
+    q.shift = bias;
+    parity_output(q, cls >> 1, cls & 1, d.H, d.W);
+    if (!supported(q)) return DECLINED;  // identical for the four classes: declines before any launch
+    if (int rc = launch(q, st)) return rc;
+  }
+  return SGB_OK;
+}
+
+int conv_dgrad(const SgbConvDesc& d, const sgb_bf16* dy, const sgb_bf16* w_crsk, sgb_bf16* dx, int accumulate, cudaStream_t st) {
+  const int Kp = ((d.K + 7) / 8) * 8;  // channels gathered per tap (w_crsk rows are padded with zeros to Kp)
+  // dy gathered through an R x S filter at stride 1, against the CRSK rows, accumulated into dx or not
+  auto dgrad_gemm = [&](int pad, int P, int Q) {
+    Problem q = gemm(dy + d.y_off, d.N, d.P, d.Q, d.K, d.y_pitch, w_crsk, d.C, Kp, d.R, d.S, 1, pad, P, Q, dx, d.x_pitch, d.x_off);
+    q.residual = accumulate ? dx : nullptr;
+    return q;
+  };
+  if (d.stride == 1 && d.pad == d.R / 2 && d.K % 16 == 0) {
+    // dgrad of a stride-1 "same" convolution == convolution of dy with the spatially flipped CRSK filter
+    Problem q = dgrad_gemm(d.R - 1 - d.pad, d.H, d.W);
+    q.flip = 1;
+    q.centre_from = d.centre_from;
+    if (supported(q)) return launch(q, st);
+  }
+  if (d.stride == 2 && d.K % 16 == 0 && d.R == 3 && d.S == 3 && d.pad == 1 && d.H == 2 * d.P && d.W == 2 * d.Q) {
+    // stride-2 dgrad = 4 output-parity classes, each an exact stride-1 gather of dy with a subset of the taps
+    for (int cls = 0; cls < 4; ++cls) {
+      Problem q = dgrad_gemm(0, d.P, d.Q);
+      parity_output(q, cls >> 1, cls & 1, d.H, d.W);
+      stride2_taps(q, cls >> 1, cls & 1, d.pad);
+      if (!supported(q)) return DECLINED;  // identical for the 4 classes: declines before any launch
+      if (int rc = launch(q, st)) return rc;
+    }
+    return SGB_OK;
+  }
+  if (d.stride == 2 && d.K % 16 == 0 && d.R == 1 && d.S == 1 && d.pad == 0 && d.H == 2 * d.P && d.W == 2 * d.Q) {
+    // 1x1 stride-2 dgrad: only the even/even input pixels receive a gradient.  With accumulate the other three parity
+    // classes are untouched; otherwise they are zero-filled first.
+    Problem q = dgrad_gemm(0, d.P, d.Q);
+    parity_output(q, 0, 0, d.H, d.W);
+    const bool dense = d.x_pitch == d.C && d.x_off == 0;
+    if (supported(q) && (accumulate || dense)) {
+      if (!accumulate) cudaMemsetAsync(dx, 0, (size_t)d.N * d.H * d.W * d.C * sizeof(sgb_bf16), st);
+      return launch(q, st);
+    }
+  }
+  return DECLINED;
+}
+
+int conv_wgrad(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* dy, float* dw, cudaStream_t st) {
+  const WgradProblem q = wgrad_problem(d, x, dy, dw);
+  if (wgrad_supported(q)) return wgrad_launch(q, st);
+  SgbConvDesc pairs;
+  if (row_pairs(d, &pairs)) return wgrad_launch(wgrad_problem(pairs, x, dy, dw), st);
+  return DECLINED;
 }
 
 }  // namespace sm100
