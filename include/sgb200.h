@@ -671,6 +671,29 @@ int sgb_imagenet_augment(const int64_t* table_host, const int64_t* table, const 
                          const float* mean_host, const float* std_host, int32_t mix_mode, float lam, float one_minus_lam,
                          const int32_t* box_host, sgb_bf16* out, void* stream);
 
+/* ---- CIFAR-10 augmentation (recipes/dataset_params/cifar10_dataset_params.yaml:9-23 train chain, torchvision 0.26's: RandomCrop(32,
+ *      padding=4) (F.pad with fill 0, then get_params's two torch.randint draws), RandomHorizontalFlip (torch.rand(1) < 0.5),
+ *      ToTensor (float32 / 255), Normalize (tensor.sub_(mean).div_(std)); cifar10_dataset_params.yaml:37-49 validation chain:
+ *      Resize(32), the identity on the 32 x 32 images of datasets/classification_datasets/cifar.py:14-45, ToTensor, Normalize) ---- */
+/* Per-sample table: int32 [batch][SGB_CF_FIELDS]: the source image's index in src, the crop's top and left corner in the
+ * 40 x 40 zero-padded image (each in [0, 8]; the validation chain is top = left = 4), the horizontal flip flag (0 or 1). */
+#define SGB_CF_SOURCE 0
+#define SGB_CF_TOP 1
+#define SGB_CF_LEFT 2
+#define SGB_CF_FLIP 3
+#define SGB_CF_FIELDS 4
+#define SGB_CF_SIZE 32
+#define SGB_CF_PAD 4
+/* table_host: the table in host memory (validated here); table: the same table in device memory.  src: device uint8
+ * [src_images][32][32][3] RGB (a batch's packed images, or a whole resident data set indexed by the table).  out: device bf16
+ * [batch, 32, 32, out_pitch] (16-byte aligned, out_pitch >= 3 and a multiple of 8; channels >= 3 written as 0).  mean_host[3] /
+ * std_host[3]: Normalize.  ONE launch for the batch: per output pixel, the zero-padded crop -> flip -> ToTensor / Normalize in
+ * float32 with IEEE division in torchvision's order -> round-to-nearest-even bf16.  Bit-exact with torchvision's chain rounded to
+ * bf16.  batch < 1, a source index outside [0, src_images), a crop corner outside [0, 8], a flip flag other than 0 / 1, a bad
+ * pitch, a misaligned out or a non-finite mean / std (or a zero std) is refused with SGB_E_INVALID. */
+int sgb_cifar_augment(const int32_t* table_host, const int32_t* table, const uint8_t* src, int64_t src_images, int32_t batch,
+                      int32_t out_pitch, const float* mean_host, const float* std_host, sgb_bf16* out, void* stream);
+
 /* ---- pose train augmentation (training/transforms/keypoints/*.py of the YOLO-NAS-POSE recipes: KeypointsRandomHorizontalFlip,
  *      KeypointsBrightnessContrast, KeypointsReverseImageChannels, KeypointsHSV, KeypointsRandomRotate90,
  *      KeypointsRandomAffineTransform, KeypointsMosaic, KeypointsLongestMaxSize, KeypointsPadIfNeeded, KeypointsImageStandardize) ---- */

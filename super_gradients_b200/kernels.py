@@ -496,6 +496,32 @@ def imagenet_augment(table_host, table, src, workspace, out, fill, mean, std, mi
     return out
 
 
+CF_FIELDS = 4  # SGB_CF_FIELDS: per-sample (source index, crop top, crop left, flip) of the CIFAR-10 augmentation (include/sgb200.h)
+CF_IMAGE_BYTES = 32 * 32 * 3
+
+
+def cifar_augment(table_host, table, src, out, mean, std):
+    """CIFAR-10 augmentation of a whole batch in one launch.  table_host: int32 [B, CF_FIELDS] CPU tensor (sgb200.h SGB_CF_*),
+    table: the same on the device; src: contiguous device uint8 [N, 32, 32, 3] images the table's source column indexes (a batch's
+    packed images or a resident data set); out: bf16 NHWC [B, c_pad, 32, 32] (channels >= 3 are zeroed); mean / std: Normalize's."""
+    for t, n in ((src, "src"), (table, "table"), (out, "out")):
+        require_cuda(t, n)
+    if out.data_ptr() % 16 or table.data_ptr() % 16:
+        raise L.SgbError("out and table must be 16-byte aligned (the kernel stores 8 channels and loads one table row at a time)")
+    if table_host.dtype != torch.int32 or table_host.dim() != 2 or table_host.shape[1] != CF_FIELDS or not table_host.is_contiguous() or table_host.is_cuda:
+        raise L.SgbError(f"table_host must be a contiguous int32 [B, {CF_FIELDS}] host tensor")
+    if table.dtype != torch.int32 or tuple(table.shape) != tuple(table_host.shape) or not table.is_contiguous():
+        raise L.SgbError("table must be the device copy of table_host")
+    if src.dtype != torch.uint8 or not src.is_contiguous() or src.numel() % CF_IMAGE_BYTES:
+        raise L.SgbError("src must be contiguous uint8 32 x 32 x 3 images")
+    B, pitch = table_host.shape[0], nhwc_pitch(out)
+    if out.dtype != torch.bfloat16 or out.shape[0] != B or out.shape[1] != pitch or tuple(out.shape[2:]) != (32, 32):
+        raise L.SgbError("out must be a dense bf16 NHWC batch [B, c_pad, 32, 32]")
+    m, s = (ctypes.c_float * 3)(*[float(v) for v in mean]), (ctypes.c_float * 3)(*[float(v) for v in std])
+    _timed("sgb_cifar_augment", ctypes.c_void_p(table_host.data_ptr()), _ptr(table), _ptr(src), src.numel() // CF_IMAGE_BYTES, B, pitch, m, s, _ptr(out), _stream())
+    return out
+
+
 POSE_FIELDS = 144  # SGB_POSE_FIELDS: per-sample draws of the pose train augmentation (include/sgb200.h)
 
 

@@ -284,7 +284,7 @@ class TrainStep:
         self.replays = 0           # steps that replayed the captured graph
         # run_padded: host targets padded into a pinned staging ring and copied into the graph's static target buffer
         self.n_max = None          # n_max of the captured padded-target graph (None: no such graph)
-        self.fallbacks = 0         # run_padded steps that ran eagerly beside a captured graph
+        self.fallbacks = 0         # steps that ran eagerly beside a captured graph
         self._n_floor = 0          # n_max agreed at the end of an epoch with an overflow: the floor of the next capture
         self._overflow_need = 0    # largest need this epoch of the steps that exceeded n_max
         self._warned_overflow = False
@@ -406,12 +406,16 @@ class TrainStep:
 
     def run(self, inputs, targets, do_optimizer_step=True):
         """inputs / targets: device tensors (targets may be any structure the criterion accepts).  With a captured
-        graph the tensors are copied into the static buffers first (inputs that ARE the static input are not copied)."""
-        if self.graph is not None:
+        graph the tensors are copied into the static buffers first (inputs that ARE the static input are not copied); a batch of
+        another size than the captured one (a loader's short last batch) runs eagerly beside the graph."""
+        if self.graph is not None and tuple(inputs.shape) == tuple(self.static_in[0].shape):
             self._check_replay(do_optimizer_step)
             self._copy_static(self.static_in, (inputs, targets))
             loss, items = self._replay(do_optimizer_step)
         else:
+            if self.graph is not None:
+                self.fallbacks += 1
+                self._arena_replayed()
             loss, items = self._step_eager(inputs, targets, do_optimizer_step)
         if do_optimizer_step:
             self.opt_steps += 1
@@ -595,9 +599,9 @@ class TrainStep:
     def _capture_region(self, fn, pool=None):
         """Records fn() into a CUDA graph; returns (graph, fn's outputs = the graph's static output tensors)."""
         g = torch.cuda.CUDAGraph()
-        # with NCCL in the process other threads (the process-group watchdog) touch CUDA during capture: thread-local capture mode
-        # keeps those calls from invalidating it
-        kw = {"capture_error_mode": "thread_local" if self.world > 1 else "global"}
+        # other threads may touch CUDA during capture -- NCCL's process-group watchdog, a DataLoader's pin-memory thread allocating
+        # pinned host memory for the next batches: thread-local capture mode keeps those calls from invalidating it
+        kw = {"capture_error_mode": "thread_local"}
         if pool is not None:
             kw["pool"] = pool
         with torch.cuda.graph(g, **kw):
