@@ -474,6 +474,22 @@ int sgb_detection_matching(const SgbMatchDesc* d, const float* preds, const int3
                            const int32_t* target_count, const float* crowd, const int32_t* crowd_count, const float* thresholds,
                            uint8_t* matched, uint8_t* ignore, void* stream);
 
+/* ---- DetectionMetricsDistanceBased matching (training/utils/detection_utils.py:1196-1290 with DistanceMatching :1008-1118,
+ * EuclideanDistance / ManhattanDistance :1293-1340, get_top_k_idx_per_cls :1342-1359; metric: training/metrics/detection_metrics.py:295-374) ----
+ * The buffers, layouts and outputs of sgb_detection_matching, with the distance between box centres as the pair score: a
+ * prediction matches the nearest free same-class target (lowest index on equal distances) when distance < threshold (strict), and
+ * is ignored at threshold j when its nearest same-class crowd target is nearer than thresholds[j].  Euclidean: sqrt(dx*dx + dy*dy)
+ * with single-rounded products, add and sqrt; Manhattan: |dx| + |dy|.  thresholds [n_thresholds] f32 pixel distances, in any
+ * order, live in HOST memory (they are checked here and travel in the launch parameters).  An unknown metric, a non-finite or
+ * negative threshold, more than SGB_MATCH_MAX_THRESHOLDS thresholds or an image over the 200 KB shared-memory bound is refused
+ * with SGB_E_INVALID. */
+#define SGB_DISTANCE_EUCLIDEAN 0
+#define SGB_DISTANCE_MANHATTAN 1
+int sgb_detection_distance_matching(const SgbMatchDesc* d, int32_t metric, const float* preds, const int32_t* pred_count,
+                                    const float* targets, const int32_t* target_count, const float* crowd,
+                                    const int32_t* crowd_count, const float* thresholds, uint8_t* matched, uint8_t* ignore,
+                                    void* stream);
+
 /* ---- PoseEstimationMetrics matching (training/metrics/pose_estimation_metrics.py:237-314, pose_estimation_utils.py:35-263) ---- */
 /* poses [B, max_preds, n_joints, 3] f32 (x, y, joint score; only x, y are read), scores [B, max_preds] f32, pred_count [B] (rows
  * in any order; the top_k by score are used); gt_joints [B, max_targets, n_joints, 3] f32 (x, y, visibility), gt_boxes

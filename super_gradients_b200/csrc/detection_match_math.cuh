@@ -120,4 +120,61 @@ SGB_HD float best_crowd_ioa(Box p, float area_p, float cls_p, const Box* cbox, c
   return nan ? NAN : best;
 }
 
+// ---- DistanceMatching (detection_utils.py:1008-1118) with EuclideanDistance / ManhattanDistance (:1293-1340) ----
+// The pair score is the distance between box centres, (x1 + x2) / 2 and (y1 + y2) / 2 of the clipped prediction and of the
+// (denormalised) target; a different class is +inf.  Per prediction the reference visits the targets by stable ascending
+// distance and takes, for threshold j, the first one still free at j with distance < thr[j] (strict) -- i.e. the nearest free
+// target, lowest index on ties, if it is nearer than thr[j].  Crowd targets: min distance < thr[j] switches "ignore" on.
+enum DistanceMetric { kEuclidean = 0, kManhattan = 1 };
+
+struct Point {
+  float x, y;
+};
+
+SGB_HD Point centre(Box b) { return Point{fdiv(fadd(b.x1, b.x2), 2.f), fdiv(fadd(b.y1, b.y2), 2.f)}; }
+
+// sqrt(dx * dx + dy * dy): two rounded products, one rounded add, a correctly rounded sqrt (== torch's (diff**2).sum(2).sqrt());
+// |dx| + |dy| for Manhattan
+SGB_HD float centre_distance(int metric, Point a, Point b) {
+  const float dx = fsub(a.x, b.x), dy = fsub(a.y, b.y);
+  if (metric == kManhattan) return fadd(fabsf(dx), fabsf(dy));
+#ifdef __CUDA_ARCH__
+  return __fsqrt_rn(fadd(fmul(dx, dx), fmul(dy, dy)));
+#else
+  return sqrtf(fadd(fmul(dx, dx), fmul(dy, dy)));
+#endif
+}
+
+// The free same-class target of smallest distance < thr among targets first, first + step, ... (lanes as best_free_target;
+// merge with nearer()).  NaN distances never match, as NaN sorts last and fails `< thr` in the reference.
+SGB_HD Best nearest_free_target(int metric, Point p, float cls_p, float thr, const Box* tbox, const float* tcls, const uint8_t* taken,
+                                int n_targets, int first, int step) {
+  Best b{thr, -1};
+  for (int t = first; t < n_targets; t += step) {
+    if (tcls[t] != cls_p || taken[t]) continue;
+    const float v = centre_distance(metric, p, centre(tbox[t]));
+    if (v < b.v) b = Best{v, t};  // ascending t keeps the first of equal distances (the stable sort's order)
+  }
+  return b;
+}
+
+SGB_HD Best nearer(Best a, Best b) {
+  if (b.t < 0) return a;
+  if (a.t < 0) return b;
+  return (b.v < a.v || (b.v == a.v && b.t < a.t)) ? b : a;
+}
+
+// min over the same-class crowd targets of the centre distance (+inf when there is none), with torch.min's NaN propagation
+SGB_HD float nearest_crowd_distance(int metric, Point p, float cls_p, const Box* cbox, const float* ccls, int n_crowd) {
+  float best = INFINITY;
+  bool nan = false;
+  for (int c = 0; c < n_crowd; ++c) {
+    if (ccls[c] != cls_p) continue;
+    const float v = centre_distance(metric, p, centre(cbox[c]));
+    if (v != v) nan = true;
+    else if (v < best) best = v;
+  }
+  return nan ? NAN : best;
+}
+
 }  // namespace sgb_match

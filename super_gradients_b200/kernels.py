@@ -608,6 +608,35 @@ def detection_matching(preds, pred_count, targets, target_count, crowd, crowd_co
     return matched, ignore
 
 
+DISTANCE_METRICS = {"euclidean": 0, "manhattan": 1}  # SGB_DISTANCE_EUCLIDEAN / SGB_DISTANCE_MANHATTAN
+
+
+def detection_distance_matching(preds, pred_count, targets, target_count, crowd, crowd_count, thresholds, metric, height, width, top_k=100, denormalize_targets=True):
+    """DetectionMetricsDistanceBased matching of one batch: the buffers of detection_matching, box-centre distance as the pair
+    score.  thresholds: pixel distances (a sequence of floats or a host tensor, any order), read on the host -- no device copy;
+    metric: "euclidean" or "manhattan".  Returns (matched, ignore) uint8 [B, P, T]."""
+    require_cuda(preds, "preds")
+    for name, t, dt in (("preds", preds, torch.float32), ("targets", targets, torch.float32), ("pred_count", pred_count, torch.int32), ("target_count", target_count, torch.int32)):
+        if t.dtype != dt or not t.is_contiguous() or t.device != preds.device:
+            raise L.SgbError(f"{name} must be a contiguous {dt} tensor on {preds.device}")
+    if preds.dim() != 3 or preds.shape[2] != 6 or targets.dim() != 3 or targets.shape[2] != 5 or targets.shape[0] != preds.shape[0]:
+        raise L.SgbError("preds must be [B, P, 6] and targets [B, M, 5]")
+    if crowd is not None and (crowd.dtype != torch.float32 or not crowd.is_contiguous() or crowd.dim() != 3 or crowd.shape[2] != 5 or crowd.shape[0] != preds.shape[0] or crowd_count.dtype != torch.int32):
+        raise L.SgbError("crowd targets must be a contiguous float32 [B, C, 5] tensor with int32 counts")
+    if metric not in DISTANCE_METRICS:
+        raise L.SgbError(f"distance metric must be one of {sorted(DISTANCE_METRICS)}, got {metric!r}")
+    if crowd is not None and crowd.shape[1] == 0:
+        crowd = crowd_count = None
+    thr = [float(v) for v in (thresholds.tolist() if isinstance(thresholds, torch.Tensor) else thresholds)]
+    host_thr = (ctypes.c_float * len(thr))(*thr)
+    d = match_desc(preds, targets, crowd, len(thr), height, width, top_k, denormalize_targets)
+    matched = torch.empty((d.B, d.max_preds, d.n_thresholds), dtype=torch.uint8, device=preds.device)
+    ignore = torch.empty_like(matched)
+    _timed("sgb_detection_distance_matching", ctypes.byref(d), DISTANCE_METRICS[metric], _ptr(preds), _ptr(pred_count), _ptr(targets), _ptr(target_count),
+           _ptr(crowd) if crowd is not None else None, _ptr(crowd_count) if crowd is not None else None, ctypes.cast(host_thr, ctypes.c_void_p), _ptr(matched), _ptr(ignore), _stream())  # fmt: skip
+    return matched, ignore
+
+
 def pose_keypoint_matching(poses, scores, pred_count, gt_joints, gt_boxes, gt_areas, gt_flags, gt_count, sigmas, thresholds, top_k, oks_out=False):
     """PoseEstimationMetrics matching of one batch.  poses [B, P, J, 3] f32 (x, y, joint score), scores [B, P] f32, pred_count [B]
     int32; gt_joints [B, M, J, 3] f32 (x, y, visibility), gt_boxes [B, M, 4] f32 XYWH, gt_areas [B, M] f32, gt_flags [B, M] uint8

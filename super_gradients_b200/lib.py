@@ -223,6 +223,7 @@ _SIGNATURES = {
     "sgb_imagenet_augment": (c_int, [P, P, P, _L, P, _L, _I, _I, _I, P, P, P, _I, c_float, c_float, P, P, P]),
     "sgb_cifar_augment": (c_int, [P, P, P, _L, _I, _I, P, P, P, P]),
     "sgb_detection_matching": (c_int, [POINTER(MatchDesc), P, P, P, P, P, P, P, P, P, P]),
+    "sgb_detection_distance_matching": (c_int, [POINTER(MatchDesc), c_int32, P, P, P, P, P, P, P, P, P, P]),
     "sgb_pose_keypoint_matching": (c_int, [P] * 10 + [_I] * 6 + [P] * 7),
     "sgb_pose_tal_workspace_bytes": (c_int64, [POINTER(PoseLossDesc)]),
     "sgb_pose_tal_assign": (c_int, [POINTER(PoseLossDesc)] + [P] * 14 + [_L, P]),

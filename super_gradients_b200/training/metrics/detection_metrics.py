@@ -9,14 +9,15 @@ inputs, crowd_targets)`, `compute()` keys and `greater_component_is_better` so `
 written for the reference work unchanged.  It is a plain object (torchmetrics is not a dependency): `reset()` clears the state,
 and in a distributed run `compute()` gathers every rank's flags (all_gather_object, as the reference's _sync_dist does)."""
 import collections
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 from torch import Tensor
 
 from ...common.registry import register_metric
-from ..utils.detection_utils import IouThreshold, compute_detection_matching_batched, compute_detection_metrics, pad_predictions
+from ..utils.detection_utils import (DistanceMatching, DistanceMetric, EuclideanDistance, IouThreshold, compute_detection_matching_batched, compute_detection_matching_with,
+                                     compute_detection_metrics, pad_predictions)  # fmt: skip
 
 
 @register_metric("DetectionMetrics")
@@ -82,14 +83,21 @@ class DetectionMetrics:
             out = cb(preds, device=device) if cb is not None else preds
             dev = next((o.device for o in out if o is not None), inputs.device)
             rows, counts = pad_predictions(out, dev)
+        matched, ignore = self._match(rows, counts, target, height, width, crowd_targets)
+        self._batches.append((rows[..., 4:6], counts, matched, ignore, target.detach()[:, 1].float().cpu().clone()))
+
+    def _match(self, rows, counts, target, height, width, crowd_targets):
+        """The batch's one matching launch: (matched, ignore) uint8 [B, P, T] on the device."""
         if self._thr_dev is None or self._thr_dev.device != rows.device:
             self._thr_dev = self.iou_thresholds.to(rows.device)
-        matched, ignore = compute_detection_matching_batched(rows, counts, target, height, width, self._thr_dev, self.denormalize_targets, crowd_targets, self.top_k_predictions)
-        self._batches.append((rows[..., 4:6], counts, matched, ignore, target.detach()[:, 1].float().cpu().clone()))
+        return compute_detection_matching_batched(rows, counts, target, height, width, self._thr_dev, self.denormalize_targets, crowd_targets, self.top_k_predictions)
+
+    def _n_thresholds(self) -> int:
+        return len(self.iou_thresholds)
 
     def _matching_info(self):
         """Device state -> the reference's five flat tensors (preds_matched, preds_to_ignore, scores, classes, target classes)."""
-        T = len(self.iou_thresholds)
+        T = self._n_thresholds()
         m, g, s, c, t = [torch.zeros((0, T), dtype=torch.bool)], [torch.zeros((0, T), dtype=torch.bool)], [torch.zeros(0)], [torch.zeros(0)], [torch.zeros(0)]
         for sc_cls, counts, matched, ignore, tcls in self._batches:
             counts = counts.cpu()
@@ -129,6 +137,39 @@ class DetectionMetrics:
             for n, v in zip(self.best_threshold_per_class_names, best_score_threshold_per_cls):
                 out[n] = float(v)
         return out
+
+
+@register_metric("DetectionMetricsDistanceBased")
+class DetectionMetricsDistanceBased(DetectionMetrics):
+    """DetectionMetricsDistanceBased (detection_metrics.py:295-374): DetectionMetrics with a true positive defined by the distance
+    between box centres (EuclideanDistance or ManhattanDistance, in pixels, strictly below the threshold) instead of IoU -- for
+    point-like or tiny objects and crowded scenes.  update() is the batched NMS plus ONE distance-matching launch
+    (csrc/detection_match.cu), with no device->host synchronisation; compute(), reset() and the distributed gather are
+    DetectionMetrics'.  Keys carry the prefix "distance_based_" and the range "@DIST5.00" / "@DIST5.00:10.00"."""
+
+    def __init__(self, num_cls: int, post_prediction_callback, normalize_targets: bool = False, distance_thresholds: Sequence[float] = (5.0,),
+                 distance_metric: DistanceMetric = EuclideanDistance(), recall_thres: Tensor = None, score_thres: float = 0.1, top_k_predictions: int = 100,
+                 dist_sync_on_step: bool = False, accumulate_on_cpu: bool = True, calc_best_score_thresholds: bool = True, include_classwise_ap: bool = False,
+                 class_names: List[str] = None):  # fmt: skip
+        # the range string -- and so every component name -- is built from these inside DetectionMetrics.__init__
+        self.distance_thresholds = distance_thresholds
+        self.distance_metric = distance_metric
+        self._matcher = DistanceMatching(distance_metric, distance_thresholds)
+        self._matcher.kernel_metric()  # a metric without a kernel fails here, not at the first validation batch
+        DetectionMetrics.__init__(self, num_cls=num_cls, post_prediction_callback=post_prediction_callback, normalize_targets=normalize_targets, recall_thres=recall_thres,
+                                  score_thres=score_thres, top_k_predictions=top_k_predictions, dist_sync_on_step=dist_sync_on_step, accumulate_on_cpu=accumulate_on_cpu,
+                                  calc_best_score_thresholds=calc_best_score_thresholds, include_classwise_ap=include_classwise_ap, class_names=class_names,
+                                  state_dict_prefix="distance_based_")  # fmt: skip
+
+    def _get_range_str(self):
+        t = self.distance_thresholds
+        return "@DIST%.2f" % t[0] if not len(t) > 1 else "@DIST%.2f:%.2f" % (t[0], t[-1])
+
+    def _match(self, rows, counts, target, height, width, crowd_targets):
+        return compute_detection_matching_with(self._matcher, rows, counts, target, height, width, self.denormalize_targets, crowd_targets, self.top_k_predictions)
+
+    def _n_thresholds(self) -> int:
+        return len(self.distance_thresholds)
 
 
 def _fixed(name, iou_thres):

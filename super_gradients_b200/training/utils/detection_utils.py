@@ -4,10 +4,12 @@ kernel as the PP-YOLOE / YOLO-NAS callback (csrc/nms.cu), i.e. for the whole bat
 images around torchvision.  The kernel keeps its IoU bit-matrix in shared memory, so an image may have at most 1024 candidates
 above the confidence threshold; more raise (the reference has no such limit).
 
-Second half (row (f)-N4): the DetectionMetrics helpers -- IouThreshold, target / prediction padding, the batched matching kernel's
-wrapper with the reference's `compute_detection_matching` signature on top, and the precision / recall / AP summary."""
+Second half (row (f)-N4): the DetectionMetrics helpers -- IouThreshold, target / prediction padding, the matching strategies
+(IoUMatching, DistanceMatching with EuclideanDistance / ManhattanDistance), the batched matching kernels' wrappers with the
+reference's `compute_detection_matching` signature on top, and the precision / recall / AP summary."""
 import enum
-from typing import List, Optional, Tuple
+from abc import ABC, abstractmethod
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -104,22 +106,73 @@ class IoUMatching:
         return self.iou_thresholds
 
 
+class DistanceMetric(ABC):
+    """detection_utils.py:1293-1296.  Only the two metrics below have a kernel (csrc/detection_match.cu); calculate_distance is the
+    reference's torch expression, kept as the definition the kernel is tested against."""
+
+    @abstractmethod
+    def calculate_distance(self, predicted: Tensor, target: Tensor) -> Tensor:
+        pass
+
+
+class EuclideanDistance(DistanceMetric):
+    """detection_utils.py:1299-1318: L2 distance between box centres, [N, 4] x [M, 4] XYXY -> [N, M]."""
+
+    def calculate_distance(self, predicted: Tensor, target: Tensor) -> Tensor:
+        centers1 = (predicted[:, :2] + predicted[:, 2:]) / 2
+        centers2 = (target[:, :2] + target[:, 2:]) / 2
+        diff = centers1.view(-1, 1, 2) - centers2.view(1, -1, 2)
+        return torch.sqrt((diff**2).sum(dim=2))
+
+
+class ManhattanDistance(DistanceMetric):
+    """detection_utils.py:1321-1339: L1 distance between box centres, [N, 4] x [M, 4] XYXY -> [N, M]."""
+
+    def calculate_distance(self, predicted: Tensor, target: Tensor) -> Tensor:
+        centers1 = (predicted[:, :2] + predicted[:, 2:]) / 2
+        centers2 = (target[:, :2] + target[:, 2:]) / 2
+        diff = centers1.view(-1, 1, 2) - centers2.view(1, -1, 2)
+        return torch.abs(diff).sum(dim=2)
+
+
+# the kernel's name of each metric it implements (exact types: a subclass may redefine the distance)
+_KERNEL_DISTANCE = {EuclideanDistance: "euclidean", ManhattanDistance: "manhattan"}
+
+
+class DistanceMatching:
+    """DistanceMatching (detection_utils.py:1008-1030): a prediction matches the nearest free same-class target whose box centre is
+    nearer than the threshold (pixels, strict); compute_targets / compute_crowd_targets are the distance matching kernel."""
+
+    def __init__(self, distance_metric: DistanceMetric, distance_thresholds: Union[Sequence[float], Tensor]):
+        self.distance_metric = distance_metric
+        self.distance_thresholds = distance_thresholds
+
+    def get_thresholds(self) -> Tensor:
+        return torch.tensor(self.distance_thresholds)
+
+    def kernel_metric(self) -> str:
+        """The kernel's name of the distance metric; any other DistanceMetric raises."""
+        name = _KERNEL_DISTANCE.get(type(self.distance_metric))
+        if name is None:
+            raise NotImplementedError(f"only EuclideanDistance and ManhattanDistance have a kernel, got {type(self.distance_metric).__name__}")
+        return name
+
+
 @torch.no_grad()
 def compute_detection_matching(output: List[Optional[Tensor]], targets: Tensor, height: int, width: int, denormalize_targets: bool, device: str = None,
                                iou_thresholds: Tensor = None, crowd_targets: Optional[Tensor] = None, top_k: int = 100, return_on_cpu: bool = True,
-                               matching_strategy: IoUMatching = None) -> List[Tuple]:  # fmt: skip
+                               matching_strategy: Union[IoUMatching, DistanceMatching] = None) -> List[Tuple]:  # fmt: skip
     """The reference's signature and return value (detection_utils.py:1120-1193): per image (preds_matched [n, T] bool,
     preds_to_ignore [n, T] bool, scores [n], classes [n], target classes).  One kernel launch for the batch
-    (compute_detection_matching_batched), then one device->host copy to split the flags per image."""
+    (compute_detection_matching_with), then one device->host copy to split the flags per image."""
     if matching_strategy is None:
         raise ValueError("matching_strategy must not be None")
-    if not isinstance(matching_strategy, IoUMatching):
-        raise NotImplementedError("only IoUMatching has a kernel (DistanceMatching is not on the YOLO-NAS validation path)")
-    thr = matching_strategy.get_thresholds()
+    if not isinstance(matching_strategy, (IoUMatching, DistanceMatching)):
+        raise NotImplementedError(f"only IoUMatching and DistanceMatching have a kernel, got {type(matching_strategy).__name__}")
     output = list(output)
     dev = next((o.device for o in output if o is not None), torch.device(device) if device is not None else targets.device)
     rows, counts = pad_predictions(output, dev)
-    matched, ignore = compute_detection_matching_batched(rows, counts, targets, height, width, thr, denormalize_targets, crowd_targets, top_k)
+    matched, ignore = compute_detection_matching_with(matching_strategy, rows, counts, targets, height, width, denormalize_targets, crowd_targets, top_k)
     if return_on_cpu:
         rows, matched, ignore = rows.cpu(), matched.cpu(), ignore.cpu()
     t = targets.detach().float().to(rows.device)
@@ -130,6 +183,17 @@ def compute_detection_matching(output: List[Optional[Tensor]], targets: Tensor, 
     return res
 
 
+def _padded_targets(dev, B: int, targets: Tensor, crowd_targets: Optional[Tensor]):
+    """The reference's flat [N, 6] targets / crowd targets -> the kernels' padded per-image layout on `dev` (crowd: None, None when
+    there is none)."""
+    t_pad, t_cnt = pad_matching_targets_host(targets, B)
+    c_pad = c_cnt = None
+    if crowd_targets is not None and crowd_targets.numel():
+        c_pad, c_cnt = pad_matching_targets_host(crowd_targets, B)
+        c_pad, c_cnt = c_pad.to(dev, non_blocking=True), c_cnt.to(dev, non_blocking=True)
+    return t_pad.to(dev, non_blocking=True), t_cnt.to(dev, non_blocking=True), c_pad, c_cnt
+
+
 @torch.no_grad()
 def compute_detection_matching_batched(rows: Tensor, counts: Tensor, targets: Tensor, height: int, width: int, iou_thresholds: Tensor, denormalize_targets: bool,
                                        crowd_targets: Optional[Tensor] = None, top_k: int = 100) -> Tuple[Tensor, Tensor]:  # fmt: skip
@@ -138,14 +202,25 @@ def compute_detection_matching_batched(rows: Tensor, counts: Tensor, targets: Te
     (image, class, cx, cy, w, h) tensors (read on the host, where the data loader left them).  Returns uint8 [B, P, T] tensors
     (preds_matched, preds_to_ignore); prediction rows past counts[b] are zero."""
     dev = rows.device
-    B = rows.shape[0]
-    t_pad, t_cnt = pad_matching_targets_host(targets, B)
-    c_pad = c_cnt = None
-    if crowd_targets is not None and crowd_targets.numel():
-        c_pad, c_cnt = pad_matching_targets_host(crowd_targets, B)
-        c_pad, c_cnt = c_pad.to(dev, non_blocking=True), c_cnt.to(dev, non_blocking=True)
-    return K.detection_matching(rows.contiguous().float(), counts.to(torch.int32), t_pad.to(dev, non_blocking=True), t_cnt.to(dev, non_blocking=True), c_pad, c_cnt,
-                                iou_thresholds.to(device=dev, dtype=torch.float32).contiguous(), height, width, top_k, denormalize_targets)  # fmt: skip
+    t_pad, t_cnt, c_pad, c_cnt = _padded_targets(dev, rows.shape[0], targets, crowd_targets)
+    return K.detection_matching(rows.contiguous().float(), counts.to(torch.int32), t_pad, t_cnt, c_pad, c_cnt, iou_thresholds.to(device=dev, dtype=torch.float32).contiguous(),
+                                height, width, top_k, denormalize_targets)  # fmt: skip
+
+
+@torch.no_grad()
+def compute_detection_matching_with(matching_strategy: Union[IoUMatching, DistanceMatching], rows: Tensor, counts: Tensor, targets: Tensor, height: int, width: int,
+                                    denormalize_targets: bool, crowd_targets: Optional[Tensor] = None, top_k: int = 100) -> Tuple[Tensor, Tensor]:  # fmt: skip
+    """compute_detection_matching_batched for either strategy: IoUMatching runs the IoU kernel, DistanceMatching
+    (detection_utils.py:1008-1118) the centre-distance kernel -- one launch for the batch either way, same inputs and outputs.  The
+    distance thresholds are read on the host (they are launch parameters), so no device synchronisation happens here."""
+    if isinstance(matching_strategy, IoUMatching):
+        return compute_detection_matching_batched(rows, counts, targets, height, width, matching_strategy.get_thresholds(), denormalize_targets, crowd_targets, top_k)
+    if not isinstance(matching_strategy, DistanceMatching):
+        raise NotImplementedError(f"only IoUMatching and DistanceMatching have a kernel, got {type(matching_strategy).__name__}")
+    metric = matching_strategy.kernel_metric()
+    t_pad, t_cnt, c_pad, c_cnt = _padded_targets(rows.device, rows.shape[0], targets, crowd_targets)
+    return K.detection_distance_matching(rows.contiguous().float(), counts.to(torch.int32), t_pad, t_cnt, c_pad, c_cnt, matching_strategy.get_thresholds(), metric, height, width,
+                                         top_k, denormalize_targets)  # fmt: skip
 
 
 def compute_detection_metrics_per_cls(preds_matched: Tensor, preds_to_ignore: Tensor, preds_scores: Tensor, n_targets, recall_thresholds: Tensor, score_threshold: float, device="cpu"):
