@@ -291,6 +291,7 @@ struct WgradParams {
   int npix;          // N*P*Q
   int slices_per_z;  // BK-pixel slices handled by one blockIdx.z
   int ncols;         // R*S*C
+  int centre_from;   // 0, or (3x3) the first row whose off-centre entries are left as they are
 };
 
 template <int CPR>
@@ -426,7 +427,8 @@ __global__ void __launch_bounds__(THREADS) wgrad_kernel(const __grid_constant__ 
         int col = n0 + wn * WTN + nt * 8 + 2 * (lane & 3);
 #pragma unroll
         for (int e = 0; e < 2; ++e)
-          if (col + e < p.ncols) atomicAdd(p.DW + (long long)ko * p.ncols + col + e, acc[mt][nt][half * 2 + e]);
+          if (col + e < p.ncols && (p.centre_from == 0 || ko < p.centre_from || (col + e) / p.C == 4))
+            atomicAdd(p.DW + (long long)ko * p.ncols + col + e, acc[mt][nt][half * 2 + e]);
       }
     }
 }
@@ -557,6 +559,7 @@ int conv_wgrad(const SgbConvDesc& d, const sgb_bf16* x, const sgb_bf16* dy, floa
   p.x_pitch = d.x_pitch; p.x_off = d.x_off; p.y_pitch = d.y_pitch; p.y_off = d.y_off;
   p.npix = d.N * d.P * d.Q;
   p.ncols = d.R * d.S * d.C;
+  p.centre_from = d.centre_from;  // check_desc: only with a 3x3 filter, whose centre tap is tap 4
   int bmw = d.K <= 32 ? 32 : (d.K <= 64 ? 64 : 128);
   if (d.K > 64 && d.K <= 96) bmw = 32;  // 3 x 32 wastes nothing
   int mt = ceil_div(d.K, bmw), nt = ceil_div(p.ncols, 64);

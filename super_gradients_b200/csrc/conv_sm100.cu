@@ -480,6 +480,7 @@ struct WParams {
   int pix_per_cta;     // multiple of WPIX
   int stages;
   int cpad;            // channel count of the KRSC output rows (x channels incl. padding)
+  int centre_from;     // 0, or the first row whose off-centre entries are not written (a row block may reach past it)
   float* dw;
   int halo_tw, halo_thw, tiles, tiles_per_cta;  // wgrad3x3_halo_kernel: 8 x 8 tiles per image row band / per image / in all
 };
@@ -487,6 +488,11 @@ constexpr int WPIX = 64;  // pixels (GEMM K) per pipeline stage
 
 __host__ __device__ __forceinline__ int wgrad_row_blocks(const WParams& p, int tap) {
   return p.R * p.S == 9 && tap != CENTRE_TAP ? p.rb_off : p.rb_all;
+}
+
+// dW rows tap `tap` writes: all K, or below centre_from off the centre of a folded filter
+__device__ __forceinline__ int wgrad_rows(const WParams& p, int tap) {
+  return p.centre_from > 0 && p.R * p.S == 9 && tap != CENTRE_TAP ? p.centre_from : p.K;
 }
 
 template <int NB>
@@ -595,7 +601,7 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_cons
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int ko = row0 + (shared_rows ? 0 : wg * 64) + wq * 16 + (lane >> 2) + 8 * h;
-        if (ko < p.K) {
+        if (ko < wgrad_rows(p, tap)) {
           float* drow = p.dw + (long long)ko * row_len + tap * p.cpad + ctile * NB + 2 * (lane & 3);
 #pragma unroll
           for (int j = 0; j < NB / 8; ++j)
@@ -682,12 +688,14 @@ __device__ __forceinline__ void wgrad_halo_consume(const WParams& p, uint32_t ri
       if (ko < p.K) {
         float* drow = p.dw + (long long)ko * row_len + tap0 * p.cpad + ctile * NB + 2 * (lane & 3);
 #pragma unroll
-        for (int t = 0; t < NT; ++t)
+        for (int t = 0; t < NT; ++t) {
+          if (ko >= wgrad_rows(p, tap0 + t)) continue;
 #pragma unroll
           for (int j = 0; j < NB / 8; ++j)
             asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(drow + t * p.cpad + 8 * j), "f"(acc[t][4 * j + 2 * h]),
                          "f"(acc[t][4 * j + 2 * h + 1])
                          : "memory");
+        }
       }
     }
   }
@@ -1172,6 +1180,7 @@ int wgrad_launch(const WgradProblem& q, cudaStream_t st) {
   // the 64-row blocks that cover K (off the centre of a folded filter: centre_from), paired, with a shared odd last one
   p.rb_all = (q.K + 63) / 64;
   p.rb_off = q.centre_from > 0 ? (q.centre_from + 63) / 64 : p.rb_all;
+  p.centre_from = q.centre_from;
   p.items = 0;
   for (int t = 0; t < q.R * q.S; ++t) p.items += (wgrad_row_blocks(p, t) + 1) / 2;
   p.cpad = q.C;

@@ -887,11 +887,12 @@ def record_bn_qarep():
             setattr(K, n, fn)
 
 
-def _run_steps(m, loss, opt_kw, x, t, lr, steps=1):
+def _run_steps(m, loss, opt_kw, x, t, lr, steps=1, recorder=record_bn_qarep):
+    """`steps` eager TrainSteps (SGD) of m, with the calls `recorder()` (a context manager yielding its list of calls) keeps."""
     from super_gradients_b200.training.sg_trainer import TrainStep
 
     st = TrainStep(m, loss, "SGD", opt_kw, zero_wd_on_bias_and_bn=True)
-    with record_bn_qarep() as calls:
+    with recorder() as calls:
         for _ in range(steps):
             st.set_hyper_params(lr)
             st.run(x, t)
@@ -899,7 +900,7 @@ def _run_steps(m, loss, opt_kw, x, t, lr, steps=1):
     return calls
 
 
-def yolo_nas_s_step_record(batch=2, img=640, seed=0):
+def yolo_nas_s_step_record(batch=2, img=640, seed=0, recorder=record_bn_qarep):
     """One eager TrainStep of YOLO-NAS-S (80 classes) on random images with detection targets (plumbing_cases' driver), recorded."""
     from super_gradients_b200.training import models
     from super_gradients_b200.training.losses import PPYoloELoss, pad_targets_host
@@ -915,10 +916,10 @@ def yolo_nas_s_step_record(batch=2, img=640, seed=0):
             w, h = (torch.rand(2, generator=g) * 150 + 30).tolist()
             rows.append([b, int(torch.randint(0, 80, (1,), generator=g)), cx, cy, w, h])
     t = tuple(a.cuda() for a in pad_targets_host(torch.tensor(rows), batch, 16))
-    return _run_steps(m, PPYoloELoss(num_classes=80, use_static_assigner=False), {"weight_decay": 1e-5, "momentum": 0.9}, x, t, 1e-3)
+    return _run_steps(m, PPYoloELoss(num_classes=80, use_static_assigner=False), {"weight_decay": 1e-5, "momentum": 0.9}, x, t, 1e-3, recorder=recorder)
 
 
-def resnet_step_record(name="resnet50", batch=2, img=224, seed=0, droppath_prob=0.0):
+def resnet_step_record(name="resnet50", batch=2, img=224, seed=0, droppath_prob=0.0, recorder=record_bn_qarep):
     """One eager TrainStep of a ResNet (1000 classes), optionally with drop-path in every block, recorded."""
     from super_gradients_b200.training import models
     from super_gradients_b200.training.losses import CrossEntropyLoss
@@ -927,7 +928,7 @@ def resnet_step_record(name="resnet50", batch=2, img=224, seed=0, droppath_prob=
     m = models.get(name, num_classes=1000, arch_params={"droppath_prob": droppath_prob} if droppath_prob else None).cuda().train()
     g = torch.Generator().manual_seed(seed + 1)
     x, y = torch.randn(batch, 3, img, img, generator=g).cuda(), torch.randint(0, 1000, (batch,), generator=g).cuda()
-    return _run_steps(m, CrossEntropyLoss(), {"weight_decay": 1e-4, "momentum": 0.9}, x, y, 0.1)
+    return _run_steps(m, CrossEntropyLoss(), {"weight_decay": 1e-4, "momentum": 0.9}, x, y, 0.1, recorder=recorder)
 
 
 def qarep_alpha_step_record(batch=2, seed=0):

@@ -42,146 +42,6 @@ def rel_err(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp_min(1e-12))
 
 
-CONV_CASES = [
-    # n, c, h, w, k, r, stride, pad
-    (2, 16, 12, 12, 24, 3, 1, 1),
-    (2, 16, 13, 11, 24, 3, 2, 1),
-    (3, 32, 20, 20, 32, 3, 1, 1),
-    (2, 48, 10, 10, 96, 3, 2, 1),
-    (2, 64, 9, 9, 64, 1, 1, 0),
-    (2, 96, 8, 8, 192, 1, 2, 0),
-    (1, 8, 33, 33, 48, 3, 2, 1),
-    (2, 8, 30, 30, 64, 7, 2, 3),
-    (2, 128, 7, 7, 256, 3, 1, 1),
-    (4, 64, 10, 10, 68, 1, 1, 0),
-    (2, 192, 5, 5, 80, 1, 1, 0),
-    (2, 16, 6, 6, 16, 2, 2, 0),
-    # multi-tile persistent loops of the wgmma kernel (tiles > SM count)
-    (16, 32, 48, 48, 32, 3, 1, 1),
-    (8, 64, 40, 40, 64, 3, 1, 1),
-    (6, 96, 40, 40, 96, 3, 1, 1),
-    (8, 48, 40, 40, 96, 3, 2, 1),
-    (4, 192, 20, 20, 384, 3, 2, 1),
-    (2, 384, 20, 20, 768, 1, 1, 0),
-    (6, 64, 31, 29, 128, 1, 1, 0),
-    (4, 16, 16, 16, 16, 3, 1, 1),
-    (4, 32, 16, 16, 32, 3, 1, 1),
-    (4, 16, 16, 16, 16, 1, 1, 0),
-    (2, 64, 24, 24, 64, 3, 1, 1),
-    (2, 16, 32, 32, 48, 3, 2, 1),
-    (3, 32, 24, 24, 64, 3, 2, 1),
-    # 3x3 stride 1: channel counts of 16 / 32 / 64-channel boxes, ragged image edges, tiles > CTAs
-    (2, 48, 20, 20, 48, 3, 1, 1),
-    (2, 192, 20, 20, 192, 3, 1, 1),
-    (3, 32, 13, 37, 32, 3, 1, 1),
-    (2, 128, 19, 16, 128, 3, 1, 1),
-    (40, 32, 64, 64, 32, 3, 1, 1),
-    # im2col kernels with channel counts that are not multiples of 64: 64-channel boxes with TMA-zero-filled tails (fprop / dgrad),
-    # weight-gradient MMAs whose N spans several boxes (48 = 3 x 16, 96 = 3 x 32, 192 = 3 x 64, 288 = 9 x 32)
-    (4, 96, 20, 20, 192, 3, 2, 1),
-    (4, 96, 20, 20, 96, 3, 2, 1),
-    (4, 96, 20, 20, 64, 1, 1, 0),
-    (4, 192, 20, 20, 64, 1, 1, 0),
-    (2, 288, 20, 20, 96, 1, 1, 0),
-    (2, 48, 40, 40, 96, 1, 2, 0),
-    (2, 80, 12, 12, 80, 1, 1, 0),
-    # im2col kernel with more tiles than co-resident CTAs (persistent loops): even / odd tile counts, several N tiles,
-    # the stride-2 dgrad parity classes
-    (9, 48, 192, 192, 96, 3, 2, 1),
-    (8, 96, 200, 200, 64, 1, 2, 0),
-    (9, 64, 96, 96, 80, 1, 1, 0),
-    # 2 x 2 / stride 2 (ConvTranspose backward) re-described as a 2-tap valid convolution over [N * H/2][2][W/2][2C] on the wgmma kernels
-    (4, 96, 40, 40, 96, 2, 2, 0),
-    (2, 192, 20, 20, 192, 2, 2, 0),
-    (3, 32, 18, 22, 48, 2, 2, 0),
-]
-
-
-@pytest.mark.parametrize("case", CONV_CASES)
-def test_conv_fprop_dgrad_wgrad(case):
-    k = K()
-    n, c, h, w, kk, r, stride, pad = case
-    g = torch.Generator().manual_seed(hash(case) % 1000)
-    x = torch.randn(n, c, h, w, generator=g).bfloat16().float()
-    wt = (torch.randn(kk, c, r, r, generator=g) * 0.2).bfloat16().float()
-    ref = F.conv2d(x, wt, stride=stride, padding=pad)
-    xg = to_nhwc_bf16(x)
-    krsc, crsk = k.weight_prepare(wt.to(DEV))
-    # fp32 output: accumulator parity
-    y32 = k.conv_fprop(xg, krsc, kk, r, r, stride, pad, out_f32=True)
-    assert rel_err(y32.cpu(), ref) < 1e-3
-    assert rel_err(y32.cpu(), ref) < 5e-5
-    # bf16 output: correctly rounded (<= 1 bf16 ulp of the oracle)
-    stats = k.new_stats(kk, DEV)
-    from super_gradients_b200 import lib
-
-    n_sm100 = lib.load().sgb_sm100_launches()
-    y = k.conv_fprop(xg, krsc, kk, r, r, stride, pad, stats=stats)
-    wgmma_shape = c % 16 == 0 and kk % 8 == 0 and ((r in (1, 3) and pad == r // 2) or (r == 2 and stride == 2 and pad == 0 and h % 2 == 0 and w % 2 == 0))
-    if wgmma_shape:
-        assert lib.load().sgb_sm100_launches() == n_sm100 + 1, "the wgmma/TMA kernel should have served this shape"
-    yc = y.float().cpu()
-    # absolute floor: fp32 accumulation noise of a c*r*r-term sum whose result cancels to ~0
-    assert ((yc - ref).abs() <= ref.abs() * 2**-7 + 2e-7 * c * r * r).all()
-    if wgmma_shape:
-        # the statistics epilogue leaves the stored tensor unchanged
-        y_plain = k.conv_fprop(xg, krsc, kk, r, r, stride, pad)
-        assert torch.equal(y_plain, y)
-    # fused per-channel statistics of the stored tensor
-    st = stats.sum(0).cpu()
-    torch.testing.assert_close(st[0], yc.double().sum((0, 2, 3)), rtol=1e-6, atol=1e-4)
-    torch.testing.assert_close(st[1], (yc.double() ** 2).sum((0, 2, 3)), rtol=1e-6, atol=1e-4)
-    # dgrad / wgrad
-    dy = torch.randn(ref.shape, generator=g).bfloat16().float()
-    dyg = to_nhwc_bf16(dy)
-    ref_dx = torch.nn.grad.conv2d_input(x.shape, wt, dy, stride=stride, padding=pad)
-    ref_dw = torch.nn.grad.conv2d_weight(x, wt.shape, dy, stride=stride, padding=pad)
-    dx = k.conv_dgrad(dyg, crsk, x.shape, r, r, stride, pad)
-    dxc = dx.float().cpu()
-    assert ((dxc - ref_dx).abs() <= ref_dx.abs() * 2**-7 + 1e-3 * ref_dx.abs().max()).all()
-    # accumulate mode
-    dx2 = k.conv_dgrad(dyg, crsk, x.shape, r, r, stride, pad, out=dx.clone(), accumulate=True)
-    assert rel_err(dx2.float().cpu(), 2 * ref_dx) < 2e-2
-    dw = k.wgrad_to_oihw(k.conv_wgrad(xg, dyg, r, r, stride, pad), c).cpu()
-    assert rel_err(dw, ref_dw) < 1e-3
-
-
-def test_conv_channel_slices_and_epilogue():
-    """Operands that are channel slices of wider NHWC buffers; bias / scale / residual / ReLU epilogue."""
-    k = K()
-    g = torch.Generator().manual_seed(11)
-    n, c, h, w, kk = 2, 32, 9, 9, 40
-    x = torch.randn(n, c, h, w, generator=g).bfloat16().float()
-    wt = (torch.randn(kk, c, 3, 3, generator=g) * 0.1).bfloat16().float()
-    scale = torch.rand(kk, generator=g) + 0.5
-    shift = torch.randn(kk, generator=g)
-    res = torch.randn(n, kk, h, w, generator=g).bfloat16().float()
-    ref = F.relu(F.conv2d(x, wt, padding=1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1) + res)
-    xg = to_nhwc_bf16(x, pitch=64, off=16)
-    out_buf = torch.zeros(n, 96, h, w, dtype=torch.bfloat16, device=DEV).contiguous(memory_format=torch.channels_last)
-    out = out_buf[:, 48:88]
-    resg = to_nhwc_bf16(res, pitch=96, off=0)
-    krsc, _ = k.weight_prepare(wt.to(DEV))
-    k.conv_fprop(xg, krsc, kk, 3, 3, 1, 1, scale=scale.to(DEV), shift=shift.to(DEV), residual=resg, act="relu", out=out)
-    yc = out.float().cpu()
-    assert ((yc - ref).abs() <= ref.abs() * 2**-7 + 2e-2).all()
-    assert float(out_buf[:, :48].abs().max()) == 0 and float(out_buf[:, 88:].abs().max()) == 0  # neighbours untouched
-
-
-def test_convt2x2():
-    k = K()
-    g = torch.Generator().manual_seed(12)
-    n, cs, p, q, cu = 2, 32, 5, 6, 24
-    x = torch.randn(n, cs, p, q, generator=g).bfloat16().float()
-    wt = (torch.randn(cs, cu, 2, 2, generator=g) * 0.2).bfloat16().float()  # ConvTranspose2d weight [in, out, kh, kw]
-    b = torch.randn(cu, generator=g)
-    ref = F.conv_transpose2d(x, wt, b, stride=2)
-    w_up = wt.permute(2, 3, 1, 0).reshape(4 * cu, cs).contiguous().to(DEV).bfloat16()  # [(dh,dw,co)][ci]
-    y = k.convt2x2_fprop(to_nhwc_bf16(x), w_up, b.to(DEV), cu)
-    yc = y.float().cpu()
-    assert ((yc - ref).abs() <= ref.abs() * 2**-7 + 1e-2).all()
-
-
 def test_layout_roundtrip():
     k = K()
     x = torch.randn(3, 3, 17, 19)

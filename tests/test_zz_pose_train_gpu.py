@@ -195,17 +195,18 @@ def test_predict_on_raw_images_gpu(golden):
 
 
 # 1x1 stride 1 on the channel counts of the halo variants (served by the im2col wgmma kernel): ragged edges, statistics with
-# K == C and K != C, tiles > CTAs.  Kept here (not in
-# test_kernels_gpu.CONV_CASES) until their first hardware run.
+# K == C and K != C, tiles > CTAs; each shape in the five modes of conv_cases.shape_modes, bit-exact with integer operands.
 ONE_BY_ONE_CASES = [(8, 32, 40, 40, 32, 1, 1, 0), (4, 96, 40, 40, 96, 1, 1, 0), (3, 48, 13, 37, 48, 1, 1, 0), (2, 128, 19, 16, 64, 1, 1, 0), (40, 32, 64, 64, 32, 1, 1, 0),
                     (4, 96, 40, 40, 32, 1, 1, 0), (4, 64, 24, 24, 96, 1, 1, 0), (2, 192, 20, 20, 64, 1, 1, 0)]  # fmt: skip
 
 
 @pytest.mark.parametrize("case", ONE_BY_ONE_CASES)
 def test_conv_1x1_fprop_dgrad_wgrad(case):
-    from test_kernels_gpu import test_conv_fprop_dgrad_wgrad as conv_case
+    from conv_cases import shape_modes
+    from test_conv_fp64_gpu import _check
 
-    conv_case(case)
+    for c in shape_modes(*case):
+        _check(c, real=False)
 
 
 @pytest.mark.parametrize("cin,cout,use_alpha", [(32, 32, True), (48, 48, False), (64, 32, True), (96, 96, True)])
